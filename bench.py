@@ -1,8 +1,9 @@
-"""Benchmark of the DBNet -> PARSeq OCR hot path (BASELINE.json metric) on N B200s of one node.
+"""Benchmark of the DBNet -> PARSeq OCR hot path (BASELINE.json metric) on N H100s of one node.
 
     python bench.py --gpus 1 --steps K --warmup W               # this repo's CUDA path
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
     python bench.py --impl reference ...                        # the reference's CPU implementation (oracle restatement)
+    python bench.py --gpus 1 --steps K --dump-outputs DIR       # also write the last timed step's outputs to DIR/*.npy
 
 One step = the hot path over one batch of synthetic 1200x1600 (H x W) pages per GPU (~200 text lines each):
 DBNet (`dbnetv2_1`) on every page + PARSeq (`parseq-large-v4_1`, dynamic_width + batch_bucketing) on every crop.
@@ -42,16 +43,17 @@ REC_MODEL = "parseq-large-v4_1"
 
 
 def peaks():
+    # fallback: NVIDIA's H100 SXM data sheet (dense fp16 / bf16, HBM3; a 700 W card) - a ceiling, not a reached rate
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return {"bf16_tflops": d.get("bf16_tflops", 1590.0), "bf16_tflops_sustained": d.get("bf16_tflops_sustained", 1400.0),
-                "hbm_gbs": d.get("hbm_gbs", 6650.0), "source": "measured"}
-    return {"bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "hbm_gbs": 6650.0, "source": "fallback"}
+        return {"bf16_tflops": d.get("bf16_tflops", 989.0), "bf16_tflops_sustained": d.get("bf16_tflops_sustained", 989.0),
+                "hbm_gbs": d.get("hbm_gbs", 3350.0), "source": "measured"}
+    return {"bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "hbm_gbs": 3350.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index=0):
         self.index = index
@@ -107,7 +109,7 @@ def _pick_cpu_threads(det_sd, x):
         return _CPU_THREADS
     from oracle import dbnet as odb
     ncpu = os.cpu_count() or 1
-    # (more intra-op threads than 64 collapse on this workload: 128 threads took 26 s for the probe in round 2)
+    # (more intra-op threads than 64 collapse on this workload)
     cands = sorted({t for t in (8, 16, 32, 64) if t <= ncpu} | {min(ncpu, 8)})
     sweep = {}
     xs = x[:, :, :384, :512].contiguous()      # a quarter-size map is enough to rank the settings
@@ -171,20 +173,14 @@ def run_reference(args):
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
+    # a step = one full page through the CPU path (tens of seconds); exactly --warmup untimed and --steps timed pages
+    warm = args.warmup
+    for _ in range(warm):
+        cpu_page_rate()
     vals, detail = [], None
-    t_start = time.perf_counter()
-    warm, steps, i = min(args.warmup, 1), args.steps, 0
-    while i < warm + steps:
-        r = cpu_page_rate()
-        if i >= warm:
-            vals.append(r["pages_per_s"])
-            detail = r
-        i += 1
-        per = (time.perf_counter() - t_start) / i
-        if per * (warm + steps) > 200.0:       # keep the whole run within a few minutes (a step = one full page)
-            steps = max(1, int(200.0 / per) - warm)
-    if not vals:
-        vals, detail = [r["pages_per_s"]], r
+    for _ in range(args.steps):
+        detail = cpu_page_rate()
+        vals.append(detail["pages_per_s"])
     v = float(np.mean(vals))
     line = {
         "impl": "reference", "metric": METRIC, "value": v, "unit": "pages/s", "n_gpus": args.gpus, "steps": len(vals),
@@ -227,7 +223,7 @@ def _time_ms(fn, steps, warmup):
 
 
 def config2_line(det, L, pk, steps=20, warmup=5):
-    """BASELINE config 2: TextDetector DBNet, ONE synthetic 1600x1200 page, 1 B200 - latency of the device path (page
+    """BASELINE config 2: TextDetector DBNet, ONE synthetic 1600x1200 page, 1 GPU - latency of the device path (page
     resident in HBM -> probability map in HBM) and its tensor roofline."""
     from yomitoku_b200 import _lib
     from yomitoku_b200.synth import synthetic_page
@@ -244,7 +240,7 @@ def config2_line(det, L, pk, steps=20, warmup=5):
     return {"metric": "pages/sec (DBNet TextDetector, one 1600x1200 page, batch 1)", "value": 1e3 / ms, "unit": "pages/s",
             "ms_per_step": ms, "steps": steps, "warmup": warmup, "dtype": "f16", "higher_is_better": True,
             "config": {"workload": "BASELINE config 2: TextDetector DBNet(dbnetv2_1), single synthetic 1200x1600 page, "
-                                   "1 B200, page and probability map resident in HBM, batch 1 (latency)"},
+                                   "1 GPU, page and probability map resident in HBM, batch 1 (latency)"},
             "roofline": {"bound": "tensor", "achieved": flops / 1e12 / (ms / 1e3), "peak": pk["bf16_tflops"],
                          "unit": "TFLOP/s", "frac": flops / 1e12 / (ms / 1e3) / pk["bf16_tflops"],
                          "gflop_per_page": flops / 1e9, "peak_source": pk["source"] + " bf16_tflops (burst: short run)",
@@ -271,7 +267,7 @@ def config5_layout_line(L, pk, batch=8, steps=10, warmup=3):
             "value": batch / (ms / 1e3), "unit": "images/s", "ms_per_step": ms, "steps": steps, "warmup": warmup,
             "dtype": "f16", "higher_is_better": True,
             "config": {"workload": "BASELINE config 5's extra model: RT-DETRv2 (PResNet-50d + HybridEncoder + 6-layer "
-                                   "deformable decoder, 300 queries), %d synthetic 640x640 inputs, 1 B200, inputs and outputs "
+                                   "deformable decoder, 300 queries), %d synthetic 640x640 inputs, 1 GPU, inputs and outputs "
                                    "resident in HBM, random weights" % batch},
             "roofline": {"bound": "tensor", "achieved": flops / 1e12 / (ms / 1e3), "peak": pk["bf16_tflops"],
                          "unit": "TFLOP/s", "frac": flops / 1e12 / (ms / 1e3) / pk["bf16_tflops"],
@@ -280,7 +276,7 @@ def config5_layout_line(L, pk, batch=8, steps=10, warmup=3):
 
 
 def config3_line(rec, L, pk, n_crops=512, steps=5, warmup=3):
-    """BASELINE config 3: TextRecognizer PARSeq (full), 512 crops, dynamic_width + batch_bucketing, 1 B200: crops/s with
+    """BASELINE config 3: TextRecognizer PARSeq (full), 512 crops, dynamic_width + batch_bucketing, 1 GPU: crops/s with
     the crops resident in HBM (reference grouping: sorted chunks of 128, each padded to its own maximum)."""
     from yomitoku_b200.data import ParseqDataset
     from yomitoku_b200.synth import synthetic_page
@@ -311,12 +307,28 @@ def config3_line(rec, L, pk, n_crops=512, steps=5, warmup=3):
             "value": n_crops / (ms / 1e3), "unit": "crops/s", "ms_per_step": ms, "steps": steps, "warmup": warmup,
             "dtype": "f16", "higher_is_better": True,
             "config": {"workload": "BASELINE config 3: TextRecognizer PARSeq(%s), 512 synthetic crops, dynamic_width + "
-                                   "batch_bucketing, 1 B200, crops resident in HBM; %d mini-batches, %d encoder tokens, "
+                                   "batch_bucketing, 1 GPU, crops resident in HBM; %d mini-batches, %d encoder tokens, "
                                    "101 AR steps (random weights)" % (REC_MODEL, len(plan), n_tok),
                        "recognizer_phase_ms": rec.model.last_phase_ms()},
             "roofline": {"bound": "tensor", "achieved": flops / 1e12 / (ms / 1e3), "peak": pk["bf16_tflops"],
                          "unit": "TFLOP/s", "frac": flops / 1e12 / (ms / 1e3) / pk["bf16_tflops"],
                          "gflop_per_step": flops / 1e9, "peak_source": pk["source"] + " bf16_tflops (burst: short run)"}}
+
+
+def dump_outputs(d, prob_dev, post_meta, rec_out, n_prob=1 << 20):
+    """The arrays a caller of the timed path receives from its last step, as float32 / float64 .npy files (< 64 MB):
+    a fixed, seeded sample of the detector's probability maps (all of them would be 120 MB) with its flat indices, the per-page counts of the
+    device post-processing front, and the recognizer's token ids and probabilities of every crop in group order."""
+    os.makedirs(d, exist_ok=True)
+    prob = prob_dev.float().cpu().numpy().reshape(-1)
+    idx = np.sort(np.random.default_rng(0).choice(prob.size, size=min(n_prob, prob.size), replace=False))
+    np.save(os.path.join(d, "det_prob_sample.npy"), prob[idx].astype(np.float32))
+    np.save(os.path.join(d, "det_prob_sample_index.npy"), idx.astype(np.float64))
+    if post_meta is not None:
+        np.save(os.path.join(d, "det_post_meta.npy"), post_meta.cpu().numpy().astype(np.float64))
+    np.save(os.path.join(d, "rec_ids.npy"), np.concatenate([g[0] for g in rec_out]).astype(np.float64))
+    np.save(os.path.join(d, "rec_probs.npy"), np.concatenate([g[1] for g in rec_out]).astype(np.float32))
+    np.save(os.path.join(d, "rec_group_len.npy"), np.asarray([g[2] for g in rec_out], np.float64))
 
 
 # ------------------------------------------------------------------------------------------------ GPU arm
@@ -334,9 +346,12 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip other_configs (config 2, config 3, EOS run)")
-    ap.add_argument("--no-window", action="store_true", help="skip the instrumented per-launch GEMM timing step "
-                                                               "(for runs under ncu)")
+    ap.add_argument("--no-window", action="store_true", help="skip the instrumented per-launch GEMM timing step")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     if args.impl == "reference":
         run_reference(args)
         return
@@ -454,7 +469,7 @@ def main():
             ev[0].record()
             det_step()
             ev[1].record()
-            rec_step()
+            rec_out = rec_step()
             ev[2].record()
             torch.cuda.synchronize()
             det_ms += ev[0].elapsed_time(ev[1])
@@ -464,6 +479,8 @@ def main():
         total_ms = t_all0.elapsed_time(t_all1)
     launches = L.ytk_launch_count() - launches0
     x_value = {k: par.STATS[k] - x0[k] for k in x0}
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, prob_dev, post_meta if det.device_post else None, rec_out)
     ar_steps = int(L.ytk_parseq_last_steps(rec.model._ensure()))
     phase_value = rec.model.last_phase_ms()     # CUDA-event phase times of the last recognizer call of the timed region
     rec_flops_local = rec.model.last_flops()
@@ -553,14 +570,6 @@ def main():
         cpu = {"value": r["pages_per_s"], "unit": "pages/s", "cores": r["cores"], "kind": "port",
                "sample": _cpu_sample_text(r)}
     if rank == 0:
-        traffic, traffic_src = None, None
-        tp = os.path.join(ROOT, "profiles", "r02_bench_step_traffic.json")
-        if os.path.exists(tp):
-            try:
-                tj = json.load(open(tp))
-                traffic, traffic_src = tj["gemm_tc_kernel_dram_bytes_per_step"], tj.get("source")
-            except Exception:
-                pass
         g_ms = g_det["ms"] + g_rec["ms"]
         g_tf = g_det["tflop"] + g_rec["tflop"]
         line = {
@@ -574,7 +583,7 @@ def main():
                                       "value and e2e" % P,
                        "skew": ("even ranks 280 text lines/page, odd ranks 120 (mean 200)" if skew else
                                 "none: 200 text lines on every page"),
-                       "l2": "working set (%.1f GB activations per step) >> 126 MB L2; no explicit flush" %
+                       "l2": "working set (%.1f GB activations per step) >> 50 MB L2; no explicit flush" %
                              (P * 1.2 + 4.0),
                        "operands": "fp16 operands (11-bit significand), fp32 accumulation / residual stream / softmax",
                        "ar_steps": ar_steps,
@@ -595,8 +604,7 @@ def main():
             "roofline": {"bound": "tensor",
                          "achieved": g_tf / (g_ms / 1e3), "peak": pk["bf16_tflops_sustained"], "unit": "TFLOP/s",
                          "frac": g_tf / (g_ms / 1e3) / pk["bf16_tflops_sustained"],
-                         "traffic": traffic, "traffic_source": traffic_src,
-                         "kernel": "gemm_tc_kernel (tcgen05 implicit GEMM): every launch of one step (DBNet convs + "
+                         "kernel": "gemm_tc_kernel (wgmma implicit GEMM): every launch of one step (DBNet convs + "
                                    "PARSeq linears), algorithmic FLOPs (2*M*N*K per launch) over the sum of the launch "
                                    "durations; CUDA events around every launch on the launching stream, one "
                                    "instrumented step right after the timed region",

@@ -37,7 +37,7 @@ void ytk_gemm_profile_begin(void);
 int ytk_gemm_profile_end(double* flops, double* ms, long long* launches);
 
 /* ---- op level (kernel parity tests; replaces the cuDNN/cuBLAS call sites listed in SURVEY.md section 2.3) ----
- * Convolution as tcgen05 implicit GEMM.  in: NHWC fp16 [N,H,W,in_ld] (first Cin channels used), w: fp16
+ * Convolution as wgmma implicit GEMM.  in: NHWC fp16 [N,H,W,in_ld] (first Cin channels used), w: fp16
  * [Cout][kh][kw][Cin], bias fp32 [Cout] or NULL, resid: [N,Ho,Wo,ldr] fp16/fp32 or NULL, out: [N,Ho,Wo,ldc]
  * fp16/fp32.  Replaces torch.nn.Conv2d + BatchNorm2d(eval, folded) + ReLU (+ residual add) of
  * torchvision ResNet-50 bottlenecks (reference models/dbnet_plus.py:30-38) and the decoder convs (:56-116).
@@ -67,8 +67,8 @@ typedef struct ytk_attn_seq {
 /* softmax(Q K^T / sqrt(head_dim)) V per (sequence, head) over packed ragged sequences; Q [q_rows, ldq], K / V
  * [kv_rows, ldkv], O [*, ldo] fp16 on the device, head h = columns [h*head_dim, (h+1)*head_dim); seqs_dev: device array.
  * masked != 0: key j visible to query i iff (i < 2 || j <= i) && j < kpad (PARSeq refinement mask, reference
- * models/parseq.py:267-297).  impl: 0 default (tcgen05 kernel), 1 legacy mma.sync kernel, 2/3 tcgen05 kernel with the
- * V-descriptor convention forced.  Replaces timm Attention's F.scaled_dot_product_attention (reference
+ * models/parseq.py:267-297).  impl: 0 default (wgmma kernel), 1 legacy mma.sync kernel, 2 wgmma kernel.
+ * Replaces timm Attention's F.scaled_dot_product_attention (reference
  * models/layers/parseq_transformer.py:206-234) and nn.MultiheadAttention's core (parseq_transformer.py:83-92). */
 int ytk_op_attention_f16(const void* Q, long long ldq, long long q_rows, const void* K, const void* V, long long ldkv,
                          long long kv_rows, void* O, long long ldo, const ytk_attn_seq* seqs_dev, int nseq, int max_q_len,

@@ -7,8 +7,8 @@ head of an untrained net amplifies noise, trained weights are smoother):
   polygons           (a) the DEVICE'S OWN map of a detector with a trained head (tests/golden/dbnet_head_trained.npz: the
                      map holds the page's ~200 text lines) through the post-processor vs the fp32 oracle's own map
                      through the same post-processor: >= 95 % of the oracle's boxes with a score clear of box_thresh
-                     are found with IoU >= 0.9 and corners within 2 px (measured on B200: 240 of 245), >= 99 % with
-                     IoU >= 0.5 (nothing lost / merged / split), box counts within 3 % (272 vs 273);
+                     are found with IoU >= 0.9 and corners within 2 px, >= 99 % with
+                     IoU >= 0.5 (nothing lost / merged / split), box counts within 3 %;
                      (b) random head: the device's actual error field superimposed on a realistic probability map,
                      every box is found again with IoU >= 0.9 and corner coordinates within 2 px."""
 import ctypes
@@ -156,7 +156,7 @@ def test_polygons_from_the_devices_own_map(page_id):
     print("[dbnet trained head] page %d: oracle %d boxes, device %d; %d of %d clear-score boxes found (IoU >= 0.9, 2 px); "
           "all boxes: %d of %d; (IoU, max corner distance) of the others: %s"
           % (page_id, len(q_ref), len(q_dev), int((ok & clear).sum()), int(clear.sum()), int(ok.sum()), len(ok), worst))
-    # measured on B200 (call 21, page 2): 240 of 245 - where the threshold cuts a blob edge with a shallow slope, a map
+    # where the threshold cuts a blob edge with a shallow slope, a map
     # difference of 0.01-0.05 moves the edge by a pixel, which the unclip step scales up to a few pixels of the box
     assert (ok & clear).sum() >= 0.95 * clear.sum()
     assert ((m[:, 0] >= 0.5) & clear).sum() >= 0.99 * clear.sum()      # no box lost, merged or split away

@@ -1,4 +1,4 @@
-"""GPU: kernel-level parity of the tcgen05 implicit-GEMM convolution / linear op through the C ABI against torch fp32
+"""GPU: kernel-level parity of the wgmma implicit-GEMM convolution / linear op through the C ABI against torch fp32
 on the same bf16-rounded operands (tolerance: bf16 output rounding, 2^-8 relative)."""
 import pytest
 import torch
@@ -27,8 +27,8 @@ def _check(got, ref, tol=6e-3):
     (128, 64, 64, 0, None, True), (300, 128, 200, 0, None, False), (1000, 768, 2304, 2, None, False),
     (517, 768, 7119, 0, None, True), (640, 3072, 768, 0, "f32", True), (33, 192, 576, 1, "f16", False),
     (257, 192, 200, 3, "f32", False), (129, 64, 100, 0, "f16", True),
-    # >= 4 tiles per SM: CTA-pair kernel (tcgen05.mma.cta_group::2, half weight tile per SM); 75 / 149 M tiles are odd,
-    # so the last pair has a ghost CTA; N = 2304 has 9 full N tiles, N = 7119 a ragged last one, K = 3072 wraps the stage ring
+    # >= 4 tiles per SM (the persistent CTAs loop over many tiles); 75 / 149 M tiles are odd; N = 2304 has 9 full N
+    # tiles, N = 7119 a ragged last one, K = 3072 wraps the stage ring
     (128 * 74 + 5, 768, 2304, 2, None, False), (128 * 148 + 77, 192, 768, 0, "f32", True),
     (128 * 21 + 1, 768, 7119, 0, None, True), (128 * 200, 3072, 768, 0, "f32", True),
     # TMA epilogue (residual boxes by TMA load, results by TMA store): ragged N with a 16-bit residual, one N tile of 64,
@@ -65,8 +65,7 @@ def test_linear(M, K, N, act, resid, f32):
     (1, 37, 50, 128, 128, 3, 1, 2, 2, 1, True), (1, 38, 52, 64, 128, 3, 2, 1, 1, 1, False),
     (1, 37, 51, 64, 128, 3, 2, 1, 1, 1, False), (2, 38, 52, 256, 512, 1, 2, 0, 1, 0, False),
     (1, 74, 100, 512, 512, 3, 1, 2, 2, 1, True),
-    # big maps (>= 4 tiles per SM, odd tile counts): layer-1-like 3x3 and a residual 1x1 on a 296x400 map; these take
-    # the CTA-pair kernel as well when YTK_PAIR_CONV=1 is set (off by default: convs lose to the pair's lock step)
+    # big maps (>= 4 tiles per SM, odd tile counts): layer-1-like 3x3 and a residual 1x1 on a 296x400 map
     (1, 296, 400, 64, 64, 3, 1, 1, 1, 1, False), (1, 296, 400, 64, 256, 1, 1, 0, 1, 1, True),
     (3, 148, 200, 128, 128, 3, 2, 1, 1, 1, False)])
 def test_conv(N, H, W, Cin, Cout, k, s, p, d, act, resid):
@@ -216,18 +215,18 @@ def _attn_case(hd, heads, lens, masked, impl, seed=0, q_shared=None, kpads=None,
     return worst
 
 
-@pytest.mark.parametrize("impl", [4, 2])     # 4: P tile in tensor memory (default), 2: P staged in shared memory
+@pytest.mark.parametrize("impl", [1, 2])     # 1: mma.sync kernel, 2: wgmma kernel (default)
 @pytest.mark.parametrize("hd,heads,lens", [(96, 8, [132, 92, 48, 200, 400, 129, 128, 4]), (32, 6, [800, 320, 64, 8, 72]),
                                            (48, 8, [100, 260]), (64, 8, [160, 96, 31])])
 def test_attention_tc_vs_torch(hd, heads, lens, impl):
-    """tcgen05 attention kernel (attn_tc.cu) vs fp32 softmax attention on the same fp16 operands: the only rounding the
+    """Both attention kernels (parseq_ops.cu mma.sync, attn_tc.cu wgmma) vs fp32 softmax attention on the same fp16 operands: the only rounding the
     kernel adds is P and O in fp16 (2^-11 relative)."""
     d = _attn_case(hd, heads, lens, False, impl)
     print("[attn] impl %d hd %d max|d| %.5f" % (impl, hd, d))
     assert d < 4e-3, d
 
 
-@pytest.mark.parametrize("impl", [4, 2])
+@pytest.mark.parametrize("impl", [1, 2])
 def test_attention_tc_masked_refinement_shape(impl):
     d = _attn_case(96, 8, [101, 40, 7, 1, 64, 65], True, impl, q_shared=101, kpads=[101, 33, 7, 1, 20, 65])
     print("[attn] impl %d masked max|d| %.5f" % (impl, d))
@@ -238,7 +237,7 @@ def test_attention_tc_many_sequences_long_rescale():
     """Many pairs per worker (the persistent pipeline wraps its barriers many times) and scores with a large spread (the
     lazy rescale of the running max fires)."""
     import ctypes
-    d = _attn_case(96, 8, [132] * 300 + [260] * 40, False, 4, seed=3, qscale=3.0)
+    d = _attn_case(96, 8, [132] * 300 + [260] * 40, False, 2, seed=3, qscale=3.0)
     assert d < 6e-3, d
 
 

@@ -5,12 +5,11 @@ TableStructureRecognizer, LayoutAnalyzer, DocumentAnalyzer).
 
 Stated tolerances (fp16 operands with fp32 accumulation through ~75 convolutions and 7 transformer layers against fp32;
 seeded "trained-like" weights, oracle.rtdetr.make_state_dict):
-  backbone / encoder maps     relative Frobenius error < 0.5 %            (measured 0.07 - 0.16 %)
-  encoder scores              max |d| < 0.05 (scores have std ~ 2)        (measured 0.024): the top-300 query set agrees
-                              except for anchors whose oracle score lies within that distance of the cut (297 - 300 of
-                              300 agree, the others are within 0.006 of the cut)
-  queries selected by both    |d logit| < 0.1, mean < 0.02                (measured 0.031 / 0.007)
-                              |d box| < 0.003 of the image side, mean < 0.0005   (measured 0.0006 / 0.00008)
+  backbone / encoder maps     relative Frobenius error < 0.5 %
+  encoder scores              max |d| < 0.05 (scores have std ~ 2): the top-300 query set agrees
+                              except for anchors whose oracle score lies within that distance of the cut
+  queries selected by both    |d logit| < 0.1, mean < 0.02
+                              |d box| < 0.003 of the image side, mean < 0.0005
   detections                  every oracle detection with score > 0.6 is found with the same label and IoU > 0.9."""
 import os
 import sys

@@ -778,16 +778,16 @@ def test_hole_count_matches_opencv_contour_count():
 
 
 def test_gelu_coefficients_in_kernel_source():
-    """The fc1 epilogue's GELU (csrc/gemm_tc.cu: gelu_fast2) evaluated in numpy fp32 with the coefficients read from the
+    """The fc1 epilogue's GELU (csrc/gemm_tc.cu: gelu_fast) evaluated in numpy fp32 with the coefficients read from the
     source: max |error| against the fp64 erf GELU (torch.nn.GELU default of reference parseq.py's MLP) below 6e-7."""
     import re
     from scipy import special
     src = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "yomitoku_b200", "csrc",
                             "gemm_tc.cu")).read()
-    body = src[src.index("void gelu_fast2(float& x0, float& x1) {"):]
-    body = body[:body.index("upk2(r, x0, x1);")]
-    clamp = float(re.search(r"fminf\(fabsf\(x0\), ([0-9.]+)f\)", body).group(1))
-    coefs = [float(m) for m in re.findall(r"pk2\((-?[0-9.]+e[+-][0-9]+)f,", body)]        # highest power first
+    body = src[src.index("float gelu_fast(float x) {"):]
+    body = body[:body.index("return fmaf(")]
+    clamp = float(re.search(r"fminf\(fabsf\(x\), ([0-9.]+)f\)", body).group(1))
+    coefs = [float(m) for m in re.findall(r"(-?[0-9.]+e[+-][0-9]+)f", body)]        # highest power first
     assert len(coefs) == 7 and clamp == 5.7
     x = np.concatenate([np.linspace(-12, 12, 400001), [-1e4, 1e4, 0.0]]).astype(np.float32)
     t = np.minimum(np.abs(x), np.float32(clamp))

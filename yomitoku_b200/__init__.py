@@ -1,11 +1,11 @@
-"""yomitoku_b200: Blackwell-native DBNet -> PARSeq OCR hot path behind yomitoku's module API.
+"""yomitoku_b200: Hopper-native DBNet -> PARSeq OCR hot path behind yomitoku's module API.
 
     from yomitoku_b200 import OCR, TextDetector, TextRecognizer, DocumentAnalyzer
     from yomitoku_b200 import LayoutAnalyzer, LayoutParser, TableStructureRecognizer
 
 The constructors, the `configs` dict and the call contracts mirror kotaro-kinoshita/yomitoku
 (src/yomitoku/{text_detector,text_recognizer,ocr,document_analyzer,layout_parser,table_structure_recognizer,
-layout_analyzer}.py); the models (DBNet++, PARSeq, RT-DETRv2) run as hand-written sm_100a CUDA kernels behind the C ABI
+layout_analyzer}.py); the models (DBNet++, PARSeq, RT-DETRv2) run as hand-written sm_90a CUDA kernels behind the C ABI
 in include/yomitoku_b200.h (libytk_b200.so).
 """
 from .document_analyzer import DocumentAnalyzer

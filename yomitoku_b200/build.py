@@ -1,6 +1,6 @@
-"""Builds libytk_b200.so (the sm_100a CUDA kernels + C ABI) in-tree with nvcc.
+"""Builds libytk_b200.so (the sm_90a CUDA kernels + C ABI) in-tree with nvcc.
 
-nvcc cross-compiles without a GPU; the resulting .so is git-ignored but travels to the GPU box with the snapshot.
+nvcc cross-compiles without a GPU; the resulting .so and objects are git-ignored build products.
 Run as `python -m yomitoku_b200.build` or through `__graft_entry__.build()`.
 """
 import hashlib
@@ -15,7 +15,7 @@ BUILD = os.path.join(HERE, "csrc", "build")
 LIB = os.path.join(HERE, "libytk_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -61,7 +61,7 @@ def build(force=False, verbose=True):
         return LIB
     srcs = _sources()
     if verbose:
-        print("[yomitoku_b200.build] nvcc sm_100a: %s" % " ".join(srcs), flush=True)
+        print("[yomitoku_b200.build] nvcc sm_90a: %s" % " ".join(srcs), flush=True)
     with ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
         objs = list(ex.map(_compile, srcs))
     cmd = ["nvcc", "-shared", "-o", LIB] + objs + ["-lcudart"]

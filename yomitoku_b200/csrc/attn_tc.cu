@@ -1,23 +1,19 @@
-// Attention on tcgen05 tensor cores for packed ragged sequences (sm_100a): softmax(Q K^T / sqrt(hd)) V per
+// Attention on wgmma tensor cores for packed ragged sequences (sm_90a): softmax(Q K^T / sqrt(hd)) V per
 // (sequence, head) - the encoder self-attention of PARSeq's ViT (timm Attention / F.scaled_dot_product_attention, no
 // mask; reference models/layers/parseq_transformer.py:206-234) and the two attentions of the refinement pass
 // (reference models/parseq.py:264-299: cross-attention over the encoder memory, and the masked self-attention over the
 // content stream whose mask has rows 0 and 1 cleared, SURVEY.md Appendix A1).
 //
-// One persistent CTA per SM runs TWO independent pipelines ("slots"); a slot works through its own list of units
-// (sequence, head, 128-query tile) and owns a Q tile, a P tile, a 2-stage K/V ring in shared memory and 256 TMEM
-// columns (two 128x64 fp32 S buffers + one 128xhd fp32 O accumulator):
-//   warp 8+s  lane 0 : TMA producer of slot s  - Q tile once per unit, K/V tiles of 64 keys (SWIZZLE_128B boxes)
-//   warp 10   lane 0 : MMA issuer for BOTH slots (polls their barriers): S = Q K^T (tcgen05.mma, K-major operands),
-//                      O += P V (P from shared memory K-major, V as MN-major B operand - the tile is stored exactly as
-//                      TMA delivers [keys][hd] rows)
-//   warps 4s..4s+3   : softmax + epilogue of slot s, ONE QUERY ROW PER THREAD (TMEM lane = query): tcgen05.ld of the
-//                      S row, mask, running max (lazy rescale: the reference max moves only when it grows by > 2^8, so
-//                      O in TMEM is almost never touched), exp2, fp16 P row into swizzled shared memory; after the last
-//                      key tile O / l -> global.
-// While the softmax warps of one slot are busy on the CUDA cores (the exp2 throughput is what bounds short sequences)
-// the tensor core works for the other slot.  Rows of a 128-query tile beyond q_len cost tensor time only (their warps
-// skip the softmax), key tiles are trimmed to multiples of 16 keys.
+// One persistent CTA per SM works through its list of units (sequence, head, 128-query tile); it owns a Q tile and a
+// 2-stage K/V ring in shared memory:
+//   warp 8   lane 0 : TMA producer - Q tile once per unit, K/V tiles of 64 keys (SWIZZLE_128B boxes)
+//   warpgroups 0, 1 : 64 queries each.  S = Q K^T by wgmma (both operands K-major in shared memory) into registers,
+//                     mask + running max (lazy rescale: the reference max moves only when it grows by > 2^8) + exp2 in
+//                     the accumulator layout, P packed to fp16 A fragments in registers, O += P V by wgmma with A from
+//                     registers and V as MN-major B operand (the tile is stored exactly as TMA delivers [keys][hd]
+//                     rows); after the last key tile O / l -> global.
+// While one warpgroup is on the CUDA cores (softmax) the tensor core works for the other.  The P V product always
+// runs its four 16-key steps; steps past the last visible key read a zero tile instead of V.
 #include <cuda.h>
 
 #include "gemm_tc.h"
@@ -28,9 +24,10 @@ namespace ytk {
 
 namespace {
 
-constexpr int kAtQ = 128;        // queries per unit = TMEM lanes
+constexpr int kAtQ = 128;        // queries per unit (two warpgroups of 64)
 constexpr int kAtKV = 64;        // keys per tile
-constexpr int kAtThreads = 352;  // 8 softmax warps, 2 producer warps, 1 MMA warp
+constexpr int kAtThreads = 288;  // 2 consumer warpgroups, 1 producer warp
+constexpr int kAtStages = 2;
 constexpr float kRescaleThreshold = 8.f;  // log2 units: P stays <= 2^8, well inside fp16
 
 struct alignas(64) AttnMaps {
@@ -44,24 +41,23 @@ struct AttnArgs {
     float scale_log2;
     op_t* O;
     long long ldo;
-    int vswap;          // debugging aid: swap LBO / SBO in the V descriptor
 };
 
 template <int HD>
 struct AtCfg {
     static constexpr int NB = (HD + 63) / 64;                 // 64-element (128 B) column blocks per row
+    static constexpr int NO = NB * 64;                        // columns of the O accumulator
     static constexpr int kQBytes = NB * kAtQ * 128;
-    static constexpr int kPBytes = kAtQ * 128;                // 128 x 64 fp16
     static constexpr int kKBytes = NB * kAtKV * 128;          // one K (or V) tile
     static constexpr int kStageBytes = 2 * kKBytes;
-    static constexpr int kSlotBytes = kQBytes + kPBytes + 2 * kStageBytes;
-    static constexpr int kSmemBytes = 2 * kSlotBytes + 256 /*barriers*/ + 1024 /*alignment slack*/;
+    static constexpr int kZeroBytes = NB * 2048;               // 16 zero V rows per column block
+    static constexpr int kSmemBytes =
+        kQBytes + kAtStages * kStageBytes + kZeroBytes + 256 /*barriers*/ + 1024 /*alignment slack*/;
 };
 
-struct SlotBars {
-    uint64_t q_full, q_empty, kv_full[2], kv_empty[2], s_full[2], s_free[2], p_full, p_empty, o_full, o_free;
+struct Bars {
+    uint64_t q_full, q_empty, kv_full[kAtStages], kv_empty[kAtStages];
 };
-static_assert(sizeof(SlotBars) == 14 * 8, "barrier block");
 
 struct Unit {
     int q_row;    // first query row of the tile in Q
@@ -96,14 +92,12 @@ __device__ __forceinline__ Unit make_unit(const SeqDesc& sd, int head, int qt, l
     return u;
 }
 
-// The units of one (CTA, slot) worker in processing order: the worker owns the pairs p = 2 * cta + slot, + 2 * ncta,
-// ...; inside a pair the query tiles in ascending order, back to back, so that the pair's K / V tiles are still in L2
-// for the second tile.  (Dealing a pair's two query tiles to the two slots of a CTA was measured (profiles/README_r02.md): the slots drift
-// apart, K / V come from DRAM twice - 4.2 instead of 2.0 GB per layer - and the layer takes 1.78 instead of 1.13 ms.)
-// Every role of a slot walks the same sequence.
+// The units of one CTA in processing order: the CTA owns the (sequence, head) pairs p = cta, cta + ncta, ...; inside a
+// pair the query tiles in ascending order, back to back, so that the pair's K / V tiles are still in L2 for the second
+// tile.  Every role of the CTA walks the same sequence.
 template <int MASKED>
 struct UnitIter {
-    int p, qt, nqt, head, W, npairs, slot, count;
+    int p, qt, nqt, head, W, npairs;
     SeqDesc sd;
     Unit u;
     const AttnArgs* a;
@@ -113,14 +107,12 @@ struct UnitIter {
         sd = a->seqs[seq];
         nqt = (sd.q_len + kAtQ - 1) / kAtQ;
     }
-    // positions on the slot's first unit; false when it has none
-    __device__ __forceinline__ bool begin(const AttnArgs* args, int cta, int ncta, int npairs_, int slot_) {
+    // positions on the CTA's first unit; false when it has none
+    __device__ __forceinline__ bool begin(const AttnArgs* args, int cta, int ncta, int npairs_) {
         a = args;
-        W = 2 * ncta;
+        W = ncta;
         npairs = npairs_;
-        slot = slot_;
-        count = 0;
-        p = 2 * cta + slot_;
+        p = cta;
         qt = -1;
         if (p >= npairs) return false;
         load_pair();
@@ -137,7 +129,6 @@ struct UnitIter {
             }
             u = make_unit<MASKED>(sd, head, qt, a->ldkv);
             if (u.nt <= 0) continue;
-            ++count;
             return true;
         }
     }
@@ -149,370 +140,215 @@ __device__ __forceinline__ float fast_exp2(float x) {
     return r;
 }
 
-template <int HD, int MASKED, int PT>
+template <int HD, int MASKED>
 __global__ void __launch_bounds__(kAtThreads, 1) attn_tc_kernel(const __grid_constant__ AttnMaps maps,
                                                                 const AttnArgs args) {
     using Cfg = AtCfg<HD>;
     constexpr int NB = Cfg::NB;
+    constexpr int NO = Cfg::NO;
     extern __shared__ uint8_t at_smem_raw[];
     const uint32_t raw_addr = smem_u32(at_smem_raw);
     uint8_t* smem = at_smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
-    SlotBars* bars = reinterpret_cast<SlotBars*>(smem + 2 * Cfg::kSlotBytes);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + 2 * Cfg::kSlotBytes + 2 * sizeof(SlotBars));
+    uint8_t* sQ = smem;
+    uint8_t* sKV = smem + Cfg::kQBytes;
+    uint8_t* sZero = sKV + kAtStages * Cfg::kStageBytes;
+    Bars& b = *reinterpret_cast<Bars*>(sZero + Cfg::kZeroBytes);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
-        for (int s = 0; s < 2; ++s) {
-            SlotBars& b = bars[s];
-            mbar_init(&b.q_full, 1);
-            mbar_init(&b.q_empty, 1);
-            for (int i = 0; i < 2; ++i) {
-                mbar_init(&b.kv_full[i], 1);
-                mbar_init(&b.kv_empty[i], 1);
-                mbar_init(&b.s_full[i], 1);
-                mbar_init(&b.s_free[i], PT ? 1 : 4);   // PT: released by the MMA thread's commit after the P V product
-            }
-            mbar_init(&b.p_full, 4);
-            mbar_init(&b.p_empty, 1);
-            mbar_init(&b.o_full, 1);
-            mbar_init(&b.o_free, 4);
+        mbar_init(&b.q_full, 1);
+        mbar_init(&b.q_empty, 8);   // one arrive per consumer warp
+        for (int i = 0; i < kAtStages; ++i) {
+            mbar_init(&b.kv_full[i], 1);
+            mbar_init(&b.kv_empty[i], 8);
         }
         fence_mbar_init();
         tma_prefetch_desc(&maps.q);
         tma_prefetch_desc(&maps.k);
         tma_prefetch_desc(&maps.v);
     }
-    if (warp == 10) {
-        tmem_alloc(tmem_slot, 512);
-        tmem_relinquish();
-    }
-    tc_fence_before();
+    for (int i = threadIdx.x; i < Cfg::kZeroBytes / 16; i += blockDim.x)
+        reinterpret_cast<uint4*>(sZero)[i] = make_uint4(0u, 0u, 0u, 0u);
+    fence_proxy_async_smem();   // the zero tile (generic-proxy stores) -> visible to the wgmma operand reads
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     const int npairs = args.nseq * args.heads;
+    const int cta = static_cast<int>(blockIdx.x), ncta = static_cast<int>(gridDim.x);
 
     if (warp < 8) {
-        // ------------------------------------------------------------------ softmax + epilogue, slot = warp / 4
-        const int s = warp >> 2, q = warp & 3;
-        const int row = q * 32 + lane;
-        SlotBars& b = bars[s];
-        uint8_t* sP = smem + s * Cfg::kSlotBytes + Cfg::kQBytes;
-        uint8_t* p_row = sP + (row >> 3) * 1024 + (row & 7) * 128;
-        const uint32_t t_lane = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(s * 256);
-        uint32_t nu = 0, c = 0;
+        // ------------------------------------------------------------------ MMA + softmax + epilogue, 64 queries
+        const int wg = warp >> 2, wl = warp & 3;
+        const int r_in = wg * 64 + wl * 16 + (lane >> 2);   // tile row of this thread's first row (second: + 8)
+        const int cq = (lane & 3) * 2;                      // first of the thread's two columns in every 8-column block
+        const uint32_t q_addr = smem_u32(sQ) + static_cast<uint32_t>(wg * 64 * 128);
+        uint32_t nu = 0, ck = 0;
         UnitIter<MASKED> it;
-        for (bool more = it.begin(&args, static_cast<int>(blockIdx.x), static_cast<int>(gridDim.x), npairs, s); more;
-             more = it.next()) {
-            {
-                const Unit u = it.u;
-                const int head = u.head;
-                const bool warp_active = q * 32 < u.rows;  // warp-uniform
-                const int qi = u.q0 + row;                 // this thread's query index inside the sequence
-                float m_ref = -INFINITY, l_run = 0.f;
-                for (int t = 0; t < u.nt; ++t, ++c) {
-                    const uint32_t buf = c & 1u;
-                    mbar_wait(&b.s_full[buf], (c >> 1) & 1u);
-                    tc_fence_after();
-                    uint32_t sv[64];
-                    if (warp_active) {
-                        tmem_ld_32x32(t_lane + buf * 64u, reinterpret_cast<uint32_t(&)[32]>(sv[0]));
-                        tmem_ld_32x32(t_lane + buf * 64u + 32u, reinterpret_cast<uint32_t(&)[32]>(sv[32]));
-                        tmem_ld_wait();
-                    }
-                    if constexpr (!PT) {
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(&b.s_free[buf]);  // the S buffer may be overwritten (tile t + 2)
-                    }
-                    const int key0 = t * kAtKV;
-                    float mt = -INFINITY;
-                    if (warp_active) {
+        for (bool more = it.begin(&args, cta, ncta, npairs); more; more = it.next(), ++nu) {
+            const Unit u = it.u;
+            float m_ref[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+            float o[NO / 2];
 #pragma unroll
-                        for (int j = 0; j < 64; ++j) {
-                            const int key = key0 + j;
-                            bool vis = key < u.k_end;
-                            if (MASKED) vis = vis && ((qi < 2) || (key <= qi));
-                            const float v = vis ? __uint_as_float(sv[j]) * args.scale_log2 : -INFINITY;
-                            sv[j] = __float_as_uint(v);
-                            mt = fmaxf(mt, v);
-                        }
-                    }
-                    // reference max: moves only when the tile max exceeds it by more than the threshold
-                    float factor = 1.f;
-                    bool moved = false;
-                    if (mt > m_ref + kRescaleThreshold || (m_ref == -INFINITY && mt > -INFINITY)) {
-                        factor = (m_ref == -INFINITY) ? 0.f : fast_exp2(m_ref - mt);
-                        moved = m_ref != -INFINITY;   // O holds contributions that must be rescaled
-                        m_ref = mt;
-                        l_run *= factor;
-                    }
-                    // exponentials first (registers only) ...
-                    const int nch = ((min(kAtKV, u.k_end - key0) + 15) >> 4) * 2;   // 8-key chunks the P V product reads
-                    uint32_t pk[32];
-                    if (warp_active) {
-                        const float m_use = (m_ref == -INFINITY) ? 0.f : m_ref;
-                        float ls = 0.f;
+            for (int i = 0; i < NO / 2; ++i) o[i] = 0.f;
+            mbar_wait(&b.q_full, nu & 1u);
+            for (int t = 0; t < u.nt; ++t, ++ck) {
+                const uint32_t st = ck % kAtStages;
+                mbar_wait(&b.kv_full[st], (ck / kAtStages) & 1u);
+                const uint32_t k_addr = smem_u32(sKV + st * Cfg::kStageBytes);
+                const uint32_t v_addr = k_addr + Cfg::kKBytes;
+                // ---- S = Q K^T (64 queries x 64 keys)
+                float s[32];
 #pragma unroll
-                        for (int ch = 0; ch < 8; ++ch) {
-                            if (ch < nch) {
+                for (int i = 0; i < 32; ++i) s[i] = 0.f;
+                reg_fence(s);
+                wgmma_fence();
 #pragma unroll
-                                for (int j = 0; j < 4; ++j) {
-                                    const float p0 = fast_exp2(__uint_as_float(sv[ch * 8 + 2 * j]) - m_use);  // exp2(-inf) = 0
-                                    const float p1 = fast_exp2(__uint_as_float(sv[ch * 8 + 2 * j + 1]) - m_use);
-                                    ls += p0 + p1;
-                                    pk[ch * 4 + j] = pack_op(p0, p1);
-                                }
-                            } else {
-#pragma unroll
-                                for (int j = 0; j < 4; ++j) pk[ch * 4 + j] = 0u;
-                            }
-                        }
-                        l_run += ls;
-                    }
-                    // ... then the only point that depends on the previous tile's P V product (by now it has almost always
-                    // completed): smem mode - the P buffer is free; both modes - O is stable and may be rescaled
-                    mbar_wait(&b.p_empty, (c & 1u) ^ 1u);
-                    if (t > 0 && __any_sync(0xffffffffu, moved)) {
-                        tc_fence_after();
-                        if (warp_active) {
-#pragma unroll
-                            for (int ch = 0; ch < (HD + 31) / 32; ++ch) {
-                                uint32_t ov[32];
-                                tmem_ld_32x32(t_lane + 128u + ch * 32u, ov);
-                                tmem_ld_wait();
-#pragma unroll
-                                for (int j = 0; j < 32; ++j) ov[j] = __float_as_uint(__uint_as_float(ov[j]) * factor);
-                                tmem_st_32x32(t_lane + 128u + ch * 32u, ov);
-                            }
-                            tmem_st_wait();
-                        }
-                    }
-                    if (warp_active) {
-                        if constexpr (PT) {
-                            // P overwrites the S buffer it came from: 64 fp16 = 32 columns of this thread's lane
-                            tmem_st_32x32(t_lane + buf * 64u, pk);
-                            tmem_st_wait();
-                        } else {
-#pragma unroll
-                            for (int ch = 0; ch < 8; ++ch) {
-                                if (ch < nch)
-                                    *reinterpret_cast<uint4*>(p_row + ((ch ^ (row & 7)) << 4)) =
-                                        make_uint4(pk[ch * 4], pk[ch * 4 + 1], pk[ch * 4 + 2], pk[ch * 4 + 3]);
-                            }
-                        }
-                    }
-                    if constexpr (!PT) fence_proxy_async_smem();  // P (generic-proxy stores) -> visible to the MMA's operand reads
-                    tc_fence_before();
+                for (int j = 0; j < HD / 16; ++j) {
+                    const uint64_t da = wgmma_desc_sw128(q_addr + (j >> 2) * (kAtQ * 128)) + static_cast<uint64_t>(2 * (j & 3));
+                    const uint64_t db = wgmma_desc_sw128(k_addr + (j >> 2) * (kAtKV * 128)) + static_cast<uint64_t>(2 * (j & 3));
+                    wgmma_ss<64>(s, da, db, j != 0 ? 1u : 0u);
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                reg_fence(s);
+                if (t == u.nt - 1) {   // the Q tile is consumed: the producer may load the next unit's
                     __syncwarp();
-                    if (lane == 0) mbar_arrive(&b.p_full);
+                    if (lane == 0) mbar_arrive(&b.q_empty);
                 }
-                // ---- epilogue: O / l -> global
-                mbar_wait(&b.o_full, nu & 1u);
-                tc_fence_after();
-                if (warp_active) {
-                    const float inv = l_run > 0.f ? 1.f / l_run : 0.f;
-                    op_t* op = args.O + static_cast<long long>(u.o_row + row) * args.ldo + head * HD;
+                // ---- mask, scale, tile max of both rows (a row is spread over the 4 lanes of a quad)
+                const int key0 = t * kAtKV;
+                float mt[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-                    for (int ch = 0; ch < (HD + 31) / 32; ++ch) {
-                        uint32_t ov[32];
-                        tmem_ld_32x32(t_lane + 128u + ch * 32u, ov);
-                        tmem_ld_wait();
-                        if (row < u.rows) {
+                for (int i = 0; i < 32; ++i) {
+                    const int h = (i >> 1) & 1;
+                    const int key = key0 + (i >> 2) * 8 + cq + (i & 1);
+                    const int qi = u.q0 + r_in + 8 * h;   // query index inside the sequence
+                    bool vis = key < u.k_end;
+                    if (MASKED) vis = vis && ((qi < 2) || (key <= qi));
+                    const float v = vis ? s[i] * args.scale_log2 : -INFINITY;
+                    s[i] = v;
+                    mt[h] = fmaxf(mt[h], v);
+                }
+                float factor[2];
 #pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                if (ch * 32 + j * 8 < HD) {
-                                    uint4 o;
-                                    o.x = pack_op(__uint_as_float(ov[8 * j + 0]) * inv, __uint_as_float(ov[8 * j + 1]) * inv);
-                                    o.y = pack_op(__uint_as_float(ov[8 * j + 2]) * inv, __uint_as_float(ov[8 * j + 3]) * inv);
-                                    o.z = pack_op(__uint_as_float(ov[8 * j + 4]) * inv, __uint_as_float(ov[8 * j + 5]) * inv);
-                                    o.w = pack_op(__uint_as_float(ov[8 * j + 6]) * inv, __uint_as_float(ov[8 * j + 7]) * inv);
-                                    *reinterpret_cast<uint4*>(op + ch * 32 + j * 8) = o;
-                                }
-                            }
-                        }
+                for (int h = 0; h < 2; ++h) {
+                    mt[h] = fmaxf(mt[h], __shfl_xor_sync(0xffffffffu, mt[h], 1));
+                    mt[h] = fmaxf(mt[h], __shfl_xor_sync(0xffffffffu, mt[h], 2));
+                    // reference max: moves only when the tile max exceeds it by more than the threshold
+                    factor[h] = 1.f;
+                    if (mt[h] > m_ref[h] + kRescaleThreshold || (m_ref[h] == -INFINITY && mt[h] > -INFINITY)) {
+                        factor[h] = (m_ref[h] == -INFINITY) ? 0.f : fast_exp2(m_ref[h] - mt[h]);
+                        m_ref[h] = mt[h];
+                        l_run[h] *= factor[h];
                     }
                 }
-                tc_fence_before();
+                if (factor[0] != 1.f || factor[1] != 1.f) {
+#pragma unroll
+                    for (int i = 0; i < NO / 2; ++i) o[i] *= factor[(i >> 1) & 1];
+                }
+                // ---- P = exp2(S - m) as fp16 A fragments: k step ks covers keys 16 ks .. 16 ks + 15
+                uint32_t pa[4][4];
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const float m_use = (m_ref[h] == -INFINITY) ? 0.f : m_ref[h];
+                    float ls = 0.f;
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) {
+                        const float p0 = fast_exp2(s[4 * j + 2 * h] - m_use);  // exp2(-inf) = 0
+                        const float p1 = fast_exp2(s[4 * j + 2 * h + 1] - m_use);
+                        ls += p0 + p1;
+                        pa[j >> 1][(j & 1) * 2 + h] = pack_op(p0, p1);
+                    }
+                    l_run[h] += ls;
+                }
+                // ---- O += P V.  All four 16-key steps are issued (a wgmma under a branch is serialised); a step past
+                // the last visible key has P = 0 and reads the zero tile instead of V rows that belong to no sequence
+                // of this unit (their contents need not be finite)
+                const int ksteps = (min(kAtKV, u.k_end - key0) + 15) >> 4;
+                reg_fence(o);
+                wgmma_fence();
+#pragma unroll
+                for (int ks = 0; ks < 4; ++ks) {
+                    const bool live = ks < ksteps;
+                    const uint64_t db = live ? wgmma_desc_sw128_mn(v_addr + ks * 2048, kAtKV * 128)
+                                             : wgmma_desc_sw128_mn(smem_u32(sZero), 2048);
+                    wgmma_rs<NO>(o, pa[ks], db, 1u);
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                reg_fence(o);
                 __syncwarp();
-                if (lane == 0) mbar_arrive(&b.o_free);
-                ++nu;
+                if (lane == 0) mbar_arrive(&b.kv_empty[st]);   // K / V stage consumed
+            }
+            // ---- epilogue: O / l -> global
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 1);
+                l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], 2);
+                const int r = r_in + 8 * h;
+                if (r < u.rows) {
+                    const float inv = l_run[h] > 0.f ? 1.f / l_run[h] : 0.f;
+                    op_t* op = args.O + static_cast<long long>(u.o_row + r) * args.ldo + u.head * HD + cq;
+#pragma unroll
+                    for (int j = 0; j < HD / 8; ++j)
+                        *reinterpret_cast<uint32_t*>(op + 8 * j) = pack_op(o[4 * j + 2 * h] * inv, o[4 * j + 2 * h + 1] * inv);
+                }
             }
         }
-    } else if (warp < 10) {
-        // ------------------------------------------------------------------ TMA producer of slot s
-        if (lane == 0) {
-            const int s = warp - 8;
-            SlotBars& b = bars[s];
-            uint8_t* sQ = smem + s * Cfg::kSlotBytes;
-            uint8_t* sKV = sQ + Cfg::kQBytes + Cfg::kPBytes;
-            uint32_t nu = 0, ck = 0;
-            UnitIter<MASKED> it, pf;     // pf runs one unit ahead: its tiles are pulled into L2 while `it` is being fed
-            bool more = it.begin(&args, static_cast<int>(blockIdx.x), static_cast<int>(gridDim.x), npairs, s);
-            bool pf_more = pf.begin(&args, static_cast<int>(blockIdx.x), static_cast<int>(gridDim.x), npairs, s);
-            if (pf_more) pf_more = pf.next();
-            while (more) {
-                const Unit u = it.u;
-                const int head = u.head;
-                if (pf_more) {
-                    const Unit& n = pf.u;
+    } else if (lane == 0) {
+        // ------------------------------------------------------------------ TMA producer
+        uint32_t nu = 0, ck = 0;
+        UnitIter<MASKED> it, pf;     // pf runs one unit ahead: its tiles are pulled into L2 while `it` is being fed
+        bool more = it.begin(&args, cta, ncta, npairs);
+        bool pf_more = pf.begin(&args, cta, ncta, npairs);
+        if (pf_more) pf_more = pf.next();
+        while (more) {
+            const Unit u = it.u;
+            const int head = u.head;
+            if (pf_more) {
+                const Unit& n = pf.u;
 #pragma unroll
-                    for (int blk = 0; blk < NB; ++blk) tma_prefetch_l2_4d(&maps.q, n.head * HD + blk * 64, n.q_row, 0, 0);
-                    if (n.q0 == 0) {      // the pair's first query tile brings its keys / values in (later tiles re-read them)
-                        const int nt = min(n.nt, 6);
-                        for (int t = 0; t < nt; ++t)
+                for (int blk = 0; blk < NB; ++blk) tma_prefetch_l2_4d(&maps.q, n.head * HD + blk * 64, n.q_row, 0, 0);
+                if (n.q0 == 0) {      // the pair's first query tile brings its keys / values in (later tiles re-read them)
+                    const int nt = min(n.nt, 6);
+                    for (int t = 0; t < nt; ++t)
 #pragma unroll
-                            for (int blk = 0; blk < NB; ++blk) {
-                                tma_prefetch_l2_4d(&maps.k, n.head * HD + blk * 64, n.k_row + t * kAtKV, 0, 0);
-                                tma_prefetch_l2_4d(&maps.v, n.head * HD + blk * 64, n.k_row + t * kAtKV, 0, 0);
-                            }
-                    }
-                    pf_more = pf.next();
-                }
-                mbar_wait(&b.q_empty, (nu & 1u) ^ 1u);
-                mbar_expect_tx(&b.q_full, Cfg::kQBytes);
-#pragma unroll
-                for (int blk = 0; blk < NB; ++blk)
-                    tma_load_4d(sQ + blk * (kAtQ * 128), &maps.q, &b.q_full, head * HD + blk * 64, u.q_row, 0, 0);
-                ++nu;
-                for (int t = 0; t < u.nt; ++t, ++ck) {
-                    const uint32_t st = ck & 1u;
-                    mbar_wait(&b.kv_empty[st], ((ck >> 1) & 1u) ^ 1u);
-                    mbar_expect_tx(&b.kv_full[st], Cfg::kStageBytes);
-                    uint8_t* sK = sKV + st * Cfg::kStageBytes;
-                    uint8_t* sV = sK + Cfg::kKBytes;
-#pragma unroll
-                    for (int blk = 0; blk < NB; ++blk) {
-                        tma_load_4d(sK + blk * (kAtKV * 128), &maps.k, &b.kv_full[st], head * HD + blk * 64,
-                                    u.k_row + t * kAtKV, 0, 0);
-                        tma_load_4d(sV + blk * (kAtKV * 128), &maps.v, &b.kv_full[st], head * HD + blk * 64,
-                                    u.k_row + t * kAtKV, 0, 0);
-                    }
-                }
-                more = it.next();
-            }
-        }
-    } else {
-        // ------------------------------------------------------------------ MMA issuer (one thread, both slots)
-        if (lane == 0) {
-            // Two cursors per slot: the S cursor may run into the NEXT unit (its Q tile arrives as soon as the last Q K^T of
-            // the current unit has been issued, S buffers and K/V stages free up tile by tile) while the P V cursor is
-            // still on the current one - the next unit's first score tile is then ready when the softmax warps come
-            // out of the epilogue.
-            struct Cur {
-                UnitIter<MASKED> it;
-                Unit u;
-                int t;        // next key tile of `u`
-                uint32_t n;   // units this cursor has finished
-                bool done;
-            };
-            struct St {
-                Cur s, p;
-                uint32_t cs, cpv;   // key tiles issued as S / as P V (per slot, across units)
-            } st[2];
-            auto advance = [&](Cur& c, bool first, int slot) {
-                const bool more = first ? c.it.begin(&args, static_cast<int>(blockIdx.x), static_cast<int>(gridDim.x),
-                                                     npairs, slot)
-                                        : c.it.next();
-                c.done = !more;
-                if (more) c.u = c.it.u;
-                c.t = 0;
-            };
-            for (int s = 0; s < 2; ++s) {
-                st[s].cs = st[s].cpv = 0;
-                st[s].s.n = st[s].p.n = 0;
-                advance(st[s].s, true, s);
-                advance(st[s].p, true, s);
-            }
-            constexpr uint32_t idesc_pv = umma_idesc_op(kAtQ, HD) | kIdescBMajorMN;
-            while (!(st[0].p.done && st[1].p.done)) {
-#pragma unroll
-                for (int s = 0; s < 2; ++s) {
-                    St& S = st[s];
-                    if (S.p.done) continue;
-                    SlotBars& b = bars[s];
-                    const uint32_t q_addr = smem_u32(smem + s * Cfg::kSlotBytes);
-                    const uint32_t p_addr = q_addr + Cfg::kQBytes;
-                    const uint32_t kv_addr = p_addr + Cfg::kPBytes;
-                    const uint32_t t_slot = tmem_base + static_cast<uint32_t>(s * 256);
-                    // ---- S = Q K^T of the next key tile (of the current or the following unit)
-                    if (!S.s.done) {
-                        const uint32_t buf = S.cs & 1u, par = (S.cs >> 1) & 1u;
-                        bool ok = mbar_test(&b.kv_full[buf], par) && mbar_test(&b.s_free[buf], par ^ 1u);
-                        if (ok && S.s.t == 0) ok = mbar_test(&b.q_full, S.s.n & 1u);
-                        if (ok) {
-                            tc_fence_after();
-                            const Unit& u = S.s.u;
-                            const int nkeys = min(kAtKV, u.k_end - S.s.t * kAtKV);
-                            const uint32_t idesc_s = umma_idesc_op(kAtQ, (nkeys + 15) & ~15);
-                            const uint32_t k_addr = kv_addr + buf * Cfg::kStageBytes;
-#pragma unroll
-                            for (int j = 0; j < HD / 16; ++j) {
-                                const uint64_t da = umma_desc_sw128(q_addr + (j >> 2) * (kAtQ * 128)) + static_cast<uint64_t>(2 * (j & 3));
-                                const uint64_t db = umma_desc_sw128(k_addr + (j >> 2) * (kAtKV * 128)) + static_cast<uint64_t>(2 * (j & 3));
-                                umma_op(t_slot + buf * 64u, da, db, idesc_s, j != 0 ? 1u : 0u);
-                            }
-                            umma_commit(&b.s_full[buf]);
-                            ++S.cs;
-                            if (++S.s.t == u.nt) {
-                                umma_commit(&b.q_empty);   // Q tile consumed: the producer may load the next unit's
-                                ++S.s.n;
-                                advance(S.s, false, s);
-                            }
+                        for (int blk = 0; blk < NB; ++blk) {
+                            tma_prefetch_l2_4d(&maps.k, n.head * HD + blk * 64, n.k_row + t * kAtKV, 0, 0);
+                            tma_prefetch_l2_4d(&maps.v, n.head * HD + blk * 64, n.k_row + t * kAtKV, 0, 0);
                         }
-                    }
-                    // ---- O += P V of the oldest key tile whose P is ready
-                    if (S.cpv < S.cs) {
-                        bool ok = mbar_test(&b.p_full, S.cpv & 1u);
-                        if (ok && S.p.t == 0) ok = mbar_test(&b.o_free, (S.p.n & 1u) ^ 1u);  // previous unit's O read out
-                        if (ok) {
-                            tc_fence_after();
-                            const Unit& u = S.p.u;
-                            const uint32_t stg = S.cpv & 1u;
-                            const int nkeys = min(kAtKV, u.k_end - S.p.t * kAtKV);
-                            const int ksteps = (nkeys + 15) >> 4;
-                            const uint32_t v_addr = kv_addr + stg * Cfg::kStageBytes + Cfg::kKBytes;
-                            for (int j = 0; j < ksteps; ++j) {
-                                const uint64_t db = umma_desc_sw128_mn(v_addr + j * 2048, kAtKV * 128, args.vswap);
-                                if constexpr (PT) {
-                                    // A = P from tensor memory: 16 keys = 8 columns of the tile's S buffer
-                                    umma_op_ts(t_slot + 128u, t_slot + stg * 64u + j * 8u, db, idesc_pv,
-                                               (S.p.t | j) != 0 ? 1u : 0u);
-                                } else {
-                                    const uint64_t da = umma_desc_sw128(p_addr) + static_cast<uint64_t>(2 * j);
-                                    umma_op(t_slot + 128u, da, db, idesc_pv, (S.p.t | j) != 0 ? 1u : 0u);
-                                }
-                            }
-                            if constexpr (PT) umma_commit(&b.s_free[stg]);   // P read: the S buffer may take tile t + 2
-                            umma_commit(&b.kv_empty[stg]);
-                            umma_commit(&b.p_empty);
-                            ++S.cpv;
-                            if (++S.p.t == u.nt) {
-                                umma_commit(&b.o_full);
-                                ++S.p.n;
-                                advance(S.p, false, s);
-                            }
-                        }
-                    }
+                }
+                pf_more = pf.next();
+            }
+            mbar_wait(&b.q_empty, (nu & 1u) ^ 1u);
+            mbar_expect_tx(&b.q_full, Cfg::kQBytes);
+#pragma unroll
+            for (int blk = 0; blk < NB; ++blk)
+                tma_load_4d(sQ + blk * (kAtQ * 128), &maps.q, &b.q_full, head * HD + blk * 64, u.q_row, 0, 0);
+            ++nu;
+            for (int t = 0; t < u.nt; ++t, ++ck) {
+                const uint32_t st = ck % kAtStages;
+                mbar_wait(&b.kv_empty[st], ((ck / kAtStages) & 1u) ^ 1u);
+                mbar_expect_tx(&b.kv_full[st], Cfg::kStageBytes);
+                uint8_t* sK = sKV + st * Cfg::kStageBytes;
+                uint8_t* sV = sK + Cfg::kKBytes;
+#pragma unroll
+                for (int blk = 0; blk < NB; ++blk) {
+                    tma_load_4d(sK + blk * (kAtKV * 128), &maps.k, &b.kv_full[st], head * HD + blk * 64,
+                                u.k_row + t * kAtKV, 0, 0);
+                    tma_load_4d(sV + blk * (kAtKV * 128), &maps.v, &b.kv_full[st], head * HD + blk * 64,
+                                u.k_row + t * kAtKV, 0, 0);
                 }
             }
+            more = it.next();
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 10) {
-        __syncwarp();
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
     }
 }
 
-template <int HD, int MASKED, int PT>
-int launch_attn(const AttnMaps& maps, const AttnArgs& a, int grid, cudaStream_t st) {
+template <int HD, int MASKED>
+int launch_attn(const AttnMaps& maps, const AttnArgs& a, int pairs, cudaStream_t st) {
     using Cfg = AtCfg<HD>;
     static unsigned long long attr_done = 0;   // per device
-    auto kern = attn_tc_kernel<HD, MASKED, PT>;
+    auto kern = attn_tc_kernel<HD, MASKED>;
     if (first_launch_on_device(&attr_done)) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
         if (e != cudaSuccess) {
@@ -520,6 +356,7 @@ int launch_attn(const AttnMaps& maps, const AttnArgs& a, int grid, cudaStream_t 
             return 1;
         }
     }
+    const int grid = pairs < num_sms() ? pairs : num_sms();
     kern<<<grid, kAtThreads, Cfg::kSmemBytes, st>>>(maps, a);
     return 0;
 }
@@ -528,7 +365,7 @@ int launch_attn(const AttnMaps& maps, const AttnArgs& a, int grid, cudaStream_t 
 
 int launch_attention_tc(const void* Q, long long ldq, long long q_rows, const void* K, const void* V, long long ldkv,
                         long long kv_rows, void* O, long long ldo, const SeqDesc* seqs, int nseq, int heads,
-                        int head_dim, int masked, int vswap, cudaStream_t st) {
+                        int head_dim, int masked, cudaStream_t st) {
     if (nseq <= 0) return 0;
     if (head_dim != 32 && head_dim != 48 && head_dim != 64 && head_dim != 96) {
         set_error("attention: head_dim %d unsupported (32/48/64/96)", head_dim);
@@ -565,18 +402,12 @@ int launch_attention_tc(const void* Q, long long ldq, long long q_rows, const vo
     a.scale_log2 = 1.4426950408889634f / sqrtf(static_cast<float>(head_dim));
     a.O = reinterpret_cast<op_t*>(O);
     a.ldo = ldo;
-    a.vswap = vswap & 1;
-    const bool p_tmem = (vswap & 2) != 0;
     const int pairs = nseq * heads;
-    int grid = (pairs + 1) / 2;
-    if (grid > num_sms()) grid = num_sms();
     int rc = 0;
-#define YTK_AT(HD_)                                                             \
-    do {                                                                        \
-        if (masked && p_tmem) rc = launch_attn<HD_, 1, 1>(maps, a, grid, st);   \
-        else if (masked) rc = launch_attn<HD_, 1, 0>(maps, a, grid, st);        \
-        else if (p_tmem) rc = launch_attn<HD_, 0, 1>(maps, a, grid, st);        \
-        else rc = launch_attn<HD_, 0, 0>(maps, a, grid, st);                    \
+#define YTK_AT(HD_)                                                  \
+    do {                                                             \
+        if (masked) rc = launch_attn<HD_, 1>(maps, a, pairs, st);    \
+        else rc = launch_attn<HD_, 0>(maps, a, pairs, st);           \
     } while (0)
     switch (head_dim) {
         case 32: YTK_AT(32); break;

@@ -1,5 +1,5 @@
 // DBNet++ (ResNet-50 dilated backbone + FPN decoder + Adaptive Scale Fusion + binarize head) as a static launch plan
-// of tcgen05 implicit-GEMM convolutions and a few memory-bound kernels.  Replaces reference
+// of wgmma implicit-GEMM convolutions and a few memory-bound kernels.  Replaces reference
 // models/dbnet_plus.py:13-246 + models/layers/dbnet_feature_attention.py:36-160 for inference.
 //
 // Data layout in HBM: every activation is NHWC bf16 (channels innermost, 16-byte vectors), batch-norm is folded into

@@ -1,4 +1,4 @@
-// Memory-bound CUDA kernels around the tcgen05 convolutions of DBNet++ (all NHWC bf16, 8-channel = 16-byte vectors).
+// Memory-bound CUDA kernels around the wgmma convolutions of DBNet++ (all NHWC bf16, 8-channel = 16-byte vectors).
 // Each kernel cites the reference op it replaces; they are HBM-bound by construction (no data reuse beyond a 3x3
 // neighbourhood), so the design rule is: coalesced 16 B accesses, one pass, no intermediate tensors.
 #include "dbnet_ops.h"

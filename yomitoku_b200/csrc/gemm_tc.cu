@@ -1,13 +1,15 @@
-// tcgen05 implicit-GEMM convolution / linear kernel for sm_100a.  See gemm_tc.h for the contract.
+// wgmma implicit-GEMM convolution / linear kernel for sm_90a.  See gemm_tc.h for the contract.
 //
-// Warp roles (320 threads, 1 CTA per SM, persistent over output tiles):
-//   warp 0      : TMA producer  (one elected lane) - A patch box + W box per 64-wide K block, STAGES-deep ring
-//   warp 1      : MMA issuer    (one lane)         - 4 x tcgen05.mma (K=16) per K block into a TMEM accumulator
-//   warps 2..9  : epilogue      (256 threads)      - tcgen05.ld -> bias/residual/activation -> TMA boxes (residual in by
-//                                                    cp.async.bulk.tensor, result out by TMA store) or, for the plans the
-//                                                    TMA path does not cover, staged per-thread global accesses
-// Pipelines: smem full/empty mbarriers (TMA <-> MMA), TMEM full/empty mbarriers (MMA <-> epilogue, 2 buffers) and, in
-// the TMA epilogue, one mbarrier per residual box of every epilogue warp's ring.
+// Warp roles (384 threads, 1 CTA per SM, persistent over output tiles):
+//   warp 8      : TMA producer  (one elected lane) - A patch box + W box per 64-wide K block, STAGES-deep ring; the
+//                 producer warpgroup (warps 8..11) hands its registers to the consumers (setmaxnreg)
+//   warps 0..7  : two consumer warpgroups          - each: 4 x wgmma (K=16) per K block into a 64 x BLOCK_N register
+//                                                    accumulator (tile rows 64 wg ..), then the epilogue of those rows:
+//                                                    bias/residual/activation -> TMA boxes (residual in by
+//                                                    cp.async.bulk.tensor, result out by TMA store) or, for the plans
+//                                                    the TMA path does not cover, staged per-thread global accesses
+// Pipelines: smem full/empty mbarriers (TMA <-> MMA) and, in the TMA epilogue, one mbarrier per residual box of every
+// epilogue warp's ring.  The producer runs ahead into the next tile's K blocks while the consumers store.
 #include "gemm_tc.h"
 
 #include <cstdarg>
@@ -37,10 +39,8 @@ void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 long long launch_count() { return g_launches.load(std::memory_order_relaxed); }
 
 int pdl_launch_attr(cudaLaunchAttribute* attr) {
-    // Opt-in (YTK_PDL=1).  Measured on B200 (profiles/README_r02.md): with programmatic stream serialization the AR
-    // loop of 3200 rows took 77-80 ms instead of 62-63 ms and the encoder 95.5 instead of 92 ms - a dependent persistent
-    // GEMM CTA that becomes resident early takes its SM away from the remaining waves of the multi-wave kernel before
-    // it, which costs more than the overlapped prologue saves.  The kernels keep their griddepcontrol.wait (a no-op for a
+    // Opt-in (YTK_PDL=1): a dependent persistent GEMM CTA that becomes resident early takes its SM away from the
+    // remaining waves of the multi-wave kernel before it, which can cost more than the overlapped prologue saves.  The kernels keep their griddepcontrol.wait (a no-op for a
     // normal launch) so that the experiment stays one environment variable away.
     static const bool on = getenv("YTK_PDL") != nullptr && getenv("YTK_NO_PDL") == nullptr;
     if (!on) return 0;
@@ -64,25 +64,31 @@ int num_sms() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 148;
+        if (n <= 0) n = 132;
     }
     return n;
 }
 
 // ------------------------------------------------------------------------------------------------ kernel
 constexpr int kBlockM = 128;
-constexpr int kBlockK = 64;  // 64 bf16 = 128 B = one swizzle row
+constexpr int kBlockK = 64;  // 64 16-bit elements = 128 B = one swizzle row
 constexpr int kABytes = kBlockM * kBlockK * 2;
-constexpr int kThreads = 320;       // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue
+constexpr int kThreads = 384;       // warps 0..7: two consumer warpgroups (MMA + epilogue), warps 8..11: TMA producer
+constexpr int kProducerWarp = 8;
 constexpr int kStagePitch = 80;     // bytes per staged row: 64 B payload + 16 B pad (conflict-free 16 B accesses)
 constexpr int kEpiStageBytes = 8 * 32 * kStagePitch;
+// Accumulator hand-off: a warpgroup's 64 x BLOCK_N accumulator lives in its registers in the wgmma fragment layout, the
+// epilogue works on one output row per thread.  64-column slices pass through a per-warpgroup buffer
+// [64 rows][kAccPitch fp32] (pitch 68 words: the row-per-thread 16-byte reads are conflict-free).
+constexpr int kAccPitch = 68;
+constexpr int kAccBytes = 2 * 64 * kAccPitch * 4;
 
-// TMA epilogue (DIRECT == 2): every epilogue warp owns a small ring of 2 KB buffers (32 tile rows x 64 bytes, 64-byte
-// swizzled = the layout a TMA box of that shape has in shared memory).  With a residual the ring is 4 deep: three
-// residual boxes are in flight (loaded by TMA long before the accumulator is ready) while the fourth is being stored;
-// without one, 2 buffers double-buffer the TMA stores.
+// TMA epilogue (DIRECT == 2): every epilogue warp owns a ring of 2 KB buffers (32 tile rows x 64 bytes, 64-byte
+// swizzled = the layout a TMA box of that shape has in shared memory).  Two per warp: with a residual one box is in
+// flight (loaded by TMA while the MMAs of the tile run) while the other is being stored; without one they double-buffer
+// the TMA stores.  A deeper ring would cost the 256-wide tiles one of their three K stages.
 constexpr int kEpiBufBytes = 32 * 64;
-constexpr int epi_tma_nbuf(int resid) { return resid ? 4 : 2; }
+constexpr int epi_tma_nbuf(int /*resid*/) { return 2; }
 constexpr int kSmemLimit = 232448;  // 227 KB of dynamic shared memory per CTA
 constexpr int kSmemFixed = 1024 /*final-conv weights*/ + 1024 /*align slack*/ + 512 /*barriers*/;
 
@@ -90,17 +96,13 @@ template <int BLOCK_N, int EPI_BYTES = kEpiStageBytes>
 struct TileCfg {
     static constexpr int kBBytes = BLOCK_N * kBlockK * 2;
     static constexpr int kStageBytes = kABytes + kBBytes;
-    static constexpr int kRingBudget = kSmemLimit - kSmemFixed - EPI_BYTES;
+    static constexpr int kRingBudget = kSmemLimit - kSmemFixed - kAccBytes - EPI_BYTES;
     static constexpr int kStages = (kRingBudget / kStageBytes) > 8 ? 8 : (kRingBudget / kStageBytes);
-    // CTA-pair mode: a CTA stages only half of the weight tile; the ring lives in the same kStages * kStageBytes bytes
-    static constexpr int kStageBytes2 = kABytes + kBBytes / 2;
-    static constexpr int kStages2 = (kRingBudget / kStageBytes2) > 8 ? 8 : (kRingBudget / kStageBytes2);
-    static constexpr int kRingBytes =
-        kStages * kStageBytes > kStages2 * kStageBytes2 ? kStages * kStageBytes : kStages2 * kStageBytes2;
-    static constexpr int kTmemCols = 2 * BLOCK_N;  // two accumulator buffers; 128/256/512 are powers of two
-    static constexpr int kSmemBytes = kRingBytes + EPI_BYTES + kSmemFixed;
+    static constexpr int kRingBytes = kStages * kStageBytes;
+    static constexpr int kSmemBytes = kRingBytes + kAccBytes + EPI_BYTES + kSmemFixed;
+    static_assert(kStages >= 3, "K pipeline depth");
     static_assert(kSmemBytes <= kSmemLimit, "shared memory budget");
-    static_assert(kRingBytes % 2048 == 0, "epilogue buffers must stay 2 KB aligned");
+    static_assert((kRingBytes + kAccBytes) % 2048 == 0, "epilogue buffers must stay 2 KB aligned");
 };
 
 // ragged last columns of a row segment: element-wise copy (rare; kept out of line)
@@ -110,44 +112,27 @@ __device__ __noinline__ void copy_elems(void* dst, const void* src, int n, int e
     else
         for (int e = 0; e < n; ++e) reinterpret_cast<uint16_t*>(dst)[e] = reinterpret_cast<const uint16_t*>(src)[e];
 }
-// Packed fp32x2 helpers (FFMA2 / FMUL2, sm_100) for the GELU below: two values per instruction.
-using f32x2 = unsigned long long;
-__device__ __forceinline__ f32x2 pk2(float a, float b) {
-    f32x2 r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-    return r;
-}
-__device__ __forceinline__ void upk2(f32x2 r, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(r)); }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-    f32x2 r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
-}
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) {
-    f32x2 r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-// Exact (erf) GELU of two values, fp32, max |error| 5e-7 (2.8e-7 for |x| < 3; the form it replaces, Abramowitz-Stegun
-// 7.1.26, had 0.5 |x| 1.5e-7):
+// Exact (erf) GELU, fp32, max |error| 5e-7 (2.8e-7 for |x| < 3; the form it replaces, Abramowitz-Stegun 7.1.26, had
+// 0.5 |x| 1.5e-7):
 //     GELU(x) = max(x, 0) - 0.5 t erfc(t / sqrt 2),   t = min(|x|, 5.7),   erfc(t / sqrt 2) = 2 ^ (t P(t))
-// P = degree-6 weighted minimax fit (experiments/gelu_fit.py).  One ex2 per element, no reciprocal, 7 packed FMAs per
-// pair: the fc1 epilogue is bound by instruction issue (profiles/README_r01.md), this form needs ~20 instructions per
-// pair instead of ~35.
+// P = degree-6 weighted minimax fit (experiments/gelu_fit.py).  One ex2 per element, no reciprocal: the fc1 epilogue is
+// bound by instruction issue, this form needs about half the instructions of a rational erf.
+__device__ __forceinline__ float gelu_fast(float x) {
+    const float t = fminf(fabsf(x), 5.7f);
+    float p = fmaf(4.278742836e-06f, t, -1.279820572e-05f);
+    p = fmaf(p, t, -5.757861654e-04f);
+    p = fmaf(p, t, 7.670783438e-03f);
+    p = fmaf(p, t, -5.294856429e-02f);
+    p = fmaf(p, t, -4.590439200e-01f);
+    p = fmaf(p, t, -1.151126981e+00f);
+    const float a = __fmul_rn(p, t);
+    float e;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(a));
+    return fmaf(__fmul_rn(t, -0.5f), e, fmaxf(x, 0.f));
+}
 __device__ __forceinline__ void gelu_fast2(float& x0, float& x1) {
-    const f32x2 t = pk2(fminf(fabsf(x0), 5.7f), fminf(fabsf(x1), 5.7f));
-    f32x2 p = fma2(pk2(4.278742836e-06f, 4.278742836e-06f), t, pk2(-1.279820572e-05f, -1.279820572e-05f));
-    p = fma2(p, t, pk2(-5.757861654e-04f, -5.757861654e-04f));
-    p = fma2(p, t, pk2(7.670783438e-03f, 7.670783438e-03f));
-    p = fma2(p, t, pk2(-5.294856429e-02f, -5.294856429e-02f));
-    p = fma2(p, t, pk2(-4.590439200e-01f, -4.590439200e-01f));
-    p = fma2(p, t, pk2(-1.151126981e+00f, -1.151126981e+00f));
-    float a0, a1, e0, e1;
-    upk2(mul2(p, t), a0, a1);
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(a0));
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(a1));
-    const f32x2 r = fma2(mul2(t, pk2(-0.5f, -0.5f)), pk2(e0, e1), pk2(fmaxf(x0, 0.f), fmaxf(x1, 0.f)));
-    upk2(r, x0, x1);
+    x0 = gelu_fast(x0);
+    x1 = gelu_fast(x1);
 }
 
 struct TileCoord {
@@ -167,51 +152,34 @@ __device__ __forceinline__ TileCoord decode_tile(const GemmArgs& a, int tile, in
     return t;
 }
 
-// Epilogue variants are compile-time (OUT_F32: fp32 vs bf16 output; RESID: 0 none, 1 bf16, 2 fp32; MODE: EpiMode) so
-// that each instantiation carries only its own store path - one kernel with every path inlined is ~190 KB of SASS and
-// thrashes the instruction cache.
+// Epilogue variants are compile-time (OUT_F32: fp32 vs 16-bit output; RESID: 0 none, 1 16-bit, 2 fp32; MODE: EpiMode)
+// so that each instantiation carries only its own store path - one kernel with every path inlined thrashes the
+// instruction cache.
 template <int BLOCK_N, int RESID, int DIRECT>
 using KernelCfg = TileCfg<BLOCK_N, DIRECT == 2 ? 8 * epi_tma_nbuf(RESID) * kEpiBufBytes : kEpiStageBytes>;
 
 // DIRECT: 0 = staged epilogue (registers -> per-warp shared staging -> coalesced per-thread global accesses),
 //         1 = row per thread straight to global memory (A/B aid, not dispatched),
 //         2 = TMA epilogue (EPI_NORMAL only): residual boxes arrive by TMA, results leave by TMA store.
-template <int BLOCK_N, int OUT_F32, int RESID, int MODE, int DIRECT, int PAIR>
+template <int BLOCK_N, int OUT_F32, int RESID, int MODE, int DIRECT>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmMaps maps,
                                                               const __grid_constant__ GemmArgs args) {
     using Cfg = KernelCfg<BLOCK_N, RESID, DIRECT>;
-    constexpr int kEpiBytes = Cfg::kSmemBytes - Cfg::kRingBytes - kSmemFixed;
+    constexpr int kEpiBytes = Cfg::kSmemBytes - Cfg::kRingBytes - kAccBytes - kSmemFixed;
+    constexpr int stage_bytes = Cfg::kStageBytes;
+    constexpr int nstages = Cfg::kStages;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw_addr = smem_u32(smem_raw);
     uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);  // 1024 B alignment for SWIZZLE_128B
+    const int worker = static_cast<int>(blockIdx.x);
+    const int n_workers = static_cast<int>(gridDim.x);
 
-    // CTA-pair mode (args.cluster == 2, launched as clusters of 2 = the two SMs of a TPC): the pair computes the
-    // M-adjacent tiles (2p, 2p+1) of one N tile with ONE tcgen05.mma.cta_group::2 (256 x BLOCK_N x 16) per k step.
-    // Each CTA stages its own 128-row A tile and only HALF of the weight tile (the MMA reads the other half from the
-    // peer's shared memory), so an SM's shared-memory traffic per k block drops from (A + B) filled + (A + B) read to
-    // (A + B/2) + (A + B/2): with both operands in shared memory the single-CTA kernel is bound by exactly that
-    // bandwidth (tensor pipe 68 % active, profiles/README_r01.md).  Protocol: both producers' TMA bytes are counted on
-    // the LEADER's (rank 0) full barrier; the leader's MMA thread issues for the pair and its commits arrive on both
-    // CTAs' empty / accumulator-full barriers; both CTAs' epilogue warps release the accumulator on the leader's
-    // accumulator-empty barrier.
-    constexpr int cl = PAIR ? 2 : 1;  // pair kernels contain cta_group::2 instructions and must be launched as clusters
-    uint32_t crank = 0u;
-    if constexpr (PAIR) crank = cluster_ctarank();
-    const bool leader = crank == 0;
-    constexpr uint16_t kPairMask = 0x3;
-    const int worker = cl > 1 ? static_cast<int>(blockIdx.x) / cl : static_cast<int>(blockIdx.x);
-    const int n_workers = cl > 1 ? static_cast<int>(gridDim.x) / cl : static_cast<int>(gridDim.x);
-    const int stage_bytes = cl > 1 ? Cfg::kStageBytes2 : Cfg::kStageBytes;
-    const int nstages = cl > 1 ? Cfg::kStages2 : Cfg::kStages;
-
-    uint8_t* epi_stage = smem + Cfg::kRingBytes;  // same carve-up in both modes (either ring fits in kRingBytes)
+    float* acc_smem = reinterpret_cast<float*>(smem + Cfg::kRingBytes);
+    uint8_t* epi_stage = smem + Cfg::kRingBytes + kAccBytes;
     float* fin_w = reinterpret_cast<float*>(epi_stage + kEpiBytes);  // [4][64] weights of the fused final conv
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_stage + kEpiBytes + 1024);
     uint64_t* empty_bar = full_bar + 8;
-    uint64_t* tfull_bar = empty_bar + 8;
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-    [[maybe_unused]] uint64_t* rbar_base = tempty_bar + 3;  // TMA epilogue: [8 warps][4] residual-box barriers
+    [[maybe_unused]] uint64_t* rbar_base = empty_bar + 8;  // TMA epilogue: [8 warps][4] residual-box barriers
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -219,11 +187,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     if (threadIdx.x == 0) {
         for (int i = 0; i < nstages; ++i) {
             mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tfull_bar[i], 1);
-            mbar_init(&tempty_bar[i], 8 * cl);  // one arrive per epilogue warp (of both CTAs in pair mode)
+            mbar_init(&empty_bar[i], 8);  // one arrive per consumer warp
         }
         if constexpr (DIRECT == 2 && RESID != 0) {
             for (int i = 0; i < 32; ++i) mbar_init(&rbar_base[i], 1);
@@ -239,23 +203,10 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             }
         }
     }
-    if (warp == 1) {
-        if constexpr (PAIR) {
-            tmem_alloc_cg2(tmem_slot, Cfg::kTmemCols);
-            tmem_relinquish_cg2();
-        } else {
-            tmem_alloc(tmem_slot, Cfg::kTmemCols);
-            tmem_relinquish();
-        }
-    }
     if constexpr (MODE == EPI_CONVT_FINAL) {
-        if (threadIdx.x >= 64) fin_w[threadIdx.x - 64] = args.fin_w[threadIdx.x - 64];
+        if (threadIdx.x < 256) fin_w[threadIdx.x] = args.fin_w[threadIdx.x];
     }
-    tc_fence_before();
     __syncthreads();
-    if constexpr (PAIR) cluster_sync_all();  // the peer's barriers must be initialised before anything is signalled on them
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     // programmatic dependent launch: the prologue above overlapped the previous kernel's tail; operands, residuals and
     // the output buffer may only be touched from here on
     pdl_wait();
@@ -263,73 +214,39 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
 
     const int tiles_m = args.n_img * args.tiles_h * args.tiles_w;
     const int num_kb = args.ntaps * args.kpt;
-    // work units: tiles, or (pair of M tiles) x (N tile) in pair mode; a rank-1 CTA whose M tile does not exist
-    // ("ghost", odd tile counts) still stages its half of the weights and follows the barrier protocol, but loads no A
-    // and stores nothing (its accumulator rows are garbage)
-    const int total_units = cl > 1 ? ((tiles_m + cl - 1) / cl) * args.tiles_n : tiles_m * args.tiles_n;
-    auto unit_tile = [&](int u, bool& ghost) {
-        if (cl == 1) {
-            ghost = false;
-            return u;
-        }
-        const int mp = u / args.tiles_n, nt = u - mp * args.tiles_n;
-        const int mt = mp * cl + static_cast<int>(crank);
-        ghost = mt >= tiles_m;
-        return mt * args.tiles_n + nt;
-    };
+    const int total_units = tiles_m * args.tiles_n;
 
-    if (warp == 0) {
+    if (warp >= kProducerWarp) {
         // ------------------------------------------------------------------ TMA producer
-        if (lane == 0) {
+        setmaxnreg_dec<40>();
+        if (warp == kProducerWarp && lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
-            // pair mode: every TMA of the pair signals the leader's full barrier
-            uint32_t full0 = 0u;
-            if constexpr (PAIR) full0 = mapa_u32(&full_bar[0], 0);
             // TMA epilogue with a residual: the rows of the NEXT tile's residual go to L2 as one whole-tile request, so
             // that the epilogue warps' 64-byte boxes hit L2 instead of fetching DRAM piecemeal
             [[maybe_unused]] auto prefetch_resid = [&](int u2) {
                 if (u2 >= total_units) return;
-                bool gh;
-                const int t2 = unit_tile(u2, gh);
-                if (gh) return;
-                const TileCoord c2 = decode_tile(args, t2, BLOCK_N);
+                const TileCoord c2 = decode_tile(args, u2, BLOCK_N);
                 tma_prefetch_l2_4d(&maps.resid_pf, c2.n0, c2.w0, c2.h0, c2.img);
             };
             if constexpr (DIRECT == 2 && RESID != 0) {
                 if (args.epi_pf) prefetch_resid(worker);
             }
             for (int u = worker; u < total_units; u += n_workers) {
-                bool ghost;
-                const int tile = unit_tile(u, ghost);
-                const TileCoord tc = decode_tile(args, tile, BLOCK_N);
+                const TileCoord tc = decode_tile(args, u, BLOCK_N);
                 if constexpr (DIRECT == 2 && RESID != 0) {
                     if (args.epi_pf) prefetch_resid(u + n_workers);
                 }
-                // does the pair's rank-1 tile exist?  (the leader must know how many bytes to expect)
-                const bool peer_ghost = cl > 1 && ((u / args.tiles_n) * 2 + 1 >= tiles_m);
                 int tap = 0, cb = 0;
                 for (int kb = 0; kb < num_kb; ++kb) {
                     mbar_wait(&empty_bar[stage], phase ^ 1u);
                     uint8_t* sa = smem + stage * stage_bytes;
                     uint8_t* sb = sa + kABytes;
                     const ConvTap tp = args.taps[tap];
-                    if constexpr (PAIR) {
-                        if (leader)
-                            mbar_expect_tx(&full_bar[stage],
-                                           2 * Cfg::kStageBytes2 - (peer_ghost ? kABytes : 0));
-                        const uint32_t fb = full0 + static_cast<uint32_t>(stage) * 8u;
-                        if (!ghost)
-                            tma_load_4d_cg2(sa, &maps.a[tp.map], fb, cb * kBlockK, tc.w0 + tp.dw, tc.h0 + tp.dh, tc.img);
-                        // my half of the weight tile: rows n0 + rank * BLOCK_N/2 ...
-                        tma_load_4d_cg2(sb, &maps.b, fb, kb * kBlockK, tc.n0 + static_cast<int>(crank) * (BLOCK_N / 2), 0,
-                                        0);
-                    } else {
-                        mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-                        tma_load_4d(sa, &maps.a[tp.map], &full_bar[stage], cb * kBlockK, tc.w0 + tp.dw, tc.h0 + tp.dh,
-                                    tc.img);
-                        tma_load_4d(sb, &maps.b, &full_bar[stage], kb * kBlockK, tc.n0, 0, 0);
-                    }
+                    mbar_expect_tx(&full_bar[stage], Cfg::kStageBytes);
+                    tma_load_4d(sa, &maps.a[tp.map], &full_bar[stage], cb * kBlockK, tc.w0 + tp.dw, tc.h0 + tp.dh,
+                                tc.img);
+                    tma_load_4d(sb, &maps.b, &full_bar[stage], kb * kBlockK, tc.n0, 0, 0);
                     if (++cb == args.kpt) {
                         cb = 0;
                         ++tap;
@@ -341,60 +258,92 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                 }
             }
         }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer (pair mode: the leader only)
-        if (lane == 0 && (cl == 1 || leader)) {
-            constexpr uint32_t idesc = umma_idesc_op(kBlockM, BLOCK_N);
-            constexpr uint32_t idesc2 = umma_idesc_op(2 * kBlockM, BLOCK_N);
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            for (int u = worker; u < total_units; u += n_workers) {
-                mbar_wait(&tempty_bar[acc], acc_phase ^ 1u);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + static_cast<uint32_t>(acc * BLOCK_N);
-                for (int kb = 0; kb < num_kb; ++kb) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    const uint32_t a_addr = smem_u32(smem + stage * stage_bytes);
-                    const uint64_t da = umma_desc_sw128(a_addr);
-                    const uint64_t db = umma_desc_sw128(a_addr + kABytes);
-#pragma unroll
-                    for (int k = 0; k < kBlockK / 16; ++k) {
-                        // advance 16 bf16 = 32 B inside the 128 B swizzle row: +2 in the (addr >> 4) field
-                        if constexpr (PAIR)
-                            umma_op_cg2(d_tmem, da + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k),
-                                          idesc2, (kb | k) != 0 ? 1u : 0u);
-                        else
-                            umma_op(d_tmem, da + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k),
-                                      idesc, (kb | k) != 0 ? 1u : 0u);
-                    }
-                    // frees the smem slot once these MMAs have read it (on both CTAs of a pair)
-                    if constexpr (PAIR) umma_commit_cg2(&empty_bar[stage], kPairMask);
-                    else umma_commit(&empty_bar[stage]);
-                    if (++stage == nstages) {
-                        stage = 0;
-                        phase ^= 1u;
-                    }
-                }
-                // accumulator complete
-                if constexpr (PAIR) umma_commit_cg2(&tfull_bar[acc], kPairMask);
-                else umma_commit(&tfull_bar[acc]);
-                acc ^= 1;
-                if (acc == 0) acc_phase ^= 1u;
-            }
-        }
     } else {
-        // ------------------------------------------------------------------ epilogue (warps 2..9)
-        // Two warps per TMEM lane quadrant; each owns every other 32-column chunk.  Values go
-        // TMEM -> registers (row per thread) -> bias/residual/activation -> per-warp shared staging -> coalesced
-        // 16-byte global stores (4 lanes per 64-byte row segment), so DRAM sees whole sectors.
+        // ------------------------------------------------------------------ consumers (warps 0..7)
+        // Warpgroup wg computes tile rows [64 wg, 64 wg + 64) with wgmma, then runs the epilogue on them: warp wl of the
+        // warpgroup stores the 32 rows of quadrant q (row per thread) and, of every 64-column slice, the 32-column chunk
+        // of its set (the CONVT_FINAL epilogue pairs chunks instead, see below).  Values go registers -> slice buffer ->
+        // bias/residual/activation -> TMA boxes (residual in by cp.async.bulk.tensor, result out by TMA store) or, for
+        // the plans the TMA path does not cover, per-warp shared staging and coalesced 16-byte global accesses (4 lanes
+        // per 64-byte row segment), so DRAM sees whole sectors.
+        setmaxnreg_inc<232>();   // 2 x 128 x 232 + 128 x 40 <= 64 K registers
+        const int wg = warp >> 2, wl = warp & 3;
+        const int q = 2 * wg + (wl & 1);   // 32-row quadrant of the tile this warp stores
+        const int wset = wl >> 1;          // 0 or 1
+        float* acc_buf = acc_smem + wg * 64 * kAccPitch;
+        const float* my_acc = acc_buf + ((wl & 1) * 32 + lane) * kAccPitch;
+        float acc[BLOCK_N / 2];
+#pragma unroll
+        for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
+        int ring_stage = 0;
+        uint32_t ring_phase = 0;
+        // the whole K loop of one tile: one wgmma group per K block, one group kept in flight; a stage is released
+        // once the group after it has been issued and its own group has completed
+        auto mma_tile = [&]() {
+            const uint32_t a_off = static_cast<uint32_t>(wg * 64 * 128);
+            int prev = -1;
+            for (int kb = 0; kb < num_kb; ++kb) {
+                mbar_wait(&full_bar[ring_stage], ring_phase);
+                const uint32_t a_addr = smem_u32(smem + ring_stage * stage_bytes);
+                const uint64_t da = wgmma_desc_sw128(a_addr + a_off);
+                const uint64_t db = wgmma_desc_sw128(a_addr + kABytes);
+                reg_fence(acc);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < kBlockK / 16; ++k)
+                    // advance 16 elements = 32 B inside the 128 B swizzle row: +2 in the (addr >> 4) field
+                    wgmma_ss<BLOCK_N>(acc, da + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k),
+                                      (kb | k) != 0 ? 1u : 0u);
+                wgmma_commit();
+                wgmma_wait<1>();
+                reg_fence(acc);
+                if (prev >= 0) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+                }
+                prev = ring_stage;
+                if (++ring_stage == nstages) {
+                    ring_stage = 0;
+                    ring_phase ^= 1u;
+                }
+            }
+            wgmma_wait<0>();
+            reg_fence(acc);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        };
+        // accumulator columns [64 s, 64 s + 64) -> the warpgroup's slice buffer, once every warp is done with the last
+        // slice (register indices must be compile-time: the slice is selected by predicate)
+        auto dump_slice = [&](int s) {
+            named_bar_sync(1 + wg, 128);
+            const int r0 = wl * 16 + (lane >> 2), c2 = (lane & 3) * 2;
+#pragma unroll
+            for (int j = 0; j < BLOCK_N / 8; ++j) {
+                if ((j >> 3) == s) {
+                    float* p = acc_buf + r0 * kAccPitch + (j & 7) * 8 + c2;
+                    *reinterpret_cast<float2*>(p) = make_float2(acc[4 * j], acc[4 * j + 1]);
+                    *reinterpret_cast<float2*>(p + 8 * kAccPitch) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+                }
+            }
+            named_bar_sync(1 + wg, 128);
+        };
+        // this thread's row of 32-column chunk c (after dump_slice(c / 2))
+        auto load_chunk = [&](int c, float (&f)[32]) {
+            const float4* a4 = reinterpret_cast<const float4*>(my_acc + (c & 1) * 32);
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const float4 x = a4[j];
+                f[4 * j + 0] = x.x;
+                f[4 * j + 1] = x.y;
+                f[4 * j + 2] = x.z;
+                f[4 * j + 3] = x.w;
+            }
+        };
         if constexpr (DIRECT == 2) {
             // ---- TMA epilogue.  A "pass" is one warp's share of 64 output bytes per row: 32 tile rows x CPP columns,
             // one 2 KB box.  The warp's passes (units -> its chunks -> passes) form one sequence that indexes a ring of
-            // NBUF boxes: residual boxes are loaded LOOK passes ahead by lane 0 (so their latency hides behind the MMAs
-            // of the tile and the passes in between), a thread adds its own row in place, and lane 0 hands the box to a
+            // NBUF boxes: residual boxes are loaded LOOK passes ahead by lane 0 (the first ones of a tile while its MMAs
+            // run), a thread adds its own row in place, and lane 0 hands the box to a
             // TMA store.  Rows / columns outside the tensor are zero-filled on load and dropped on store by the hardware.
             static_assert(MODE == EPI_NORMAL, "TMA epilogue: plain stores only");
             static_assert(RESID == 0 || (RESID == 2) == (OUT_F32 != 0), "TMA epilogue: residual and output boxes match");
@@ -402,13 +351,11 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             constexpr int LOOK = NBUF - 1;
             constexpr int CPP = OUT_F32 ? 16 : 32;
             constexpr int NPASS = 32 / CPP;
-            const int q = warp & 3;            // TMEM lane quadrant this warp may access
-            const int wset = (warp - 2) >> 2;  // 0 or 1
             const int bw_mask = (1 << args.bw_log2) - 1;
             const int qw = (q * 32) & bw_mask;          // where the quadrant's 32 rows start inside the BH x BW patch
             const int qh = (q * 32) >> args.bw_log2;
-            uint8_t* bufs = epi_stage + (warp - 2) * (NBUF * kEpiBufBytes);
-            [[maybe_unused]] uint64_t* rbar = rbar_base + (warp - 2) * 4;
+            uint8_t* bufs = epi_stage + warp * (NBUF * kEpiBufBytes);
+            [[maybe_unused]] uint64_t* rbar = rbar_base + warp * 4;
             const int sw = args.epi_swz ? ((lane >> 1) & 3) : 0;   // SWIZZLE_64B: 16 B chunk ^= (row / 2) % 4
             const int row_off = lane * 64;
             // residual prefetch cursor (lane 0 only): position (unit, chunk, pass) of the next box to load
@@ -416,12 +363,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             [[maybe_unused]] TileCoord pf_tc{};
             [[maybe_unused]] auto pf_seek = [&]() {   // moves the cursor to the next existing pass at or after its position
                 while (pf_u < total_units) {
-                    bool gh;
-                    const int tile = unit_tile(pf_u, gh);
-                    if (!gh) {
-                        pf_tc = decode_tile(args, tile, BLOCK_N);
-                        if (pf_c < BLOCK_N / 32 && pf_tc.n0 + pf_c * 32 + pf_p * CPP < args.Cout) return;
-                    }
+                    pf_tc = decode_tile(args, pf_u, BLOCK_N);
+                    if (pf_c < BLOCK_N / 32 && pf_tc.n0 + pf_c * 32 + pf_p * CPP < args.Cout) return;
                     pf_c = wset;       // nothing (left) for this warp in the unit
                     pf_p = 0;
                     pf_u += n_workers;
@@ -451,38 +394,19 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                 }
             }
             int gc = 0;  // passes consumed so far (warp-uniform)
-            int acc = 0;
-            uint32_t acc_phase = 0;
             for (int u = worker; u < total_units; u += n_workers) {
-                bool ghost;
-                const int tile = unit_tile(u, ghost);
-                if (ghost) {  // nothing to store: just hand the accumulator buffer back to the leader
-                    mbar_wait(&tfull_bar[acc], acc_phase);
-                    tc_fence_after();
-                    tc_fence_before();
-                    __syncwarp();
-                    if constexpr (PAIR) {
-                        if (lane == 0) mbar_arrive_cluster(mapa_u32(&tempty_bar[acc], 0));
-                    }
-                    acc ^= 1;
-                    if (acc == 0) acc_phase ^= 1u;
-                    continue;
-                }
-                const TileCoord tc = decode_tile(args, tile, BLOCK_N);
-                mbar_wait(&tfull_bar[acc], acc_phase);
-                tc_fence_after();
-                const uint32_t t_addr =
-                    tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(acc * BLOCK_N);
+                const TileCoord tc = decode_tile(args, u, BLOCK_N);
+                mma_tile();
 #pragma unroll 1
-                for (int c = wset; c < BLOCK_N / 32; c += 2) {
+                for (int c = 0; c < BLOCK_N / 32; ++c) {
                     const int col0 = tc.n0 + c * 32;
-                    if (col0 >= args.Cout) break;  // warp-uniform
-                    uint32_t v[32];
-                    tmem_ld_32x32(t_addr + static_cast<uint32_t>(c * 32), v);
-                    tmem_ld_wait();
+                    if ((c & 1) == 0) {
+                        if (col0 >= args.Cout) break;  // warpgroup-uniform
+                        dump_slice(c >> 1);
+                    }
+                    if ((c & 1) != wset || col0 >= args.Cout) continue;
                     float f[32];
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
+                    load_chunk(c, f);
                     if (args.bias != nullptr) {
                         if (col0 + 32 <= args.Cout) {
                             const float4* b4 = reinterpret_cast<const float4*>(args.bias + col0);
@@ -579,14 +503,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                         }
                     }
                 }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) {
-                    if constexpr (PAIR) mbar_arrive_cluster(mapa_u32(&tempty_bar[acc], 0));  // the leader's MMA thread waits
-                    else mbar_arrive(&tempty_bar[acc]);
-                }
-                acc ^= 1;
-                if (acc == 0) acc_phase ^= 1u;
             }
             if (lane == 0) bulk_wait_read<0>();   // shared memory must outlive the last stores' reads
             __syncwarp();
@@ -597,31 +513,13 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         constexpr int NPASS = 32 / CPP;
         constexpr int OESZ = OUT_F32 ? 4 : 2;
         constexpr int RESZ = (RESID == 2) ? 4 : 2;
-        const int q = warp & 3;            // TMEM lane quadrant this warp may access
-        const int wset = (warp - 2) >> 2;  // 0 or 1
         const int row = q * 32 + lane;
         const int bw_mask = (1 << args.bw_log2) - 1;
-        uint8_t* stage = epi_stage + (warp - 2) * (32 * kStagePitch);
+        uint8_t* stage = epi_stage + warp * (32 * kStagePitch);
         uint8_t* my_row = stage + lane * kStagePitch;
         const int piece = lane & 3;
-        int acc = 0;
-        uint32_t acc_phase = 0;
         for (int u = worker; u < total_units; u += n_workers) {
-            bool ghost;
-            const int tile = unit_tile(u, ghost);
-            if (ghost) {  // nothing to store: just hand the accumulator buffer back to the leader
-                mbar_wait(&tfull_bar[acc], acc_phase);
-                tc_fence_after();
-                tc_fence_before();
-                __syncwarp();
-                if constexpr (PAIR) {
-                    if (lane == 0) mbar_arrive_cluster(mapa_u32(&tempty_bar[acc], 0));
-                }
-                acc ^= 1;
-                if (acc == 0) acc_phase ^= 1u;
-                continue;
-            }
-            const TileCoord tc = decode_tile(args, tile, BLOCK_N);
+            const TileCoord tc = decode_tile(args, u, BLOCK_N);
             const int hh = tc.h0 + (row >> args.bw_log2);
             const int ww = tc.w0 + (row & bw_mask);
             const bool row_ok = (hh < args.Ho) && (ww < args.Wo);
@@ -635,20 +533,21 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                 c_w[it] = tc.w0 + (rr & bw_mask);
                 c_ok[it] = (c_h[it] < args.Ho) && (c_w[it] < args.Wo);
             }
-            mbar_wait(&tfull_bar[acc], acc_phase);
-            tc_fence_after();
-            const uint32_t t_addr =
-                tmem_base + (static_cast<uint32_t>(q * 32) << 16) + static_cast<uint32_t>(acc * BLOCK_N);
+            mma_tile();
             [[maybe_unused]] float dots[4] = {0.f, 0.f, 0.f, 0.f};
             [[maybe_unused]] float rm_m = -INFINITY, rm_s = 0.f;   // EPI_ROWMAX: running (max, sum exp, arg-max)
             [[maybe_unused]] int rm_i = 0x7fffffff;
 #pragma unroll 1
             for (int c = 0; c < BLOCK_N / 32; ++c) {
-                if (((kFin ? (c >> 1) : c) & 1) != wset) continue;  // chunk belongs to the other warp set
                 const int col0 = tc.n0 + c * 32;
-                if (col0 >= args.Cout) break;  // warp-uniform
-                // residual prefetch: issue the coalesced global loads of every pass of this chunk before touching TMEM so
-                // that their latency overlaps the accumulator load and the bias math
+                if ((c & 1) == 0) {
+                    if (col0 >= args.Cout) break;  // warpgroup-uniform
+                    dump_slice(c >> 1);
+                }
+                if (((kFin ? (c >> 1) : c) & 1) != wset) continue;  // chunk belongs to the other warp set
+                if (col0 >= args.Cout) continue;
+                // residual prefetch: issue the coalesced global loads of every pass of this chunk before reading the
+                // accumulator so that their latency overlaps the accumulator load and the bias math
                 // DIRECT variant: the thread's own row segment (32 columns) straight from / to global memory
                 [[maybe_unused]] uint4 dres[RESID == 2 ? 8 : 4];
                 if constexpr (RESID != 0 && !kFin && DIRECT == 1) {
@@ -685,12 +584,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                         }
                     }
                 }
-                uint32_t v[32];
-                tmem_ld_32x32(t_addr + static_cast<uint32_t>(c * 32), v);
-                tmem_ld_wait();
                 float f[32];
-#pragma unroll
-                for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
+                load_chunk(c, f);
                 if (args.bias != nullptr) {
                     if (col0 + 32 <= args.Cout) {
                         const float4* b4 = reinterpret_cast<const float4*>(args.bias + col0);
@@ -989,26 +884,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                     reinterpret_cast<float4*>(args.out)[pixo * args.ldc + (tc.n0 / BLOCK_N) * 2 + wset] = o;
                 }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                if constexpr (PAIR) mbar_arrive_cluster(mapa_u32(&tempty_bar[acc], 0));  // the leader's MMA thread waits
-                else mbar_arrive(&tempty_bar[acc]);
-            }
-            acc ^= 1;
-            if (acc == 0) acc_phase ^= 1u;
         }
         }  // legacy (DIRECT 0 / 1) epilogue
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if constexpr (PAIR) cluster_sync_all();  // no CTA leaves while its peer can still use its memories / barriers
-    if (warp == 1) {
-        __syncwarp();
-        tc_fence_after();
-        if constexpr (PAIR) tmem_dealloc_cg2(tmem_base, Cfg::kTmemCols);
-        else tmem_dealloc(tmem_base, Cfg::kTmemCols);
     }
 }
 
@@ -1055,7 +932,7 @@ int make_tmap_op_4d(CUtensorMap* m, const void* base, const uint64_t dims[4], co
 }
 
 // Output / residual tensor [n_img][Ho][Wo][Cout] (row pitch ld elements) as a 4-D map whose box is one epilogue warp's
-// share of a pass: 64 bytes of columns x the 32 tile rows of a TMEM lane quadrant (32 consecutive pixels of a row when
+// share of a pass: 64 bytes of columns x the 32 tile rows of a quadrant (32 consecutive pixels of a row when
 // the patch is at least 32 wide, else 32 / BW full patch rows).
 static int make_tmap_epi(CUtensorMap* m, const void* base, int f32, const GemmArgs& a, int Cout, long long ld, int swz,
                          int tile_cols = 0) {
@@ -1075,7 +952,7 @@ static int make_tmap_epi(CUtensorMap* m, const void* base, int f32, const GemmAr
         bx[2] = (cuuint32_t)(128 / bw);
         swz = 0;
     }
-    // L2 promotion of the box fetches: 128 B by default; YTK_EPI_L2P=256 measured no better (profiles/README_r02.md)
+    // L2 promotion of the box fetches: 128 B by default; YTK_EPI_L2P=256 opts into 256 B
     static const bool l2_256 = getenv("YTK_EPI_L2P") != nullptr && getenv("YTK_EPI_L2P")[0] == '2';
     cuuint32_t est[4] = {1, 1, 1, 1};
     const CUtensorMapDataType dt = f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
@@ -1127,14 +1004,12 @@ static int pick_bw_log2(int Ho, int Wo) {
     return best;
 }
 
-static int finish_plan(GemmPlan* plan, const void* w_packed, int Ktot, int Cout, const Epilogue& e,
-                       bool allow_pair = false) {
+static int finish_plan(GemmPlan* plan, const void* w_packed, int Ktot, int Cout, const Epilogue& e) {
     GemmArgs& a = plan->args;
     plan->block_n = pick_block_n(Cout);
     static const bool no_shrink = getenv("YTK_NO_SHRINK") != nullptr;  // debugging aid
-    // YTK_WAVE_MODEL=1: choose the N tile of few-wave problems by waves x relative tile time.  Measured and rejected
-    // (profiles/README_r02.md): 64-wide tiles cost 0.75, not 0.56, of a 128-wide tile (3200 x 768 x 3072: 59.8 vs
-    // 45.0 us), the AR loop went from 62.4 to 66.0 ms.  Kept as an experiment switch only.
+    // YTK_WAVE_MODEL=1: choose the N tile of few-wave problems by waves x relative tile time (experiment switch: the
+    // relative tile times below are a model, not a measurement of this kernel).
     static const bool no_wave_model = getenv("YTK_WAVE_MODEL") == nullptr;
     if (e.mode != EPI_CONVT_FINAL && !no_shrink) {
         const int m_tiles = a.n_img * a.tiles_h * a.tiles_w;
@@ -1145,7 +1020,7 @@ static int finish_plan(GemmPlan* plan, const void* w_packed, int Ktot, int Cout,
             while (plan->block_n > 64 && tiles_at(plan->block_n) < sms) plan->block_n >>= 1;
         } else {
             // a handful of waves: the last, partly filled wave costs as much as a full one (3200 decode rows x 768
-            // columns = 150 tiles of 128 columns on 148 SMs = two waves).  Pick the N tile with the smallest
+            // columns = 150 tiles of 128 columns on 132 SMs = two waves).  Pick the N tile with the smallest
             // waves x (relative time of one tile of that width); ties go to the wider tile.
             int best = plan->block_n;
             double best_cost = 1e30;
@@ -1201,21 +1076,9 @@ static int finish_plan(GemmPlan* plan, const void* w_packed, int Ktot, int Cout,
         set_error("gemm plan: SHUFFLE2X needs Cout/4 to be a multiple of 32 (Cout=%d)", Cout);
         return 1;
     }
-    // Large plain GEMMs (the PARSeq linears) run as CTA pairs (gemm_tc_kernel PAIR: tcgen05.mma.cta_group::2), worth it
-    // once every SM has several tiles to work through.  Measured on the bench shapes: PARSeq encoder 62.0 -> 60.9 ms;
-    // the DBNet convolutions that would qualify are epilogue / HBM bound and LOSE 5 % to the pair's lock step, so
-    // convolutions stay single-CTA.  YTK_NO_CLUSTER=1 switches pair mode off, YTK_PAIR_CONV=1 on for convs (A/B aids).
-    const int tiles_m = a.n_img * a.tiles_h * a.tiles_w;
-    const int tiles = tiles_m * a.tiles_n;
-    static const bool no_cluster = getenv("YTK_NO_CLUSTER") != nullptr;
-    static const bool pair_conv = getenv("YTK_PAIR_CONV") != nullptr;
-    a.cluster = (!no_cluster && (allow_pair || pair_conv) && e.mode != EPI_CONVT_FINAL && e.mode != EPI_ROWMAX &&
-                 tiles >= 4 * num_sms() &&
-                 tiles_m >= 8)
-                    ? 2
-                    : 1;
+    const int tiles = a.n_img * a.tiles_h * a.tiles_w * a.tiles_n;
     // TMA epilogue: plain stores whose residual (if any) has the output's element size; 16-byte aligned bases
-    // and rows whose extent is a multiple of 16 bytes: measured on B200, a TMA store clips the box at the tensor's inner
+    // and rows whose extent is a multiple of 16 bytes: a TMA store clips the box at the tensor's inner
     // extent in 16-byte units (Cout = 7119 fp32 columns: column 7119 of a 7120-wide buffer was written)
     a.epi_tma = 0;
     a.epi_swz = 0;
@@ -1224,9 +1087,7 @@ static int finish_plan(GemmPlan* plan, const void* w_packed, int Ktot, int Cout,
         ((long long)Cout * (e.out_f32 ? 4 : 2)) % 16 == 0 &&
         (reinterpret_cast<uintptr_t>(e.out) & 15) == 0 && (reinterpret_cast<uintptr_t>(e.resid) & 15) == 0) {
         static const bool no_swz = getenv("YTK_EPI_SWZ") != nullptr && getenv("YTK_EPI_SWZ")[0] == '0';
-        // whole-tile L2 prefetch of the residual one tile ahead: opt-in (YTK_EPI_PF=1).  Measured (call 19, one box):
-        // proj 10.40 ms with it vs 9.37-9.66 without, fc2 20.6 vs 19.0-19.3, DBNet residual 1x1 convs 1.60 vs 1.42 ms -
-        // the 64-byte boxes are not what limits these kernels.
+        // whole-tile L2 prefetch of the residual one tile ahead: opt-in (YTK_EPI_PF=1).
         static const bool no_pf = !(getenv("YTK_EPI_PF") != nullptr && getenv("YTK_EPI_PF")[0] == '1');
         a.epi_tma = 1;
         a.epi_swz = no_swz ? 0 : 1;
@@ -1240,10 +1101,10 @@ static int finish_plan(GemmPlan* plan, const void* w_packed, int Ktot, int Cout,
             plan->maps.resid_pf = plan->maps.out;
         }
     }
-    // weights: [Cout][Ktot] bf16, K-major; in cluster mode a CTA fetches block_n / cluster rows per k block
+    // weights: [Cout][Ktot] 16-bit, K-major
     uint64_t dims[4] = {(uint64_t)Ktot, (uint64_t)Cout, 1, 1};
     uint64_t strides[3] = {(uint64_t)Ktot * 2, (uint64_t)Ktot * 2 * Cout, (uint64_t)Ktot * 2 * Cout};
-    uint32_t box[4] = {(uint32_t)kBlockK, (uint32_t)(plan->block_n / a.cluster), 1, 1};
+    uint32_t box[4] = {(uint32_t)kBlockK, (uint32_t)plan->block_n, 1, 1};
     if (make_tmap_op_4d(&plan->maps.b, w_packed, dims, strides, box)) return 1;
     plan->grid = tiles < num_sms() ? tiles : num_sms();
     if (plan->grid < 1) plan->grid = 1;
@@ -1356,7 +1217,7 @@ int gemm_plan_create(GemmPlan* plan, const void* A, long long lda, int M, int K,
     if (make_tmap_op_4d(&plan->maps.a[0], A, dims, strides, box)) return 1;
     for (int i = 1; i < 4; ++i) plan->maps.a[i] = plan->maps.a[0];
     plan->flops = 2.0 * M * (double)N * K;
-    return finish_plan(plan, Wt, K, N, e, /*allow_pair=*/true);
+    return finish_plan(plan, Wt, K, N, e);
 }
 
 int stem_plan_create(GemmPlan* plan, const void* in_padded, int N, int Hn, int Wn, const void* w_packed,
@@ -1416,11 +1277,11 @@ void gemm_plan_set_m(GemmPlan* plan, int M) {
     if (plan->grid < 1) plan->grid = 1;
 }
 
-template <int BLOCK_N, int OUT_F32, int RESID, int MODE, int DIRECT, int PAIR>
-static int launch_variant3(const GemmPlan* plan, cudaStream_t stream) {
+template <int BLOCK_N, int OUT_F32, int RESID, int MODE, int DIRECT>
+static int launch_variant2(const GemmPlan* plan, cudaStream_t stream) {
     using Cfg = KernelCfg<BLOCK_N, RESID, DIRECT>;
     static unsigned long long attr_done = 0;   // per device (a process may hold handles on several GPUs)
-    auto kern = gemm_tc_kernel<BLOCK_N, OUT_F32, RESID, MODE, DIRECT, PAIR>;
+    auto kern = gemm_tc_kernel<BLOCK_N, OUT_F32, RESID, MODE, DIRECT>;
     if (first_launch_on_device(&attr_done)) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
         if (e != cudaSuccess) {
@@ -1428,71 +1289,22 @@ static int launch_variant3(const GemmPlan* plan, cudaStream_t stream) {
             return 1;
         }
     }
-    if constexpr (PAIR != 0) {
-        // persistent grid = every cluster the device can hold at once (clusters cannot straddle GPCs, so this can be
-        // fewer than num_sms / 2), capped by the number of work units
-        const int cl = plan->args.cluster;
-        cudaLaunchConfig_t cfg = {};
-        cudaLaunchAttribute attr[2];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = cl;
-        attr[0].val.clusterDim.y = 1;
-        attr[0].val.clusterDim.z = 1;
-        cfg.blockDim = dim3(kThreads);
-        cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-        cfg.stream = stream;
-        cfg.attrs = attr;
-        cfg.numAttrs = 1 + pdl_launch_attr(attr + 1);
-        static int max_clusters = -1;
-        if (max_clusters < 0) {
-            cfg.gridDim = dim3((num_sms() / cl) * cl);
-            int n = 0;
-            cudaError_t e = cudaOccupancyMaxActiveClusters(&n, kern, &cfg);
-            if (e != cudaSuccess || n < 1) {
-                set_error("cudaOccupancyMaxActiveClusters: %s (n=%d)", cudaGetErrorString(e), n);
-                return 1;
-            }
-            max_clusters = n;
-        }
-        const GemmArgs& a = plan->args;
-        const int tiles_m = a.n_img * a.tiles_h * a.tiles_w;
-        const int units = ((tiles_m + cl - 1) / cl) * a.tiles_n;
-        const int clusters = units < max_clusters ? units : max_clusters;
-        cfg.gridDim = dim3(clusters * cl);
-        cudaError_t e = cudaLaunchKernelEx(&cfg, kern, plan->maps, plan->args);
-        count_launch();
-        if (e != cudaSuccess) {
-            set_error("gemm_tc_kernel<%d,%d,%d,%d,%d> cluster launch: %s", BLOCK_N, OUT_F32, RESID, MODE, DIRECT,
-                      cudaGetErrorString(e));
-            return 1;
-        }
-        return 0;
-    } else {
-        cudaLaunchConfig_t cfg = {};
-        cudaLaunchAttribute attr[1];
-        cfg.gridDim = dim3(plan->grid);
-        cfg.blockDim = dim3(kThreads);
-        cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-        cfg.stream = stream;
-        cfg.attrs = attr;
-        cfg.numAttrs = pdl_launch_attr(attr);
-        cudaError_t e = cudaLaunchKernelEx(&cfg, kern, plan->maps, plan->args);
-        count_launch();
-        if (e != cudaSuccess) {
-            set_error("gemm_tc_kernel<%d,%d,%d,%d,%d> launch: %s", BLOCK_N, OUT_F32, RESID, MODE, DIRECT,
-                      cudaGetErrorString(e));
-            return 1;
-        }
-        return 0;
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute attr[1];
+    cfg.gridDim = dim3(plan->grid);
+    cfg.blockDim = dim3(kThreads);
+    cfg.dynamicSmemBytes = Cfg::kSmemBytes;
+    cfg.stream = stream;
+    cfg.attrs = attr;
+    cfg.numAttrs = pdl_launch_attr(attr);
+    cudaError_t e = cudaLaunchKernelEx(&cfg, kern, plan->maps, plan->args);
+    count_launch();
+    if (e != cudaSuccess) {
+        set_error("gemm_tc_kernel<%d,%d,%d,%d,%d> launch: %s", BLOCK_N, OUT_F32, RESID, MODE, DIRECT,
+                  cudaGetErrorString(e));
+        return 1;
     }
-}
-
-template <int BLOCK_N, int OUT_F32, int RESID, int MODE, int DIRECT>
-static int launch_variant2(const GemmPlan* plan, cudaStream_t stream) {
-    if constexpr (MODE != EPI_CONVT_FINAL) {
-        if (plan->args.cluster > 1) return launch_variant3<BLOCK_N, OUT_F32, RESID, MODE, DIRECT, 1>(plan, stream);
-    }
-    return launch_variant3<BLOCK_N, OUT_F32, RESID, MODE, DIRECT, 0>(plan, stream);
+    return 0;
 }
 
 // Epilogue path per plan: the TMA epilogue (args.epi_tma, set by finish_plan) or the staged one.
@@ -1513,7 +1325,7 @@ static int launch_bn(const GemmPlan* plan, cudaStream_t stream) {
         set_error("CONVT_FINAL needs BLOCK_N = 256");
         return 1;
     }
-    if (a.mode == EPI_ROWMAX) return launch_variant3<BLOCK_N, 1, 0, EPI_ROWMAX, 0, 0>(plan, stream);
+    if (a.mode == EPI_ROWMAX) return launch_variant2<BLOCK_N, 1, 0, EPI_ROWMAX, 0>(plan, stream);
     if (a.mode == EPI_SHUFFLE2X) {
         if (resid == 0 && !a.out_f32) return launch_variant<BLOCK_N, 0, 0, EPI_SHUFFLE2X>(plan, stream);
         if (resid == 0 && a.out_f32) return launch_variant<BLOCK_N, 1, 0, EPI_SHUFFLE2X>(plan, stream);
@@ -1535,7 +1347,7 @@ namespace {
 struct ProfRec {
     cudaEvent_t a, b;
     double flops;
-    int pixels, cout, k, block_n, cluster, mode, act, resid, out_f32, ntaps;   // shape of the launch (YTK_GEMM_DUMP)
+    int pixels, cout, k, block_n, mode, act, resid, out_f32, ntaps;   // shape of the launch (YTK_GEMM_DUMP)
 };
 std::mutex g_prof_mu;
 bool g_prof_on = false;
@@ -1582,12 +1394,12 @@ int gemm_profile_end(double* flops, double* ms, long long* launches) {
     if (launches) *launches = (long long)g_prof.size();
     if (const char* path = getenv("YTK_GEMM_DUMP")) {      // per-launch table of the window for shape-level analysis
         if (FILE* fp = fopen(path, "a")) {
-            fprintf(fp, "pixels,cout,k,ntaps,block_n,cluster,mode,act,resid,out_f32,flops,ms\n");
+            fprintf(fp, "pixels,cout,k,ntaps,block_n,mode,act,resid,out_f32,flops,ms\n");
             for (ProfRec& r : g_prof) {
                 float e = 0.f;
                 cudaEventElapsedTime(&e, r.a, r.b);
-                fprintf(fp, "%d,%d,%d,%d,%d,%d,%d,%d,%d,%d,%.0f,%.6f\n", r.pixels, r.cout, r.k, r.ntaps, r.block_n,
-                        r.cluster, r.mode, r.act, r.resid, r.out_f32, r.flops, e);
+                fprintf(fp, "%d,%d,%d,%d,%d,%d,%d,%d,%d,%.0f,%.6f\n", r.pixels, r.cout, r.k, r.ntaps, r.block_n,
+                        r.mode, r.act, r.resid, r.out_f32, r.flops, e);
             }
             fclose(fp);
         }
@@ -1610,7 +1422,6 @@ int gemm_plan_launch(const GemmPlan* plan, cudaStream_t stream) {
             rec.k = g.kpt * 64;
             rec.ntaps = g.ntaps;
             rec.block_n = plan->block_n;
-            rec.cluster = g.cluster;
             rec.mode = g.mode;
             rec.act = g.act;
             rec.resid = g.resid ? (g.resid_f32 ? 2 : 1) : 0;

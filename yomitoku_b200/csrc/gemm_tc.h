@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution / linear layer on tcgen05 tensor cores (sm_100a).
+// Implicit-GEMM convolution / linear layer on wgmma tensor cores (sm_90a).
 //
 //   D[pixel, co] = act( sum_{tap, ci} A[pixel + tap, ci] * W[co, tap, ci] + bias[co] (+ resid[pixel, co]) )
 //
@@ -6,8 +6,9 @@
 // patch (BH*BW = 128), and a filter tap is just a shifted TMA box whose out-of-bounds part is zero-filled by the
 // hardware (= convolution padding).  Stride-2 convolutions read through up to four "phase" tensor maps (even/odd
 // rows x even/odd columns).  A plain linear layer is the degenerate case H = 1, W = M, one tap.
-// W is a K-major bf16 matrix [Cout][taps*Cin] read through a 2-D TMA map.  Accumulators live in TMEM (fp32),
-// double-buffered so the epilogue of tile i overlaps the MMAs of tile i+1 (persistent CTAs, one per SM).
+// W is a K-major bf16 matrix [Cout][taps*Cin] read through a 2-D TMA map.  Accumulators live in the registers of two
+// consumer warpgroups (fp32); the TMA producer fills the K ring for tile i+1 while they store tile i (persistent CTAs,
+// one per SM).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -72,8 +73,6 @@ struct GemmArgs {
     int epi_swz;                   // 1: the TMA epilogue's boxes are 64-byte swizzled (conflict-free row accesses)
     int epi_pf;                    // 1: the TMA producer prefetches the next tile's residual rows into L2 (whole rows of
                                    // the tile in one request instead of 64-byte pieces fetched from DRAM one by one)
-    int cluster;                   // 1, or 2: CTA pairs (thread-block cluster) work on M-adjacent tiles of one N tile
-                                   // and multicast the weight tile - each CTA fetches half of it from L2
 };
 
 struct Epilogue {
@@ -102,7 +101,7 @@ struct GemmPlan {
     GemmMaps maps;
     GemmArgs args;
     int block_n;
-    int grid;      // CTAs to launch (cluster mode: set at launch from the occupancy query)
+    int grid;      // CTAs to launch
     double flops;  // 2*M*N*K of the true problem (for roofline accounting)
 };
 
@@ -128,7 +127,7 @@ int make_tmap_op_4d(CUtensorMap* m, const void* base, const uint64_t dims[4], co
                       const uint32_t box[4]);
 
 // Launch attribute set for kernels that call pdl_wait() (ptx.cuh): programmatic stream serialization when YTK_PDL=1
-// (off by default: measured slower, see gemm_tc.cu).  Returns the number of attributes written to attr[0..].
+// (off by default, see gemm_tc.cu).  Returns the number of attributes written to attr[0..].
 int pdl_launch_attr(cudaLaunchAttribute* attr);
 void set_error(const char* fmt, ...);
 const char* last_error();

@@ -1,5 +1,5 @@
 // PARSeq recognizer (ViT encoder + 1-layer two-stream decoder, greedy AR decode + one refinement pass) as a launch
-// plan of tcgen05 GEMMs, tensor-core flash attention and small fused kernels.  Replaces reference
+// plan of wgmma GEMMs, tensor-core flash attention and small fused kernels.  Replaces reference
 // models/parseq.py:159-311 and models/layers/parseq_transformer.py:69-244 for inference.
 //
 // What differs from the reference *implementation* while keeping its *results* (SURVEY.md Appendix A):
@@ -524,10 +524,9 @@ int ParseqEngine::forward(const ParseqBatch& b, int* ids_out, float* probs_out, 
         // content K/V cache [row][position 0..S-1][2D]; position 0 (<bos>) is the same for every row
         if (launch_bcast_rows(m->ckv0, ckv, 2 * D * 2, (long long)S * 2 * D * 2, B, st)) return 1;
         // The decode loop can run as two PARTS (row ranges that end on a group boundary), each on its own stream, so
-        // that one part's GEMMs overlap the other part's HBM-bound attention.  MEASURED (3200 rows, 101 steps): 72.6 ms
-        // split vs 61.0 ms unsplit - the step's kernels are latency-bound, halving M does not halve their time and the
-        // persistent GEMM CTAs (200 KB of shared memory each) do not co-reside - so it is OFF unless YTK_AR_SPLIT_MIN=<rows>
-        // asks for it (the GPU tests run both ways).  Parts share nothing but read-only weights / memory K/V.
+        // that one part's GEMMs overlap the other part's HBM-bound attention.  The step's kernels are latency-bound: halving
+        // M does not halve their time, and the persistent GEMM CTAs (over 200 KB of shared memory each) do not co-reside -
+        // so it is OFF unless YTK_AR_SPLIT_MIN=<rows> asks for it (the GPU tests run both ways).  Parts share nothing but read-only weights / memory K/V.
         struct Part {
             int r0, rows, g0, ng;
             ArState a;

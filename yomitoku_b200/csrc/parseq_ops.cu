@@ -1,4 +1,4 @@
-// Non-GEMM kernels of the PARSeq recognizer (sm_100a): patchify, LayerNorm, flash attention over packed ragged
+// Non-GEMM kernels of the PARSeq recognizer (sm_90a): patchify, LayerNorm, flash attention over packed ragged
 // sequences, the decoder's small attention kernels and the device-side greedy / EOS / repetition control logic that
 // removes every host sync from the AR loop.  Reference: models/parseq.py:133-311, models/layers/parseq_transformer.py.
 #include "parseq_ops.h"
@@ -26,7 +26,7 @@ static cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
 }
 
 // =================================================================================================== patchify
-// Replaces timm PatchEmbed.proj's im2col (reference parseq_transformer.py:220-227): the conv itself is a tcgen05 GEMM;
+// Replaces timm PatchEmbed.proj's im2col (reference parseq_transformer.py:220-227): the conv itself is a wgmma GEMM;
 // this kernel writes its A operand and seeds the fp32 residual stream with the cropped positional embedding.
 // Normalisation = ToTensor + Normalize(0.5, 0.5) (data/dataset.py:57-62); pixels right of the stored canvas are the
 // collate padding value -1.0 (text_recognizer.py:146-156).
@@ -115,7 +115,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(float* __restrict__ x, i
                                                         int period, const int* __restrict__ add_row0_dev,
                                                         int add_row0, int writeback) {
     pdl_wait();   // (no early launch_dependents: this grid runs in many waves and a dependent persistent GEMM CTA that
-                  // becomes resident early takes its SM away from the remaining waves - measured: AR loop +17 ms)
+                  // becomes resident early takes its SM away from the remaining waves)
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     if (warp >= M) return;
@@ -453,21 +453,19 @@ int launch_flash_attention(const void* Q, long long ldq, long long q_rows, const
                            int heads, int head_dim, int masked, cudaStream_t st, int impl) {
     if (nseq <= 0) return 0;
     if (impl == 0) {
-        // YTK_ATTN=legacy: the round-1 mma.sync kernel; YTK_ATTN=vswap: tcgen05 kernel with the other V descriptor
-        // YTK_ATTN=legacy: the round-1 mma.sync kernel; ptmem: tcgen05 kernel with the P tile in tensor memory (A operand
-        // from TMEM - correct, but measured 17 % slower than staging P in shared memory: the S buffer is then held until
-        // the P V product has read it); default: tcgen05 kernel, P in shared memory
+        // YTK_ATTN=legacy: the round-1 mma.sync kernel; default: the wgmma kernel
         static const int env_impl = [] {
             const char* e = getenv("YTK_ATTN");
-            if (e && e[0] == 'l') return 1;
-            if (e && e[0] == 'p') return 4;
-            return 2;
+            return (e && e[0] == 'l') ? 1 : 2;
         }();
         impl = env_impl;
     }
-    if (impl >= 2)   // 2: P in smem, 3: P in smem + swapped V descriptor (debug), 4: P in TMEM
-        return launch_attention_tc(Q, ldq, q_rows, K, V, ldkv, kv_rows, O, ldo, seqs, nseq, heads, head_dim, masked,
-                                   impl == 3 ? 1 : (impl == 4 ? 2 : 0), st);
+    if (impl != 1 && impl != 2) {
+        set_error("flash attention: impl %d unknown (1 = mma.sync, 2 = wgmma)", impl);
+        return 1;
+    }
+    if (impl == 2)
+        return launch_attention_tc(Q, ldq, q_rows, K, V, ldkv, kv_rows, O, ldo, seqs, nseq, heads, head_dim, masked, st);
     // 128-query tiles (8 warps) halve the K/V re-reads of the typical 92..200-token crop; short sequences keep 64
     const int qt = max_q_len > 64 ? 128 : 64;
     dim3 grid((max_q_len + qt - 1) / qt, heads, nseq);
@@ -507,7 +505,7 @@ constexpr int kMaxMem = 800;
 //   mode 1  cross: q = qc[row],        keys = the row's encoder memory K/V (stride 2D), nk = ntok
 // One warp per (row, head), no block-level synchronisation.  LPK lanes share a key (each owns CPL 16-byte chunks of the
 // head dim), 32/LPK key subsets run side by side, so every lane keeps several independent 16-byte loads in flight -
-// the step is HBM-bound on exactly these reads (profiles/README_r01.md).
+// the step is HBM-bound on exactly these reads.
 template <int HD>
 __global__ void __launch_bounds__(128) single_query_attn_kernel(int mode, const op_t* __restrict__ qsrc,
                                                                 const op_t* __restrict__ kv, int B, int S,
@@ -520,7 +518,7 @@ __global__ void __launch_bounds__(128) single_query_attn_kernel(int mode, const 
     constexpr int NSUB = 32 / LPK;                // key subsets
     __shared__ float sP[4][kMaxMem];
     pdl_wait();   // (no early launch_dependents: this grid runs in many waves and a dependent persistent GEMM CTA that
-                  // becomes resident early takes its SM away from the remaining waves - measured: AR loop +17 ms)
+                  // becomes resident early takes its SM away from the remaining waves)
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int wid = blockIdx.x * 4 + warp;
     if (wid >= B * heads) return;
@@ -706,7 +704,7 @@ __global__ void __launch_bounds__(256) ar_control_kernel(const float* __restrict
     __shared__ float red[8];
     __shared__ int s_last;
     pdl_wait();   // (no early launch_dependents: this grid runs in many waves and a dependent persistent GEMM CTA that
-                  // becomes resident early takes its SM away from the remaining waves - measured: AR loop +17 ms)
+                  // becomes resident early takes its SM away from the remaining waves)
     const int row = blockIdx.x;
     const int i = *a.step;
     const int j = i + 1;

@@ -42,15 +42,15 @@ struct SeqDesc {
 };
 // masked = 0: plain softmax(QK^T)V.  masked = 1: PARSeq refinement self-attention - key j is visible to query i iff
 // (i < 2 || j <= i) && j < kpad (reference parseq.py:267-297; rows 0 and 1 of the causal mask are cleared).
-// q_rows / kv_rows: number of rows of the Q and K/V matrices (TMA extents of the tcgen05 path, attn_tc.cu).
-// impl: 0 = default (attn_tc_kernel: tcgen05 + TMEM + TMA; YTK_ATTN=legacy selects the mma.sync kernel), 1 = legacy
-// mma.sync kernel, 2 / 3 = tcgen05 kernel with the V-descriptor convention forced (debugging aid).
+// q_rows / kv_rows: number of rows of the Q and K/V matrices (TMA extents of the wgmma path, attn_tc.cu).
+// impl: 0 = default (attn_tc_kernel: wgmma + TMA; YTK_ATTN=legacy selects the mma.sync kernel), 1 = legacy mma.sync
+// kernel, 2 = wgmma kernel.
 int launch_flash_attention(const void* Q, long long ldq, long long q_rows, const void* K, const void* V, long long ldkv,
                            long long kv_rows, void* O, long long ldo, const SeqDesc* seqs, int nseq, int max_q_len,
                            int heads, int head_dim, int masked, cudaStream_t st, int impl = 0);
 int launch_attention_tc(const void* Q, long long ldq, long long q_rows, const void* K, const void* V, long long ldkv,
                         long long kv_rows, void* O, long long ldo, const SeqDesc* seqs, int nseq, int heads,
-                        int head_dim, int masked, int vswap, cudaStream_t st);
+                        int head_dim, int masked, cudaStream_t st);
 
 // AR attention, one query per (row, head) (single_query_attn_kernel):
 //  self : step i = *step_dev, q = q_shared[i], keys 0..i of the row's content K/V cache [row][S positions][2D] -> out[row]

@@ -1,5 +1,5 @@
 // RT-DETRv2 (PResNet-50d backbone + HybridEncoder + 6-layer deformable decoder) as a static launch plan: every
-// convolution and linear layer is a tcgen05 implicit GEMM (gemm_tc.cu), the two kinds of self-attention run on the tcgen05
+// convolution and linear layer is a wgmma implicit GEMM (gemm_tc.cu), the two kinds of self-attention run on the wgmma
 // attention kernel (attn_tc.cu), the rest are the small kernels of rtdetr_ops.cu.  Replaces, for inference, reference
 // models/rtdetr.py:9-22 = layers/rtdetr_backbone.py:245-334 + layers/rtdetr_hybrid_encoder.py:216-410 +
 // layers/rtdetrv2_decoder.py:446-815 (the layout parser and the table structure recognizer share the architecture).

@@ -2,7 +2,7 @@
 
 Mirrors reference src/yomitoku/layout_parser.py:23-274 - same catalog names (`rtdetrv2`, `rtdetrv2v2`), constructor
 kwargs, `preprocess` / `postprocess` / `filtering_elements` / `__call__` contract and result schema.  The model forward
-runs as sm_100a kernels (csrc/rtdetr_engine.cu behind ytk_rtdetr_forward_f32); the PIL resize in front of it and the
+runs as sm_90a kernels (csrc/rtdetr_engine.cu behind ytk_rtdetr_forward_f32); the PIL resize in front of it and the
 containment filters behind it are host code like in the reference.  `infer_onnx` is accepted and ignored.
 """
 import cv2

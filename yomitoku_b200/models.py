@@ -3,7 +3,7 @@
 They keep the surface the reference's modules touch from outside (SURVEY.md section 8b "model-level seam"):
 `model(tensor)`, `.eval()`, `.to(device)`, `.state_dict()/.load_state_dict()` (reference key set, Appendix C),
 `.from_pretrained(repo, cfg=cfg)`, `PARSeq.tokenizer`, `PARSeq.refine_iters`, `PARSeq.export_onnx` - but the forward
-pass is the hand-written sm_100a engine behind the C ABI (include/yomitoku_b200.h).  There is no CPU fallback: a
+pass is the hand-written sm_90a engine behind the C ABI (include/yomitoku_b200.h).  There is no CPU fallback: a
 forward without the CUDA library and a GPU raises.
 
 Reference: src/yomitoku/models/dbnet_plus.py:233-246, src/yomitoku/models/parseq.py:49-311.
@@ -82,7 +82,7 @@ class _DeviceModel:
     def _require_cuda(self):
         if not torch.cuda.is_available():
             raise _lib.YtkError(
-                "%s runs only on a CUDA device (sm_100a): no GPU is visible and there is no CPU fallback on the "
+                "%s runs only on a CUDA device (sm_90a): no GPU is visible and there is no CPU fallback on the "
                 "hot path" % type(self).__name__)
 
     @classmethod
@@ -700,7 +700,7 @@ def _rtdetr_random_state_dict(num_classes, seed=0):
 class RTDETRv2(_DeviceModel):
     """reference models/rtdetr.py:9-22 (PResNet-50d + HybridEncoder + RTDETRTransformerv2, eval).  `model(tensor)` takes
     the (n, 3, 640, 640) fp32 tensor in [0, 1] that LayoutParser / TableStructureRecognizer.preprocess produce and returns
-    {"pred_logits": (n, 300, C), "pred_boxes": (n, 300, 4)} on the tensor's device.  The forward is the sm_100a engine
+    {"pred_logits": (n, 300, C), "pred_boxes": (n, 300, 4)} on the tensor's device.  The forward is the sm_90a engine
     behind ytk_rtdetr_forward_f32 (csrc/rtdetr_engine.cu); there is no CPU fallback."""
 
     def __init__(self, cfg=None, seed=0):

@@ -23,8 +23,8 @@ from .text_recognizer import plan_mini_batches
 
 _W = {}
 # Cost of a mini-batch group for the cross-rank balancer, in encoder-token units: the encoder and the attention over the
-# encoder memory scale with the group's tokens, the AR steps / refinement / head with its rows.  Measured on B200
-# (profiles/README_r02.md, 101 AR steps): ~0.31 us per token and ~12.5 us per row, i.e. one row costs about 40 tokens.
+# encoder memory scale with the group's tokens, the AR steps / refinement / head with its rows; with 101 AR steps one
+# row costs about as much as 40 tokens.
 ROW_COST_TOKENS = 40
 TRACE = None     # set to a list to collect (stage, thread name, t0, t1) tuples (scripts/gpu_trace_e2e.py)
 

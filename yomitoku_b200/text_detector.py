@@ -2,7 +2,7 @@
 
 Mirrors reference src/yomitoku/text_detector.py:26-146 - same catalog names (`dbnet`, `dbnetv2`, `dbnetv2_1`),
 constructor kwargs, `preprocess` / `postprocess` / `__call__` contract and result schema.  The model forward (and,
-for pages that only need decimation, the resize + normalisation in front of it) runs as sm_100a kernels; contour
+for pages that only need decimation, the resize + normalisation in front of it) runs as sm_90a kernels; contour
 extraction / unclip stay on the host like the reference (SURVEY.md R3).  `infer_onnx` is accepted and ignored:
 ONNX / multi-backend dispatch is out of scope for this path.
 """
