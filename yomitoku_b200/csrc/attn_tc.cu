@@ -4,16 +4,22 @@
 // (reference models/parseq.py:264-299: cross-attention over the encoder memory, and the masked self-attention over the
 // content stream whose mask has rows 0 and 1 cleared, SURVEY.md Appendix A1).
 //
-// One persistent CTA per SM works through its list of units (sequence, head, 128-query tile); it owns a Q tile and a
-// 2-stage K/V ring in shared memory:
-//   warp 8   lane 0 : TMA producer - Q tile once per unit, K/V tiles of 64 keys (SWIZZLE_128B boxes)
-//   warpgroups 0, 1 : 64 queries each.  S = Q K^T by wgmma (both operands K-major in shared memory) into registers,
+// One persistent CTA per SM works through its list of units (sequence, head, 64-query tile).  Every consumer
+// warpgroup owns whole units: unit n of the CTA belongs to warpgroup n % 3, which has its own Q buffer and barrier
+// phases and computes no rows outside its tile.  Up to three consecutive units of one (sequence, head) pair form a
+// chunk; the chunk's K/V tiles are loaded once into a shared ring and read by every warpgroup of the chunk.
+//   warp 12  lane 0 : TMA producer - per chunk the Q tile of each unit, then the K/V tiles of 64 keys (SWIZZLE_128B
+//                     boxes).  Every consumer warp passes every K/V tile in order, also those it does not read (not in
+//                     the chunk, or its causal range ends earlier).  The ring is deeper than a chunk at the bench's
+//                     lengths: the next chunk's loads run while this one computes.
+//   warpgroups 0-2  : 64 queries each.  S = Q K^T by wgmma (both operands K-major in shared memory) into registers,
 //                     mask + running max (lazy rescale: the reference max moves only when it grows by > 2^8) + exp2 in
 //                     the accumulator layout, P packed to fp16 A fragments in registers, O += P V by wgmma with A from
 //                     registers and V as MN-major B operand (the tile is stored exactly as TMA delivers [keys][hd]
-//                     rows); after the last key tile O / l -> global.
-// While one warpgroup is on the CUDA cores (softmax) the tensor core works for the other.  The P V product always
-// runs its four 16-key steps; steps past the last visible key read a zero tile instead of V.
+//                     rows); after the last key tile O / l -> global.  S of tile t is issued together with P V of tile
+//                     t-1, and the softmax of tile t runs while that P V is on the tensor core (one S and one P register
+//                     set: two S sets do not fit the 160 registers a thread of three consumer warpgroups gets).
+// The P V product always runs its four 16-key steps; steps past the last visible key read a zero tile instead of V.
 #include <cuda.h>
 
 #include "gemm_tc.h"
@@ -24,10 +30,13 @@ namespace ytk {
 
 namespace {
 
-constexpr int kAtQ = 128;        // queries per unit (two warpgroups of 64)
+constexpr int kAtQ = 64;         // queries per unit (one warpgroup)
 constexpr int kAtKV = 64;        // keys per tile
-constexpr int kAtThreads = 288;  // 2 consumer warpgroups, 1 producer warp
-constexpr int kAtStages = 2;
+constexpr int kAtWG = 3;         // consumer warpgroups
+constexpr int kAtProducerWarp = 4 * kAtWG;
+constexpr int kAtThreads = 128 * (kAtWG + 1);
+constexpr int kAtMaxStages = 8;
+constexpr int kAtMaxSmem = 227 * 1024;
 constexpr float kRescaleThreshold = 8.f;  // log2 units: P stays <= 2^8, well inside fp16
 
 struct alignas(64) AttnMaps {
@@ -47,16 +56,17 @@ template <int HD>
 struct AtCfg {
     static constexpr int NB = (HD + 63) / 64;                 // 64-element (128 B) column blocks per row
     static constexpr int NO = NB * 64;                        // columns of the O accumulator
-    static constexpr int kQBytes = NB * kAtQ * 128;
+    static constexpr int kQBytes = NB * kAtQ * 128;           // one warpgroup's Q tile
     static constexpr int kKBytes = NB * kAtKV * 128;          // one K (or V) tile
     static constexpr int kStageBytes = 2 * kKBytes;
     static constexpr int kZeroBytes = NB * 2048;               // 16 zero V rows per column block
-    static constexpr int kSmemBytes =
-        kQBytes + kAtStages * kStageBytes + kZeroBytes + 256 /*barriers*/ + 1024 /*alignment slack*/;
-};
-
-struct Bars {
-    uint64_t q_full, q_empty, kv_full[kAtStages], kv_empty[kAtStages];
+    static constexpr int kFixedBytes = kAtWG * kQBytes + kZeroBytes + 256 /*barriers*/ + 1024 /*alignment slack*/;
+    static constexpr int kStages = (kAtMaxSmem - kFixedBytes) / kStageBytes < kAtMaxStages
+                                       ? (kAtMaxSmem - kFixedBytes) / kStageBytes
+                                       : kAtMaxStages;
+    static constexpr int kSmemBytes = kFixedBytes + kStages * kStageBytes;
+    // a warpgroup holds K/V tile t-1 while it waits for t
+    static_assert(kStages >= 2, "attention: K/V ring too shallow");
 };
 
 struct Unit {
@@ -66,72 +76,67 @@ struct Unit {
     int q0;       // index of the tile's first query inside its sequence
     int k_row;    // first key row in K / V
     int k_end;    // keys this tile can see
-    int k_len, kpad;
     int nt;       // key tiles
-    int head;
 };
 
 template <int MASKED>
-__device__ __forceinline__ Unit make_unit(const SeqDesc& sd, int head, int qt, long long ldkv) {
+__device__ __forceinline__ int pair_keys(const SeqDesc& sd) {
+    return MASKED ? min(sd.k_len, sd.kpad) : sd.k_len;
+}
+
+template <int MASKED>
+__device__ __forceinline__ Unit make_unit(const SeqDesc& sd, int qt, long long ldkv) {
     Unit u;
     u.q0 = qt * kAtQ;
     u.q_row = sd.q_off + u.q0;
     u.o_row = sd.o_off + u.q0;
     u.rows = min(kAtQ, sd.q_len - u.q0);
     u.k_row = static_cast<int>(sd.k_base / ldkv);
-    u.k_len = sd.k_len;
-    u.kpad = sd.kpad;
-    int k_end = sd.k_len;
-    if (MASKED) {
-        k_end = min(k_end, sd.kpad);
-        if (u.q0 >= 2) k_end = min(k_end, u.q0 + kAtQ);  // causal rows stop at their own index
-    }
+    int k_end = pair_keys<MASKED>(sd);
+    if (MASKED && u.q0 >= 2) k_end = min(k_end, u.q0 + kAtQ);  // causal rows stop at their own index
     u.k_end = k_end;
     u.nt = (k_end + kAtKV - 1) / kAtKV;
-    u.head = head;
     return u;
 }
 
-// The units of one CTA in processing order: the CTA owns the (sequence, head) pairs p = cta, cta + ncta, ...; inside a
-// pair the query tiles in ascending order, back to back, so that the pair's K / V tiles are still in L2 for the second
-// tile.  Every role of the CTA walks the same sequence.
+// The chunks of one CTA in processing order: the CTA owns the (sequence, head) pairs p = cta, cta + ncta, ...; a
+// pair's query tiles are cut into chunks of up to kAtWG consecutive tiles, run back to back so that the pair's K / V
+// is still in L2 for a second chunk.  Units are numbered across the CTA (n0 = number of the chunk's first unit);
+// kc0 counts the K/V tiles the ring received before the chunk.  Every role of the CTA walks the same sequence.
 template <int MASKED>
-struct UnitIter {
-    int p, qt, nqt, head, W, npairs;
+struct ChunkIter {
+    int p, W, npairs, head, nqt, qt0, cnt, n0, ntiles;
+    uint32_t kc0;
     SeqDesc sd;
-    Unit u;
     const AttnArgs* a;
-    __device__ __forceinline__ void load_pair() {
-        const int seq = p / a->heads;
-        head = p - seq * a->heads;
-        sd = a->seqs[seq];
-        nqt = (sd.q_len + kAtQ - 1) / kAtQ;
-    }
-    // positions on the CTA's first unit; false when it has none
     __device__ __forceinline__ bool begin(const AttnArgs* args, int cta, int ncta, int npairs_) {
         a = args;
         W = ncta;
         npairs = npairs_;
-        p = cta;
-        qt = -1;
-        if (p >= npairs) return false;
-        load_pair();
+        p = cta - ncta;
+        nqt = qt0 = cnt = n0 = ntiles = 0;
+        kc0 = 0;
         return next();
     }
     __device__ __forceinline__ bool next() {
-        for (;;) {
-            ++qt;
-            while (qt >= nqt) {
-                p += W;
-                qt = 0;
-                if (p >= npairs) return false;
-                load_pair();
-            }
-            u = make_unit<MASKED>(sd, head, qt, a->ldkv);
-            if (u.nt <= 0) continue;
-            return true;
+        n0 += cnt;
+        kc0 += static_cast<uint32_t>(ntiles);
+        qt0 += cnt;
+        while (qt0 >= nqt) {
+            p += W;
+            if (p >= npairs) return false;
+            const int seq = p / a->heads;
+            head = p - seq * a->heads;
+            sd = a->seqs[seq];
+            nqt = (sd.q_len > 0 && pair_keys<MASKED>(sd) > 0) ? (sd.q_len + kAtQ - 1) / kAtQ : 0;
+            qt0 = 0;
         }
+        cnt = min(kAtWG, nqt - qt0);
+        ntiles = 0;
+        for (int i = 0; i < cnt; ++i) ntiles = max(ntiles, unit(i).nt);
+        return true;
     }
+    __device__ __forceinline__ Unit unit(int i) const { return make_unit<MASKED>(sd, qt0 + i, a->ldkv); }
 };
 
 __device__ __forceinline__ float fast_exp2(float x) {
@@ -146,21 +151,27 @@ __global__ void __launch_bounds__(kAtThreads, 1) attn_tc_kernel(const __grid_con
     using Cfg = AtCfg<HD>;
     constexpr int NB = Cfg::NB;
     constexpr int NO = Cfg::NO;
+    constexpr int S = Cfg::kStages;
     extern __shared__ uint8_t at_smem_raw[];
     const uint32_t raw_addr = smem_u32(at_smem_raw);
     uint8_t* smem = at_smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
     uint8_t* sQ = smem;
-    uint8_t* sKV = smem + Cfg::kQBytes;
-    uint8_t* sZero = sKV + kAtStages * Cfg::kStageBytes;
-    Bars& b = *reinterpret_cast<Bars*>(sZero + Cfg::kZeroBytes);
+    uint8_t* sKV = smem + kAtWG * Cfg::kQBytes;
+    uint8_t* sZero = sKV + S * Cfg::kStageBytes;
+    uint64_t* q_full = reinterpret_cast<uint64_t*>(sZero + Cfg::kZeroBytes);
+    uint64_t* q_empty = q_full + kAtWG;
+    uint64_t* kv_full = q_empty + kAtWG;
+    uint64_t* kv_empty = kv_full + S;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
-        mbar_init(&b.q_full, 1);
-        mbar_init(&b.q_empty, 8);   // one arrive per consumer warp
-        for (int i = 0; i < kAtStages; ++i) {
-            mbar_init(&b.kv_full[i], 1);
-            mbar_init(&b.kv_empty[i], 8);
+        for (int i = 0; i < kAtWG; ++i) {
+            mbar_init(&q_full[i], 1);
+            mbar_init(&q_empty[i], 4);       // one arrive per warp of the owning warpgroup
+        }
+        for (int i = 0; i < S; ++i) {
+            mbar_init(&kv_full[i], 1);
+            mbar_init(&kv_empty[i], 4 * kAtWG);  // one arrive per consumer warp
         }
         fence_mbar_init();
         tma_prefetch_desc(&maps.q);
@@ -175,30 +186,55 @@ __global__ void __launch_bounds__(kAtThreads, 1) attn_tc_kernel(const __grid_con
     const int npairs = args.nseq * args.heads;
     const int cta = static_cast<int>(blockIdx.x), ncta = static_cast<int>(gridDim.x);
 
-    if (warp < 8) {
+    if (warp < kAtProducerWarp) {
         // ------------------------------------------------------------------ MMA + softmax + epilogue, 64 queries
+        setmaxnreg_inc<160>();   // 3 x 128 x 160 + 128 x 32 = 64 K registers
         const int wg = warp >> 2, wl = warp & 3;
-        const int r_in = wg * 64 + wl * 16 + (lane >> 2);   // tile row of this thread's first row (second: + 8)
-        const int cq = (lane & 3) * 2;                      // first of the thread's two columns in every 8-column block
-        const uint32_t q_addr = smem_u32(sQ) + static_cast<uint32_t>(wg * 64 * 128);
-        uint32_t nu = 0, ck = 0;
-        UnitIter<MASKED> it;
-        for (bool more = it.begin(&args, cta, ncta, npairs); more; more = it.next(), ++nu) {
-            const Unit u = it.u;
+        const int r_in = wl * 16 + (lane >> 2);   // tile row of this thread's first row (second: + 8)
+        const int cq = (lane & 3) * 2;            // first of the thread's two columns in every 8-column block
+        const uint32_t q_addr = smem_u32(sQ + wg * Cfg::kQBytes);
+        // K/V tiles of the chunk that this warpgroup does not read: it still observes every fill of every stage in
+        // order (a phase-parity wait is only unambiguous when the waiter has seen the previous phase) and counts itself
+        // done with the tile
+        auto pass_tiles = [&](uint32_t c, uint32_t end) {
+            for (; c < end; ++c) {
+                mbar_wait(&kv_full[c % S], (c / S) & 1u);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&kv_empty[c % S]);
+            }
+        };
+        ChunkIter<MASKED> it;
+        for (bool more = it.begin(&args, cta, ncta, npairs); more; more = it.next()) {
+            int i = wg - it.n0 % kAtWG;
+            if (i < 0) i += kAtWG;
+            if (i >= it.cnt) {
+                pass_tiles(it.kc0, it.kc0 + it.ntiles);
+                continue;
+            }
+            const int n = it.n0 + i;   // unit number inside the CTA
+            const Unit u = it.unit(i);
+            const uint32_t kc0 = it.kc0;
             float m_ref[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
             float o[NO / 2];
 #pragma unroll
-            for (int i = 0; i < NO / 2; ++i) o[i] = 0.f;
-            mbar_wait(&b.q_full, nu & 1u);
-            for (int t = 0; t < u.nt; ++t, ++ck) {
-                const uint32_t st = ck % kAtStages;
-                mbar_wait(&b.kv_full[st], (ck / kAtStages) & 1u);
+            for (int j = 0; j < NO / 2; ++j) o[j] = 0.f;
+            float s[32];
+            uint32_t pa[4][4];
+            float factor[2];
+
+            auto release_kv = [&](int t) {   // K / V tile t consumed by this warp
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&kv_empty[(kc0 + t) % S]);
+            };
+            auto release_q = [&]() {         // the unit's last S is done: the Q tile may be replaced
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&q_empty[wg]);
+            };
+            // ---- S = Q K^T (64 queries x 64 keys) of key tile t, one wgmma group
+            auto issue_s = [&](int t) {
+                const uint32_t c = kc0 + t, st = c % S;
+                mbar_wait(&kv_full[st], (c / S) & 1u);
                 const uint32_t k_addr = smem_u32(sKV + st * Cfg::kStageBytes);
-                const uint32_t v_addr = k_addr + Cfg::kKBytes;
-                // ---- S = Q K^T (64 queries x 64 keys)
-                float s[32];
-#pragma unroll
-                for (int i = 0; i < 32; ++i) s[i] = 0.f;
                 reg_fence(s);
                 wgmma_fence();
 #pragma unroll
@@ -208,27 +244,41 @@ __global__ void __launch_bounds__(kAtThreads, 1) attn_tc_kernel(const __grid_con
                     wgmma_ss<64>(s, da, db, j != 0 ? 1u : 0u);
                 }
                 wgmma_commit();
-                wgmma_wait<0>();
-                reg_fence(s);
-                if (t == u.nt - 1) {   // the Q tile is consumed: the producer may load the next unit's
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&b.q_empty);
+            };
+            // ---- O += P V of key tile t, one wgmma group.  All four 16-key steps are issued (a wgmma under a branch
+            // is serialised); a step past the last visible key has P = 0 and reads the zero tile instead of V rows that
+            // belong to no sequence of this unit (their contents need not be finite)
+            auto issue_pv = [&](int t) {
+                const uint32_t v_addr = smem_u32(sKV + ((kc0 + t) % S) * Cfg::kStageBytes) + Cfg::kKBytes;
+                const int ksteps = (min(kAtKV, u.k_end - t * kAtKV) + 15) >> 4;
+                reg_fence(o);
+                wgmma_fence();
+#pragma unroll
+                for (int ks = 0; ks < 4; ++ks) {
+                    const bool live = ks < ksteps;
+                    const uint64_t db = live ? wgmma_desc_sw128_mn(v_addr + ks * 2048, kAtKV * 128)
+                                             : wgmma_desc_sw128_mn(smem_u32(sZero), 2048);
+                    wgmma_rs<NO>(o, pa[ks], db, 1u);
                 }
-                // ---- mask, scale, tile max of both rows (a row is spread over the 4 lanes of a quad)
+                wgmma_commit();
+            };
+            // ---- softmax of key tile t on S: mask, scale, running max, l; S becomes P = exp2(S - m) in place.  O is
+            // not touched (the previous P V may still be running): its rescale by `factor` follows the wait.
+            auto softmax = [&](int t) {
+                // tile max of both rows (a row is spread over the 4 lanes of a quad)
                 const int key0 = t * kAtKV;
                 float mt[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                    const int h = (i >> 1) & 1;
-                    const int key = key0 + (i >> 2) * 8 + cq + (i & 1);
+                for (int j = 0; j < 32; ++j) {
+                    const int h = (j >> 1) & 1;
+                    const int key = key0 + (j >> 2) * 8 + cq + (j & 1);
                     const int qi = u.q0 + r_in + 8 * h;   // query index inside the sequence
                     bool vis = key < u.k_end;
                     if (MASKED) vis = vis && ((qi < 2) || (key <= qi));
-                    const float v = vis ? s[i] * args.scale_log2 : -INFINITY;
-                    s[i] = v;
+                    const float v = vis ? s[j] * args.scale_log2 : -INFINITY;
+                    s[j] = v;
                     mt[h] = fmaxf(mt[h], v);
                 }
-                float factor[2];
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                     mt[h] = fmaxf(mt[h], __shfl_xor_sync(0xffffffffu, mt[h], 1));
@@ -241,12 +291,6 @@ __global__ void __launch_bounds__(kAtThreads, 1) attn_tc_kernel(const __grid_con
                         l_run[h] *= factor[h];
                     }
                 }
-                if (factor[0] != 1.f || factor[1] != 1.f) {
-#pragma unroll
-                    for (int i = 0; i < NO / 2; ++i) o[i] *= factor[(i >> 1) & 1];
-                }
-                // ---- P = exp2(S - m) as fp16 A fragments: k step ks covers keys 16 ks .. 16 ks + 15
-                uint32_t pa[4][4];
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
                     const float m_use = (m_ref[h] == -INFINITY) ? 0.f : m_ref[h];
@@ -256,29 +300,50 @@ __global__ void __launch_bounds__(kAtThreads, 1) attn_tc_kernel(const __grid_con
                         const float p0 = fast_exp2(s[4 * j + 2 * h] - m_use);  // exp2(-inf) = 0
                         const float p1 = fast_exp2(s[4 * j + 2 * h + 1] - m_use);
                         ls += p0 + p1;
-                        pa[j >> 1][(j & 1) * 2 + h] = pack_op(p0, p1);
+                        s[4 * j + 2 * h] = p0;
+                        s[4 * j + 2 * h + 1] = p1;
                     }
                     l_run[h] += ls;
                 }
-                // ---- O += P V.  All four 16-key steps are issued (a wgmma under a branch is serialised); a step past
-                // the last visible key has P = 0 and reads the zero tile instead of V rows that belong to no sequence
-                // of this unit (their contents need not be finite)
-                const int ksteps = (min(kAtKV, u.k_end - key0) + 15) >> 4;
-                reg_fence(o);
-                wgmma_fence();
+            };
+            // ---- P as fp16 A fragments (k step ks covers keys 16 ks .. 16 ks + 15), O rescaled to the new max
+            auto pack_rescale = [&]() {
 #pragma unroll
-                for (int ks = 0; ks < 4; ++ks) {
-                    const bool live = ks < ksteps;
-                    const uint64_t db = live ? wgmma_desc_sw128_mn(v_addr + ks * 2048, kAtKV * 128)
-                                             : wgmma_desc_sw128_mn(smem_u32(sZero), 2048);
-                    wgmma_rs<NO>(o, pa[ks], db, 1u);
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) pa[j >> 1][(j & 1) * 2 + h] = pack_op(s[4 * j + 2 * h], s[4 * j + 2 * h + 1]);
+                if (factor[0] != 1.f || factor[1] != 1.f) {
+#pragma unroll
+                    for (int j = 0; j < NO / 2; ++j) o[j] *= factor[(j >> 1) & 1];
                 }
-                wgmma_commit();
+            };
+
+            mbar_wait(&q_full[wg], (n / kAtWG) & 1u);
+            issue_s(0);
+            wgmma_wait<0>();
+            reg_fence(s);
+            if (u.nt == 1) release_q();
+            softmax(0);
+            pack_rescale();
+            // key tile t: S(t) and P(t-1) V(t-1) go to the tensor core together; the softmax of tile t runs while
+            // P(t-1) V(t-1) is still on it
+            for (int t = 1; t < u.nt; ++t) {
+                issue_s(t);
+                issue_pv(t - 1);
+                wgmma_wait<1>();
+                reg_fence(s);
+                if (t == u.nt - 1) release_q();
+                softmax(t);
                 wgmma_wait<0>();
                 reg_fence(o);
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&b.kv_empty[st]);   // K / V stage consumed
+                release_kv(t - 1);
+                pack_rescale();
             }
+            issue_pv(u.nt - 1);
+            wgmma_wait<0>();
+            reg_fence(o);
+            release_kv(u.nt - 1);
+            pass_tiles(kc0 + u.nt, kc0 + it.ntiles);   // masked: a later query tile of the chunk sees more keys
             // ---- epilogue: O / l -> global
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
@@ -287,59 +352,50 @@ __global__ void __launch_bounds__(kAtThreads, 1) attn_tc_kernel(const __grid_con
                 const int r = r_in + 8 * h;
                 if (r < u.rows) {
                     const float inv = l_run[h] > 0.f ? 1.f / l_run[h] : 0.f;
-                    op_t* op = args.O + static_cast<long long>(u.o_row + r) * args.ldo + u.head * HD + cq;
+                    op_t* op = args.O + static_cast<long long>(u.o_row + r) * args.ldo + it.head * HD + cq;
 #pragma unroll
                     for (int j = 0; j < HD / 8; ++j)
                         *reinterpret_cast<uint32_t*>(op + 8 * j) = pack_op(o[4 * j + 2 * h] * inv, o[4 * j + 2 * h + 1] * inv);
                 }
             }
         }
-    } else if (lane == 0) {
+    } else {
         // ------------------------------------------------------------------ TMA producer
-        uint32_t nu = 0, ck = 0;
-        UnitIter<MASKED> it, pf;     // pf runs one unit ahead: its tiles are pulled into L2 while `it` is being fed
-        bool more = it.begin(&args, cta, ncta, npairs);
-        bool pf_more = pf.begin(&args, cta, ncta, npairs);
-        if (pf_more) pf_more = pf.next();
-        while (more) {
-            const Unit u = it.u;
-            const int head = u.head;
-            if (pf_more) {
-                const Unit& n = pf.u;
+        setmaxnreg_dec<32>();
+        if (warp == kAtProducerWarp && lane == 0) {
+            ChunkIter<MASKED> it;
+            for (bool more = it.begin(&args, cta, ncta, npairs); more; more = it.next()) {
+                const int head = it.head;
 #pragma unroll
-                for (int blk = 0; blk < NB; ++blk) tma_prefetch_l2_4d(&maps.q, n.head * HD + blk * 64, n.q_row, 0, 0);
-                if (n.q0 == 0) {      // the pair's first query tile brings its keys / values in (later tiles re-read them)
-                    const int nt = min(n.nt, 6);
-                    for (int t = 0; t < nt; ++t)
+                for (int i = 0; i < kAtWG; ++i) {
+                    if (i < it.cnt) {
+                        const int n = it.n0 + i;
+                        const int w = n % kAtWG;
+                        const Unit u = it.unit(i);
+                        mbar_wait(&q_empty[w], ((n / kAtWG) & 1u) ^ 1u);
+                        mbar_expect_tx(&q_full[w], Cfg::kQBytes);
 #pragma unroll
-                        for (int blk = 0; blk < NB; ++blk) {
-                            tma_prefetch_l2_4d(&maps.k, n.head * HD + blk * 64, n.k_row + t * kAtKV, 0, 0);
-                            tma_prefetch_l2_4d(&maps.v, n.head * HD + blk * 64, n.k_row + t * kAtKV, 0, 0);
-                        }
+                        for (int blk = 0; blk < NB; ++blk)
+                            tma_load_4d(sQ + w * Cfg::kQBytes + blk * (kAtQ * 128), &maps.q, &q_full[w],
+                                        head * HD + blk * 64, u.q_row, 0, 0);
+                    }
                 }
-                pf_more = pf.next();
-            }
-            mbar_wait(&b.q_empty, (nu & 1u) ^ 1u);
-            mbar_expect_tx(&b.q_full, Cfg::kQBytes);
+                const int k_row = static_cast<int>(it.sd.k_base / args.ldkv);
+                for (int t = 0; t < it.ntiles; ++t) {
+                    const uint32_t c = it.kc0 + t, st = c % S;
+                    mbar_wait(&kv_empty[st], ((c / S) & 1u) ^ 1u);
+                    mbar_expect_tx(&kv_full[st], Cfg::kStageBytes);
+                    uint8_t* sK = sKV + st * Cfg::kStageBytes;
+                    uint8_t* sV = sK + Cfg::kKBytes;
 #pragma unroll
-            for (int blk = 0; blk < NB; ++blk)
-                tma_load_4d(sQ + blk * (kAtQ * 128), &maps.q, &b.q_full, head * HD + blk * 64, u.q_row, 0, 0);
-            ++nu;
-            for (int t = 0; t < u.nt; ++t, ++ck) {
-                const uint32_t st = ck % kAtStages;
-                mbar_wait(&b.kv_empty[st], ((ck / kAtStages) & 1u) ^ 1u);
-                mbar_expect_tx(&b.kv_full[st], Cfg::kStageBytes);
-                uint8_t* sK = sKV + st * Cfg::kStageBytes;
-                uint8_t* sV = sK + Cfg::kKBytes;
-#pragma unroll
-                for (int blk = 0; blk < NB; ++blk) {
-                    tma_load_4d(sK + blk * (kAtKV * 128), &maps.k, &b.kv_full[st], head * HD + blk * 64,
-                                u.k_row + t * kAtKV, 0, 0);
-                    tma_load_4d(sV + blk * (kAtKV * 128), &maps.v, &b.kv_full[st], head * HD + blk * 64,
-                                u.k_row + t * kAtKV, 0, 0);
+                    for (int blk = 0; blk < NB; ++blk) {
+                        tma_load_4d(sK + blk * (kAtKV * 128), &maps.k, &kv_full[st], head * HD + blk * 64,
+                                    k_row + t * kAtKV, 0, 0);
+                        tma_load_4d(sV + blk * (kAtKV * 128), &maps.v, &kv_full[st], head * HD + blk * 64,
+                                    k_row + t * kAtKV, 0, 0);
+                    }
                 }
             }
-            more = it.next();
         }
     }
 }
