@@ -74,6 +74,13 @@ int ytk_op_attention_f16(const void* Q, long long ldq, long long q_rows, const v
                          long long kv_rows, void* O, long long ldo, const ytk_attn_seq* seqs_dev, int nseq, int max_q_len,
                          int heads, int head_dim, int masked, int impl, void* cuda_stream);
 
+/* Query selection of the RT-DETRv2 decoder (torch.topk over the encoder scores, reference
+ * models/layers/rtdetrv2_decoder.py:724-727).  scores_dev: [n, L] fp32 on the device; out_idx_dev: [n, K] int32 on the
+ * device = per row the indices of the K largest scores, descending, equal scores in ascending index order (-0 sorts
+ * below +0).  1 <= K <= L; L is bounded by shared memory (about 45k on an H100), a larger L is an error, not a launch.
+ * Asynchronous on the stream. */
+int ytk_op_topk_f32(const float* scores_dev, int n, int L, int K, int* out_idx_dev, void* cuda_stream);
+
 /* ---- Device-side front half of the DBNet post-processing (reference postprocessor/dbnet_postporcessor.py:39-82:
  * binarize, findContours, and the pixel work of minAreaRect / box_score_fast).  One record per horizontal run of an
  * 8-connected component of (prob > thresh). ---- */
@@ -219,15 +226,16 @@ int ytk_extract_crops_u8(const uint8_t* pages_dev, int n_pages, int H0, int W0, 
 int ytk_halve_pages_u8(const uint8_t* src_dev, int n_pages, int H, int W, uint8_t* dst_dev, int dH, int dW,
                        void* cuda_stream);
 
-/* ---- RT-DETRv2 layout parser / table structure recognizer: replaces `self.model(img_tensor)` in reference
- * LayoutParser.__call__ (src/yomitoku/layout_parser.py:258-262 -> models/rtdetr.py:17-22) and
- * TableStructureRecognizer.__call__ (table_structure_recognizer.py:272-276).  One architecture, two weight sets
- * (num_classes 6 / 3). ---- */
+/* ---- RT-DETRv2 layout parser / table structure recognizer / table cell detector: replaces `self.model(img_tensor)` in
+ * reference LayoutParser.__call__ (src/yomitoku/layout_parser.py:258-262 -> models/rtdetr.py:17-22),
+ * TableStructureRecognizer.__call__ (table_structure_recognizer.py:272-276) and CellDetector.__call__
+ * (table_cell_detector.py:502-504).  One architecture, three weight sets (num_classes 6 / 3 / 6, num_queries
+ * 300 / 300 / 1500, img_size 640 / 640 / 960). ---- */
 typedef struct ytk_rtdetr ytk_rtdetr;
 
 /* tensors: the reference's state_dict (RTDETRv2(cfg).state_dict() keys, host fp32; the boolean `decoder.valid_mask` may
  * be passed as 0/1 floats or left out - it is derived from the finite entries of `decoder.anchors`).  img_size: the square
- * evaluation size (cfg.data.img_size = eval_spatial_size, 640). */
+ * evaluation size (cfg.data.img_size = eval_spatial_size: 640 or 960, a multiple of 32). */
 int ytk_rtdetr_create(const ytk_tensor* tensors, int n_tensors, int num_classes, int num_queries, int img_size,
                       ytk_rtdetr** out);
 void ytk_rtdetr_destroy(ytk_rtdetr* h);

@@ -38,6 +38,8 @@ def _declare(lib):
     lib.ytk_op_attention_f16.restype = c_int
     lib.ytk_op_attention_f16.argtypes = [c_void_p, c_ll, c_ll, c_void_p, c_void_p, c_ll, c_ll, c_void_p, c_ll, c_void_p,
                                          c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]
+    lib.ytk_op_topk_f32.restype = c_int
+    lib.ytk_op_topk_f32.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]
 
 
 class YtkAttnSeq(ctypes.Structure):

@@ -173,6 +173,15 @@ int ytk_op_attention_f16(const void* Q, long long ldq, long long q_rows, const v
                : YTK_OK;
 }
 
+int ytk_op_topk_f32(const float* scores_dev, int n, int L, int K, int* out_idx_dev, void* cuda_stream) {
+    if (!scores_dev || !out_idx_dev) {
+        ytk::set_error("ytk_op_topk_f32: null argument");
+        return YTK_ERR;
+    }
+    return ytk::launch_rt_topk(scores_dev, n, L, K, out_idx_dev, static_cast<cudaStream_t>(cuda_stream)) ? YTK_ERR
+                                                                                                         : YTK_OK;
+}
+
 static_assert(sizeof(ytk_db_run) == sizeof(ytk::DbRun), "ytk_db_run and ytk::DbRun must have one layout");
 
 int ytk_dbnet_post_front(const float* prob_dev, int n_pages, int H, int W, float thresh, void* scratch_dev,

@@ -2,11 +2,12 @@
 // convolution and linear layer is a wgmma implicit GEMM (gemm_tc.cu), the two kinds of self-attention run on the wgmma
 // attention kernel (attn_tc.cu), the rest are the small kernels of rtdetr_ops.cu.  Replaces, for inference, reference
 // models/rtdetr.py:9-22 = layers/rtdetr_backbone.py:245-334 + layers/rtdetr_hybrid_encoder.py:216-410 +
-// layers/rtdetrv2_decoder.py:446-815 (the layout parser and the table structure recognizer share the architecture).
+// layers/rtdetrv2_decoder.py:446-815 (the layout parser, the table structure recognizer and the table cell detector share
+// the architecture; the image size and the query count come from the config: 640 / 300 or 960 / 1500).
 //
 // Data layout in HBM: activations NHWC fp16 (BatchNorm folded into weights / bias, RepVgg blocks re-parameterised into
 // one 3x3 convolution); the decoder's token matrices are level-major (rtdetr_ops.h) so that a level IS the NHWC output of
-// its 1x1 projection; the decoder state (300 queries per image) is fp32 with an fp16 copy as GEMM operand; the value
+// its 1x1 projection; the decoder state (num_queries rows per image) is fp32 with an fp16 copy as GEMM operand; the value
 // projections of all six decoder layers are one GEMM (256 -> 1536) over the memory.
 #include "rtdetr_engine.h"
 

@@ -122,35 +122,128 @@ __global__ void enc_scores_kernel(const float* __restrict__ logits, long long ld
     scores[(long long)img * lv.total + a] = m;
 }
 
-// torch.topk(scores, K) per image: one CTA sorts (score, anchor) keys with a bitonic network in shared memory.
-// Order: descending score, ascending anchor among equal scores.  NP = power of two >= number of anchors.
-__device__ __forceinline__ unsigned long long topk_key(float s, int a) {
-    unsigned u = __float_as_uint(s);
-    u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);           // monotone map of the float order onto unsigned
-    return ((unsigned long long)u << 32) | (unsigned)(0x7fffffff - a);
+// torch.topk(scores, K) per image (rtdetrv2_decoder.py:724-727).  Order: descending score, ascending anchor among equal
+// scores.  One CTA per image, everything in shared memory, one launch:
+//   1. the image's scores become 32-bit keys (monotone map of the float order onto unsigned: -0 < +0);
+//   2. an MSB radix select (four 8-bit digits, per-warp histograms) finds the K-th largest key T and the number of keys
+//      above it;
+//   3. every key above T is taken, keys equal to T in ascending anchor order (a block-wide count in index order) until
+//      exactly K are selected;
+//   4. the K (key, anchor) pairs are sorted by a bitonic network over the next power of two >= K.
+// The pair (key << 32 | 0x7fffffff - anchor) orders exactly like (score desc, anchor asc), so the result is the first K
+// of a stable descending sort of all L scores.
+constexpr int kTopkThreads = 1024;
+constexpr int kTopkWarps = kTopkThreads / 32;
+constexpr int kTopkBins = 256;
+
+__device__ __forceinline__ unsigned topk_key(float s) {
+    const unsigned u = __float_as_uint(s);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
-__global__ void topk_kernel(const float* __restrict__ scores, int L, int NP, int K, int* __restrict__ out_idx) {
-    extern __shared__ unsigned long long keys[];
+
+// dynamic shared memory: pairs [KP] u64 | hist [kTopkWarps][kTopkBins] u32 | keys [L] u32
+__global__ void __launch_bounds__(kTopkThreads, 1)
+topk_select_kernel(const float* __restrict__ scores, int L, int K, int KP, int* __restrict__ out_idx) {
+    extern __shared__ unsigned long long tk_smem[];
+    unsigned long long* pairs = tk_smem;
+    unsigned* hist = reinterpret_cast<unsigned*>(pairs + KP);
+    unsigned* keys = hist + kTopkWarps * kTopkBins;
+    __shared__ unsigned s_wsum[kTopkWarps];
+    __shared__ unsigned s_prefix, s_above, s_bin_above;
+    __shared__ int s_n_gt;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const float* s = scores + (long long)blockIdx.x * L;
-    for (int i = threadIdx.x; i < NP; i += blockDim.x) keys[i] = i < L ? topk_key(s[i], i) : 0ull;
+    for (int i = tid; i < L; i += kTopkThreads) keys[i] = topk_key(__ldg(s + i));
+    if (tid == 0) {
+        s_prefix = 0;
+        s_above = 0;
+        s_n_gt = 0;
+    }
+    // ---- radix select of the K-th largest key
+    unsigned mask = 0;
+    for (int shift = 24; shift >= 0; shift -= 8) {
+        for (int i = tid; i < kTopkWarps * kTopkBins; i += kTopkThreads) hist[i] = 0;
+        __syncthreads();
+        const unsigned prefix = s_prefix;
+        unsigned* wh = hist + warp * kTopkBins;
+        for (int i = tid; i < L; i += kTopkThreads) {
+            const unsigned k = keys[i];
+            if ((k & mask) == prefix) atomicAdd(wh + ((k >> shift) & 0xffu), 1u);
+        }
+        __syncthreads();
+        // inclusive count of keys whose digit is >= b, b = 255 - tid: a scan over the bins in descending order
+        unsigned v = 0, incl = 0;
+        if (tid < kTopkBins) {
+            const int b = kTopkBins - 1 - tid;
+            for (int w = 0; w < kTopkWarps; ++w) v += hist[w * kTopkBins + b];
+            incl = v;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const unsigned t = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl += t;
+            }
+            if (lane == 31) s_wsum[warp] = incl;
+        }
+        __syncthreads();
+        if (tid < kTopkBins) {
+            for (int w = 0; w < warp; ++w) incl += s_wsum[w];
+            const unsigned need = (unsigned)K - s_above;       // rank of the K-th key among the keys matching prefix
+            const unsigned excl = incl - v;
+            if (excl < need && incl >= need) {                  // exactly one bin holds it
+                s_prefix = prefix | ((unsigned)(kTopkBins - 1 - tid) << shift);
+                s_bin_above = excl;
+            }
+        }
+        __syncthreads();
+        if (tid == 0) s_above += s_bin_above;
+        mask |= 0xffu << shift;
+        __syncthreads();
+    }
+    const unsigned T = s_prefix;
+    const int n_gt = (int)s_above;                              // keys > T; K - n_gt keys equal to T are taken
+    const int n_eq = K - n_gt;
+    // ---- selection: keys above T in any slot of [0, n_gt), keys equal to T at n_gt + (their rank in index order)
+    int eq_before = 0;
+    for (int base = 0; base < L; base += kTopkThreads) {
+        const int i = base + tid;
+        const unsigned k = i < L ? keys[i] : 0u;
+        const bool eq = i < L && k == T;
+        const unsigned ball = __ballot_sync(0xffffffffu, eq);
+        if (lane == 0) s_wsum[warp] = __popc(ball);
+        if (i < L && k > T) {
+            const int slot = atomicAdd(&s_n_gt, 1);
+            pairs[slot] = ((unsigned long long)k << 32) | (unsigned)(0x7fffffff - i);
+        }
+        __syncthreads();
+        int rank = eq_before + __popc(ball & ((1u << lane) - 1u)), chunk = 0;
+        for (int w = 0; w < kTopkWarps; ++w) {
+            const int c = (int)s_wsum[w];
+            if (w < warp) rank += c;
+            chunk += c;
+        }
+        if (eq && rank < n_eq) pairs[n_gt + rank] = ((unsigned long long)k << 32) | (unsigned)(0x7fffffff - i);
+        eq_before += chunk;
+        __syncthreads();                                        // s_wsum is rewritten by the next chunk
+    }
+    for (int i = K + tid; i < KP; i += kTopkThreads) pairs[i] = 0ull;   // padding sorts last
     __syncthreads();
-    for (int k = 2; k <= NP; k <<= 1)
+    // ---- bitonic sort of the K selected pairs, descending
+    for (int k = 2; k <= KP; k <<= 1)
         for (int j = k >> 1; j > 0; j >>= 1) {
-            for (int i = threadIdx.x; i < NP; i += blockDim.x) {
-                const int p = i ^ j;
-                if (p > i) {
-                    const unsigned long long a = keys[i], b = keys[p];
-                    const bool desc = (i & k) == 0;              // descending blocks first: final order is descending
-                    if (desc ? (a < b) : (a > b)) {
-                        keys[i] = b;
-                        keys[p] = a;
-                    }
+            for (int t = tid; t < (KP >> 1); t += kTopkThreads) {
+                const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1));   // lower element of the t-th compared pair
+                const int p = i | j;
+                const unsigned long long a = pairs[i], b = pairs[p];
+                const bool desc = (i & k) == 0;                 // descending blocks first: final order is descending
+                if (desc ? (a < b) : (a > b)) {
+                    pairs[i] = b;
+                    pairs[p] = a;
                 }
             }
             __syncthreads();
         }
-    for (int i = threadIdx.x; i < K; i += blockDim.x)
-        out_idx[(long long)blockIdx.x * K + i] = 0x7fffffff - (int)(keys[i] & 0xffffffffu);
+    for (int i = tid; i < K; i += kTopkThreads)
+        out_idx[(long long)blockIdx.x * K + i] = 0x7fffffff - (int)(pairs[i] & 0xffffffffu);
 }
 
 // decoder start: target rows = output_memory[top-k rows] (fp32 + fp16), anchors of the selected positions
@@ -325,21 +418,29 @@ int launch_rt_enc_scores(const float* logits, long long ldl, int C, const RtLeve
 }
 
 int launch_rt_topk(const float* scores, int n_img, int L, int K, int* out_idx, cudaStream_t st) {
-    int NP = 1;
-    while (NP < L) NP <<= 1;
-    const size_t smem = (size_t)NP * sizeof(unsigned long long);
+    if (n_img < 1 || L < 1 || K < 1 || K > L) {
+        set_error("topk: %d images, %d candidates, k = %d unsupported (1 <= k <= candidates)", n_img, L, K);
+        return 1;
+    }
+    int KP = 1;
+    while (KP < K) KP <<= 1;
+    const size_t smem = (size_t)KP * sizeof(unsigned long long) + (size_t)kTopkWarps * kTopkBins * 4 + (size_t)L * 4;
+    int dev = 0, optin = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+    optin -= 1024;                             // the kernel's static shared memory comes out of the same budget
+    if (smem > (size_t)optin) {
+        set_error("topk: %d candidates / k = %d need %zu bytes of shared memory, a CTA can have %d", L, K, smem, optin);
+        return 1;
+    }
     static unsigned long long attr_done = 0;   // per device
     if (first_launch_on_device(&attr_done)) {
-        if (cudaFuncSetAttribute(topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess) {
-            set_error("topk: cannot raise the shared memory limit");
+        if (cudaFuncSetAttribute(topk_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, optin) != cudaSuccess) {
+            set_error("topk: cannot raise the shared memory limit to %d bytes", optin);
             return 1;
         }
     }
-    if (smem > 200 * 1024 || K > L) {
-        set_error("topk: %d candidates / k = %d unsupported", L, K);
-        return 1;
-    }
-    topk_kernel<<<n_img, 1024, smem, st>>>(scores, L, NP, K, out_idx);
+    topk_select_kernel<<<n_img, kTopkThreads, smem, st>>>(scores, L, K, KP, out_idx);
     count_launch();
     return cudaGetLastError() != cudaSuccess;
 }

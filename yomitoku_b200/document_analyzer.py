@@ -60,6 +60,64 @@ def is_contained(a, b, threshold=0.8):
     return overlap_ratio(a, b)[0] > threshold
 
 
+def calc_iou(a, b):
+    """Intersection over union (utils/misc.py:182-201): the intersection of the int-truncated boxes, the areas of the
+    raw values."""
+    inter = _intersection(a, b)
+    if inter is None:
+        return 0
+    i_area = (inter[2] - inter[0]) * (inter[3] - inter[1])
+    return i_area / ((a[2] - a[0]) * (a[3] - a[1]) + (b[2] - b[0]) * (b[3] - b[1]) - i_area)
+
+
+def _point_segment_dist(px, py, ax, ay, bx, by):
+    """Distance of (px, py) to the segment (ax, ay)-(bx, by) (utils/misc.py:208-221)."""
+    dx, dy = bx - ax, by - ay
+    den = dx * dx + dy * dy
+    if den == 0:
+        return math.hypot(px - ax, py - ay)
+    t = min(1.0, max(0.0, ((px - ax) * dx + (py - ay) * dy) / den))
+    return math.hypot(px - (ax + t * dx), py - (ay + t * dy))
+
+
+def _edge_dists(a1, a2, b1, b2, edge_a, edge_b, vertical):
+    """The four corner-to-edge distance pairs between the edge of A at coordinate edge_a spanning [a1, a2] and the edge
+    of B at edge_b spanning [b1, b2] (utils/misc.py:224-267).  vertical: the edges are vertical (x = edge)."""
+    def d(e_p, p, e0, e1, e):        # corner (e_p, p) of one box to the edge e spanning [e0, e1] of the other
+        return (_point_segment_dist(e_p, p, e, e0, e, e1) if vertical else _point_segment_dist(p, e_p, e0, e, e1, e))
+    d1 = d(edge_a, a1, b1, b2, edge_b)
+    d2 = d(edge_a, a2, b1, b2, edge_b)
+    d3 = d(edge_b, b1, a1, a2, edge_a)
+    d4 = d(edge_b, b2, a1, a2, edge_a)
+    return max(d1, d4), max(d2, d3), max(d3, d4), max(d1, d2)
+
+
+def _adjacent(a, b, axis, dist_threshold, overlap_ratio_th, ignore_dist_threshold):
+    """B lies next to A along `axis` (0: to the right, 1: below); utils/misc.py:299-427 with rule "soft"."""
+    c, o = axis, 1 - axis                            # the coordinate that advances / the one that must overlap
+    if b[c] < a[c]:
+        return False
+    if max(0.0, min(a[o + 2], b[o + 2]) - max(a[o], b[o])) < overlap_ratio_th * min(a[o + 2] - a[o], b[o + 2] - b[o]):
+        return False
+    # corners that touch diagonally are no neighbours: A's far corner vs B's near corner, and the crossed pair
+    if math.hypot(a[2] - b[0], a[3] - b[1]) < ignore_dist_threshold:
+        return False
+    if axis == 0 and math.hypot(a[2] - b[0], a[1] - b[3]) < ignore_dist_threshold:
+        return False
+    if axis == 1 and math.hypot(a[0] - b[2], a[3] - b[1]) < ignore_dist_threshold:
+        return False
+    dists = _edge_dists(a[o], a[o + 2], b[o], b[o + 2], a[c + 2], b[c], vertical=(axis == 0))
+    return any(v < dist_threshold for v in dists)
+
+
+def is_right_adjacent(box_a, box_b, dist_threshold=15, overlap_ratio_th=0.1, ignore_dist_threshold=10):
+    return _adjacent(box_a, box_b, 0, dist_threshold, overlap_ratio_th, ignore_dist_threshold)
+
+
+def is_bottom_adjacent(box_a, box_b, dist_threshold=15, overlap_ratio_th=0.1, ignore_dist_threshold=10):
+    return _adjacent(box_a, box_b, 1, dist_threshold, overlap_ratio_th, ignore_dist_threshold)
+
+
 def _side_lengths(quad):
     q = np.array(quad)
     return np.linalg.norm(q[0] - q[1]), np.linalg.norm(q[1] - q[2])
