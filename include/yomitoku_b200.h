@@ -229,7 +229,8 @@ int ytk_halve_pages_u8(const uint8_t* src_dev, int n_pages, int H, int W, uint8_
 /* ---- RT-DETRv2 layout parser / table structure recognizer / table cell detector: replaces `self.model(img_tensor)` in
  * reference LayoutParser.__call__ (src/yomitoku/layout_parser.py:258-262 -> models/rtdetr.py:17-22),
  * TableStructureRecognizer.__call__ (table_structure_recognizer.py:272-276) and CellDetector.__call__
- * (table_cell_detector.py:502-504).  One architecture, three weight sets (num_classes 6 / 3 / 6, num_queries
+ * (table_cell_detector.py:502-504) and, in the u8 entry, also their `self.transforms` (cvtColor, the table crop, PIL
+ * bilinear resize, ToTensor).  One architecture, three weight sets (num_classes 6 / 3 / 6, num_queries
  * 300 / 300 / 1500, img_size 640 / 640 / 960). ---- */
 typedef struct ytk_rtdetr ytk_rtdetr;
 
@@ -246,6 +247,34 @@ int ytk_rtdetr_device(const ytk_rtdetr* h);
  * score).  Outputs on the host: the call returns after the copy; on the device: asynchronous on the stream. */
 int ytk_rtdetr_forward_f32(ytk_rtdetr* h, const float* x, int x_on_device, int n, float* pred_logits, float* pred_boxes,
                            int out_on_device, void* cuda_stream);
+
+/* One model input of the u8 entry: a rectangle of a BGR page.  Invalid records (a page extent beyond pages_bytes, an
+ * empty rectangle, a rectangle outside its page) are an error, not a launch. */
+typedef struct {
+    long long page_off;   /* byte offset of the page in `pages`: H*W*3 bytes, BGR, rows of W*3 bytes */
+    int H, W;             /* page size (pages of different sizes may share one buffer) */
+    int x0, y0, x1, y1;   /* the model input is page[y0:y1, x0:x1]; 0 <= x0 < x1 <= W, 0 <= y0 < y1 <= H */
+} ytk_rtdetr_src;         /* 32 bytes */
+
+/* The reference's whole input path on the device: per record, the rectangle as RGB,
+ * Image.fromarray(rgb_crop).resize((img, img), Image.BILINEAR) bit for bit (Pillow's fixed-point separable resample,
+ * horizontal pass first) and ToTensor, then the forward of ytk_rtdetr_forward_f32 with the same outputs, ordering and
+ * copy semantics.  The layout parser reads whole pages, the table structure recognizer and the cell detector table
+ * crops of them; one upload of the pages serves all three.  pages: pages_bytes bytes on the device iff pages_on_device,
+ * else on the host (copied into a buffer the handle owns; page-locked memory must stay valid until the stream has
+ * passed the call).  srcs: n host records. */
+int ytk_rtdetr_forward_u8(ytk_rtdetr* h, const uint8_t* pages, int pages_on_device, long long pages_bytes,
+                          const ytk_rtdetr_src* srcs, int n, float* pred_logits, float* pred_boxes, int out_on_device,
+                          void* cuda_stream);
+/* op level, for the parity tests: the resize of ytk_rtdetr_forward_u8 alone.  out_rgb_dev = [n][size][size][3] u8 RGB
+ * (the resized images, before / 255); scratch_dev holds at least ytk_op_resize_bilinear_scratch_bytes(srcs, n, size)
+ * bytes: the call allocates nothing.  Asynchronous on the stream: one H2D copy + two kernel launches. */
+int ytk_op_resize_bilinear_u8(const uint8_t* pages_dev, long long pages_bytes, const ytk_rtdetr_src* srcs, int n,
+                              int size, uint8_t* scratch_dev, long long scratch_bytes, uint8_t* out_rgb_dev,
+                              void* cuda_stream);
+/* scratch bytes ytk_op_resize_bilinear_u8 needs for these records (page extents are not checked here), -1 if a record
+ * is invalid */
+long long ytk_op_resize_bilinear_scratch_bytes(const ytk_rtdetr_src* srcs, int n, int size);
 double ytk_rtdetr_flops(ytk_rtdetr* h, int n);
 /* test hook: copies an intermediate activation (by name, see rtdetr_engine.cu) of the LAST forward of batch size n to
  * the host as fp32; shape4 = {n, h, w, c} (token matrices: {1, 1, rows, c}) */

@@ -122,8 +122,22 @@ def _declare_crops(lib):
     lib.ytk_halve_pages_u8.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p]
 
 
+class YtkRtdetrSrc(ctypes.Structure):
+    """ytk_rtdetr_src: the model input page[y0:y1, x0:x1] of the H x W BGR page at byte page_off."""
+    _fields_ = [("page_off", c_ll), ("H", c_int), ("W", c_int), ("x0", c_int), ("y0", c_int), ("x1", c_int),
+                ("y1", c_int)]
+
+
 def _declare_rtdetr(lib):
     P = ctypes.POINTER
+    lib.ytk_rtdetr_forward_u8.restype = c_int
+    lib.ytk_rtdetr_forward_u8.argtypes = [c_void_p, c_void_p, c_int, c_ll, c_void_p, c_int, c_void_p, c_void_p, c_int,
+                                          c_void_p]
+    lib.ytk_op_resize_bilinear_u8.restype = c_int
+    lib.ytk_op_resize_bilinear_u8.argtypes = [c_void_p, c_ll, c_void_p, c_int, c_int, c_void_p, c_ll, c_void_p,
+                                              c_void_p]
+    lib.ytk_op_resize_bilinear_scratch_bytes.restype = c_ll
+    lib.ytk_op_resize_bilinear_scratch_bytes.argtypes = [c_void_p, c_int, c_int]
     lib.ytk_rtdetr_create.restype = c_int
     lib.ytk_rtdetr_create.argtypes = [P(YtkTensor), c_int, c_int, c_int, c_int, P(c_void_p)]
     lib.ytk_rtdetr_destroy.restype = None

@@ -23,8 +23,10 @@ NVCC_FLAGS = [
 
 
 # OpenCV's float / double expressions are not contracted into FMAs: the bit-exact restatement in crop_math.h needs the
-# same (csrc/crop_ops.cu header)
-EXTRA_FLAGS = {"crop_ops.cu": ["--fmad=false"]}
+# same (csrc/crop_ops.cu header).  Pillow's resample coefficients are double arithmetic computed on the host
+# (csrc/resample_ops.cu header): neither the device nor the host compiler may contract them.
+EXTRA_FLAGS = {"crop_ops.cu": ["--fmad=false"],
+               "resample_ops.cu": ["--fmad=false", "-Xcompiler", "-ffp-contract=off"]}
 
 
 def _sources():

@@ -2,6 +2,7 @@
 #include "../../include/yomitoku_b200.h"
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdlib>
 #include <map>
@@ -15,6 +16,7 @@
 #include "dbpost_ops.h"
 #include "gemm_tc.h"
 #include "parseq_engine.h"
+#include "resample_ops.h"
 #include "rtdetr_engine.h"
 
 // Binds the calling host thread to a device for the duration of an API call and puts the previous device back (host
@@ -542,7 +544,46 @@ struct ytk_rtdetr {
     std::mutex mu;
     int device = 0;
     cudaEvent_t last_done = nullptr;   // buffers of an engine are shared by all calls: order them (see ytk_dbnet)
+    // ytk_rtdetr_forward_u8: device copy of host pages, and the resize scratch (records, coefficients, intermediates)
+    uint8_t* pages = nullptr;
+    size_t pages_cap = 0;
+    uint8_t* scratch = nullptr;
+    size_t scratch_cap = 0;
 };
+
+// Grows a handle-owned buffer; the previous call may still be reading the old one.
+static int rt_reserve(ytk_rtdetr* h, uint8_t** buf, size_t* cap, size_t bytes, const char* what) {
+    if (*cap >= bytes) return 0;
+    if (h->last_done) cudaEventSynchronize(h->last_done);
+    if (*buf) cudaFree(*buf);
+    *buf = nullptr;
+    *cap = 0;
+    if (cudaMalloc(buf, bytes) != cudaSuccess) {
+        *buf = nullptr;
+        ytk::set_error("cudaMalloc(%zu) for the %s failed", bytes, what);
+        return 1;
+    }
+    *cap = bytes;
+    return 0;
+}
+
+// Runs the engine on its packed input and copies the outputs (the common tail of both forward entries).
+static int rt_finish(ytk_rtdetr* h, ytk::RtdetrEngine* e, int n, float* pred_logits, float* pred_boxes, int out_on_device,
+                     cudaStream_t st) {
+    if (e->run(st)) return YTK_ERR;
+    const int K = h->model.cfg.num_queries, C = h->model.cfg.num_classes;
+    const cudaMemcpyKind kind = out_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+    cudaError_t err = cudaMemcpyAsync(pred_logits, e->out_logits, (size_t)n * K * C * 4, kind, st);
+    if (err == cudaSuccess) err = cudaMemcpyAsync(pred_boxes, e->boxes, (size_t)n * K * 16, kind, st);
+    if (!h->last_done) cudaEventCreateWithFlags(&h->last_done, cudaEventDisableTiming);
+    if (h->last_done) cudaEventRecord(h->last_done, st);
+    if (err == cudaSuccess && !out_on_device) err = cudaStreamSynchronize(st);
+    if (err != cudaSuccess) {
+        ytk::set_error("RT-DETRv2 output copy failed: %s", cudaGetErrorString(err));
+        return YTK_ERR;
+    }
+    return YTK_OK;
+}
 
 static ytk::RtdetrEngine* rt_engine(ytk_rtdetr* h, int n) {
     auto it = h->engines.find(n);
@@ -595,6 +636,8 @@ void ytk_rtdetr_destroy(ytk_rtdetr* h) {
         cudaEventDestroy(h->last_done);
     }
     cudaDeviceSynchronize();
+    if (h->pages) cudaFree(h->pages);
+    if (h->scratch) cudaFree(h->scratch);
     delete h;
 }
 
@@ -612,7 +655,7 @@ int ytk_rtdetr_forward_f32(ytk_rtdetr* h, const float* x, int x_on_device, int n
     ytk::RtdetrEngine* e = rt_engine(h, n);
     if (!e) return YTK_ERR;
     if (h->last_done) cudaStreamWaitEvent(st, h->last_done, 0);
-    const int S = h->model.cfg.img, K = h->model.cfg.num_queries, C = h->model.cfg.num_classes;
+    const int S = h->model.cfg.img;
     const float* src = x;
     if (!x_on_device) {
         if (cudaMemcpyAsync(e->in_f32, x, (size_t)n * 3 * S * S * 4, cudaMemcpyHostToDevice, st) != cudaSuccess) {
@@ -621,18 +664,78 @@ int ytk_rtdetr_forward_f32(ytk_rtdetr* h, const float* x, int x_on_device, int n
         }
         src = e->in_f32;
     }
-    if (ytk::launch_rt_pack_input(src, n, S, S, e->input, st) || e->run(st)) return YTK_ERR;
-    const cudaMemcpyKind kind = out_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-    cudaError_t err = cudaMemcpyAsync(pred_logits, e->out_logits, (size_t)n * K * C * 4, kind, st);
-    if (err == cudaSuccess) err = cudaMemcpyAsync(pred_boxes, e->boxes, (size_t)n * K * 16, kind, st);
-    if (!h->last_done) cudaEventCreateWithFlags(&h->last_done, cudaEventDisableTiming);
-    if (h->last_done) cudaEventRecord(h->last_done, st);
-    if (err == cudaSuccess && !out_on_device) err = cudaStreamSynchronize(st);
-    if (err != cudaSuccess) {
-        ytk::set_error("RT-DETRv2 output copy failed: %s", cudaGetErrorString(err));
+    if (ytk::launch_rt_pack_input(src, n, S, S, e->input, st)) return YTK_ERR;
+    return rt_finish(h, e, n, pred_logits, pred_boxes, out_on_device, st);
+}
+
+static_assert(sizeof(ytk_rtdetr_src) == sizeof(ytk::RtSrc), "ytk_rtdetr_src and ytk::RtSrc must have one layout");
+
+int ytk_rtdetr_forward_u8(ytk_rtdetr* h, const uint8_t* pages, int pages_on_device, long long pages_bytes,
+                          const ytk_rtdetr_src* srcs, int n, float* pred_logits, float* pred_boxes, int out_on_device,
+                          void* cuda_stream) {
+    if (!h || !pages || !srcs || !pred_logits || !pred_boxes || n < 1 || pages_bytes < 1) {
+        ytk::set_error("ytk_rtdetr_forward_u8: null or empty argument");
         return YTK_ERR;
     }
-    return YTK_OK;
+    std::lock_guard<std::mutex> lk(h->mu);
+    DevGuard dev_guard(h->device);
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    ytk::ResampleJob job;
+    if (ytk::resample_prepare(reinterpret_cast<const ytk::RtSrc*>(srcs), n, h->model.cfg.img, pages_bytes,
+                              "ytk_rtdetr_forward_u8", &job))
+        return YTK_ERR;
+    ytk::RtdetrEngine* e = rt_engine(h, n);
+    if (!e) return YTK_ERR;
+    if (!pages_on_device && rt_reserve(h, &h->pages, &h->pages_cap, (size_t)pages_bytes, "page staging buffer"))
+        return YTK_ERR;
+    if (rt_reserve(h, &h->scratch, &h->scratch_cap, (size_t)job.bytes, "resize scratch")) return YTK_ERR;
+    if (h->last_done) cudaStreamWaitEvent(st, h->last_done, 0);
+    const uint8_t* src = pages;
+    if (!pages_on_device) {
+        cudaError_t err = cudaMemcpyAsync(h->pages, pages, (size_t)pages_bytes, cudaMemcpyHostToDevice, st);
+        if (err != cudaSuccess) {
+            ytk::set_error("H2D copy of the pages failed: %s", cudaGetErrorString(err));
+            return YTK_ERR;
+        }
+        src = h->pages;
+    }
+    if (ytk::launch_resample(src, job, h->scratch, e->input, 1, st)) return YTK_ERR;
+    return rt_finish(h, e, n, pred_logits, pred_boxes, out_on_device, st);
+}
+
+long long ytk_op_resize_bilinear_scratch_bytes(const ytk_rtdetr_src* srcs, int n, int size) {
+    ytk::ResampleJob job;
+    if (ytk::resample_prepare(reinterpret_cast<const ytk::RtSrc*>(srcs), n, size, LLONG_MAX,
+                              "ytk_op_resize_bilinear_scratch_bytes", &job))
+        return -1;
+    return job.bytes;
+}
+
+int ytk_op_resize_bilinear_u8(const uint8_t* pages_dev, long long pages_bytes, const ytk_rtdetr_src* srcs, int n,
+                              int size, uint8_t* scratch_dev, long long scratch_bytes, uint8_t* out_rgb_dev,
+                              void* cuda_stream) {
+    if (!pages_dev || !srcs || !scratch_dev || !out_rgb_dev) {
+        ytk::set_error("ytk_op_resize_bilinear_u8: null argument");
+        return YTK_ERR;
+    }
+    ytk::ResampleJob job;
+    if (ytk::resample_prepare(reinterpret_cast<const ytk::RtSrc*>(srcs), n, size, pages_bytes,
+                              "ytk_op_resize_bilinear_u8", &job))
+        return YTK_ERR;
+    if (scratch_bytes < job.bytes) {
+        ytk::set_error("ytk_op_resize_bilinear_u8: scratch_dev holds %lld bytes, need %lld", scratch_bytes, job.bytes);
+        return YTK_ERR;
+    }
+    cudaPointerAttributes attr;
+    if (cudaPointerGetAttributes(&attr, pages_dev) != cudaSuccess || attr.type != cudaMemoryTypeDevice) {
+        cudaGetLastError();
+        ytk::set_error("ytk_op_resize_bilinear_u8: pages_dev is not a device pointer");
+        return YTK_ERR;
+    }
+    DevGuard dev_guard(attr.device);
+    return ytk::launch_resample(pages_dev, job, scratch_dev, out_rgb_dev, 0, static_cast<cudaStream_t>(cuda_stream))
+               ? YTK_ERR
+               : YTK_OK;
 }
 
 double ytk_rtdetr_flops(ytk_rtdetr* h, int n) {

@@ -2,14 +2,17 @@
 
 Mirrors reference src/yomitoku/layout_parser.py:23-274 - same catalog names (`rtdetrv2`, `rtdetrv2v2`), constructor
 kwargs, `preprocess` / `postprocess` / `filtering_elements` / `__call__` contract and result schema.  The model forward
-runs as sm_90a kernels (csrc/rtdetr_engine.cu behind ytk_rtdetr_forward_f32); the PIL resize in front of it and the
-containment filters behind it are host code like in the reference.  `infer_onnx` is accepted and ignored.
+runs as sm_90a kernels (csrc/rtdetr_engine.cu).  On a CUDA device the page goes up as u8 and the PIL resize in front of
+the model runs there too, bit for bit (csrc/resample_ops.cu behind ytk_rtdetr_forward_u8, shared with the table
+structure recognizer and the cell detector through `rtdetr_device_forward`); `preprocess` stays the host form of it.
+The containment filters behind the model are host code like in the reference.  `infer_onnx` is accepted and ignored.
 """
 import cv2
 import numpy as np
 import torch
 from PIL import Image
 
+from . import _lib
 from .base import BaseModelCatalog, BaseModule, logger
 from .config import LayoutParserRTDETRv2Config, LayoutParserRTDETRv2V2Config
 from .document_analyzer import is_contained
@@ -65,6 +68,67 @@ def rtdetr_input_tensor(rgb, img_size):
     return torch.from_numpy(np.ascontiguousarray(small.transpose(2, 0, 1))).to(torch.float32).div(255)[None]
 
 
+RTDETR_SRC_DTYPE = np.dtype(_lib.YtkRtdetrSrc)
+
+
+def rtdetr_sources(page_shapes, boxes):
+    """Model inputs of RTDETRv2.forward_u8: page_shapes are the (h, w, ...) shapes of the pages packed back to back,
+    boxes are (page index, (x1, y1, x2, y2)) pairs.  Each box is read as the modules read it, `int(v)` per coordinate,
+    with numpy slicing semantics: `rgb[y1:y2, x1:x2]`, x2 / y2 clamped to the page.  Returns (records, sizes), sizes[i]
+    = (h, w) of that crop (its `crop.shape[:2]`), or None when numpy would not make a plain crop of some box (a
+    negative coordinate wraps around, or the crop is empty): the caller then takes the host path for the whole call."""
+    offs, off = [], 0
+    for shape in page_shapes:
+        offs.append(off)
+        off += int(shape[0]) * int(shape[1]) * 3
+    recs = np.zeros(len(boxes), RTDETR_SRC_DTYPE)
+    sizes = []
+    for i, (p, box) in enumerate(boxes):
+        H, W = int(page_shapes[p][0]), int(page_shapes[p][1])
+        x1, y1, x2, y2 = (int(v) for v in box)
+        if min(x1, y1, x2, y2) < 0:
+            return None
+        x2, y2 = min(x2, W), min(y2, H)
+        if x1 >= x2 or y1 >= y2:
+            return None
+        recs[i] = (offs[p], H, W, x1, y1, x2, y2)
+        sizes.append((y2 - y1, x2 - x1))
+    return recs, sizes
+
+
+def upload_pages(pages, model):
+    """BGR u8 pages -> one flat uint8 tensor on `model`'s CUDA device, pages back to back (what forward_u8 reads), so
+    that several RT-DETRv2 models read one upload.  None when the device path does not apply: the model is not on a
+    CUDA device, or a page is not a non-empty (h, w, 3) uint8 array."""
+    if model._device.type != "cuda" or not torch.cuda.is_available() or not pages:
+        return None
+    for p in pages:
+        if not (isinstance(p, np.ndarray) and p.dtype == np.uint8 and p.ndim == 3 and p.shape[2] == 3 and p.size):
+            return None
+    flat = np.concatenate([np.ascontiguousarray(p).reshape(-1) for p in pages])
+    return torch.from_numpy(flat).to(model.cuda_device())
+
+
+def rtdetr_device_forward(model, pages, boxes, pages_dev=None):
+    """The device path of the three RT-DETRv2 modules: `model`'s outputs (on the host) for the crops `boxes` (page
+    index, box) of the BGR u8 `pages`, resized on the device, and the crop sizes.  pages_dev: those pages as
+    upload_pages made them (shared with another model), else they are uploaded here.  None when the device path does
+    not apply (upload_pages, rtdetr_sources): the caller then runs `model(torch.cat(preprocess(...)))`, which gives the
+    same bits."""
+    if model._device.type != "cuda" or not torch.cuda.is_available():
+        return None
+    src = rtdetr_sources([p.shape for p in pages], boxes)
+    if src is None:
+        return None
+    if pages_dev is None or pages_dev.device != model.cuda_device():
+        pages_dev = upload_pages(pages, model)
+        if pages_dev is None:
+            return None
+    recs, sizes = src
+    preds = model.forward_u8(pages_dev, recs)
+    return {k: v.cpu() for k, v in preds.items()}, sizes
+
+
 class LayoutParser(BaseModule):
     model_catalog = LayoutParserModelCatalog()
 
@@ -109,17 +173,19 @@ class LayoutParser(BaseModule):
         by_category = filter_contained_rectangles_within_category(by_category)
         return filter_contained_rectangles_across_categories(by_category, "tables", "paragraphs")
 
-    def __call__(self, img):
-        ori_h, ori_w = img.shape[:2]
-        preds = self.model(self.preprocess(img))
-        results = self.postprocess(preds, (ori_h, ori_w))
+    def __call__(self, img, pages_dev=None):
+        """pages_dev (optional): `img` already on the device as upload_pages([img], ...) made it."""
+        results = self.parse_pages([img], pages_dev)[0]
         vis = layout_visualizer(results, img) if self.visualize else None
         return results, vis
 
-    def parse_pages(self, pages):
-        """Batched entry (new surface): list of BGR pages (any sizes) -> list of LayoutParserSchema; one device call."""
-        x = torch.cat([self.preprocess(p) for p in pages])
-        preds = self.model(x)
+    def parse_pages(self, pages, pages_dev=None):
+        """Batched entry (new surface): list of BGR pages (any sizes) -> list of LayoutParserSchema; one device call.
+        On a CUDA device the pages go up once as u8 (or are read from pages_dev, upload_pages(pages, ...)) and are
+        resized there; otherwise they are preprocessed on the host."""
+        whole = [(i, (0, 0, p.shape[1], p.shape[0])) for i, p in enumerate(pages)]
+        dev = rtdetr_device_forward(self.model, pages, whole, pages_dev)
+        preds = dev[0] if dev is not None else self.model(torch.cat([self.preprocess(p) for p in pages]))
         return [self.postprocess({k: v[i:i + 1] for k, v in preds.items()}, p.shape[:2]) for i, p in enumerate(pages)]
 
 

@@ -757,6 +757,30 @@ class RTDETRv2(_DeviceModel):
                                                      _stream_ptr(stream)))
         return {"pred_logits": logits, "pred_boxes": boxes}
 
+    def forward_u8(self, pages, srcs, stream=None):
+        """The model on u8 pages: resize, ToTensor and forward on the device (C ABI ytk_rtdetr_forward_u8).
+
+        pages: flat uint8 BGR pages back to back - a torch tensor on the host or on the model's CUDA device, or a numpy
+        array; srcs: one ytk_rtdetr_src record per model input (layout_parser.rtdetr_sources).  Input i is
+        Image.fromarray(rgb[y0:y1, x0:x1]).resize((S, S), Image.BILINEAR) + ToTensor bit for bit, so the result equals
+        `forward` on the stacked `preprocess` tensors.  Returns the dict of `forward`, on the pages' device."""
+        h = self._ensure()
+        if isinstance(pages, np.ndarray):
+            pages = torch.from_numpy(np.ascontiguousarray(pages).reshape(-1))
+        if not isinstance(pages, torch.Tensor) or pages.dtype != torch.uint8:
+            raise ValueError("RTDETRv2.forward_u8: pages must be a uint8 torch tensor or numpy array")
+        pages = pages.detach().contiguous().reshape(-1)
+        if pages.is_cuda and pages.device != self.cuda_device():
+            raise ValueError("RTDETRv2.forward_u8: pages on %s, the model runs on %s" % (pages.device, self.cuda_device()))
+        recs = np.ascontiguousarray(srcs, dtype=np.dtype(_lib.YtkRtdetrSrc))
+        n = len(recs)
+        logits = torch.empty((n, self.num_queries, self.num_classes), dtype=torch.float32, device=pages.device)
+        boxes = torch.empty((n, self.num_queries, 4), dtype=torch.float32, device=pages.device)
+        on_dev = 1 if pages.is_cuda else 0
+        _lib.check(_lib.lib().ytk_rtdetr_forward_u8(h, pages.data_ptr(), on_dev, pages.numel(), recs.ctypes.data, n,
+                                                    logits.data_ptr(), boxes.data_ptr(), on_dev, _stream_ptr(stream)))
+        return {"pred_logits": logits, "pred_boxes": boxes}
+
     def flops(self, n=1):
         return _lib.lib().ytk_rtdetr_flops(self._ensure(), n)
 

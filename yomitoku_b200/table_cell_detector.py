@@ -15,7 +15,7 @@ import torch
 from .base import BaseModelCatalog, BaseModule, logger
 from .config import TableCellParserRTDETRv2Config, load_config
 from .document_analyzer import calc_iou, is_bottom_adjacent, is_contained, is_right_adjacent
-from .layout_parser import _area, filter_contained_rectangles_across_categories, rtdetr_input_tensor
+from .layout_parser import _area, filter_contained_rectangles_across_categories, rtdetr_device_forward, rtdetr_input_tensor
 from .models import RTDETRv2
 from .postprocessor import RTDETRPostProcessor
 from .schemas import CellSchema, RegionSchema, TableDetectorSchema
@@ -221,11 +221,17 @@ class CellDetector(BaseModule):
 
     def __call__(self, img, tables):
         """BGR page + the layout parser's tables -> List[TableDetectorSchema], tables without cells left out."""
-        data = self.preprocess(img, tables)
         outputs = []
-        if not data:
+        if not tables:
             return outputs
-        preds = self.model(torch.cat([d["tensor"] for d in data]))        # every table of the page in one batch
+        # every table of the page in one batch, resized on the device when rtdetr_device_forward applies
+        boxes = [[int(v) for v in table.box] for table in tables]
+        dev = rtdetr_device_forward(self.model, [img], [(0, b) for b in boxes])
+        if dev is not None:
+            preds, data = dev[0], [{"size": s, "offset": (b[0], b[1])} for s, b in zip(dev[1], boxes)]
+        else:
+            data = self.preprocess(img, tables)
+            preds = self.model(torch.cat([d["tensor"] for d in data]))
         for i, (d, table) in enumerate(zip(data, tables)):
             cells, kv_regions, grid_regions = self.postprocess({k: v[i:i + 1] for k, v in preds.items()}, d, table.box)
             if not cells:

@@ -12,7 +12,7 @@ import torch
 from .base import BaseModelCatalog, BaseModule, logger
 from .config import TableStructureRecognizerRTDETRv2Config
 from .document_analyzer import _intersection, is_contained
-from .layout_parser import filter_contained_rectangles_within_category, rtdetr_input_tensor
+from .layout_parser import filter_contained_rectangles_within_category, rtdetr_device_forward, rtdetr_input_tensor
 from .models import RTDETRv2
 from .postprocessor import RTDETRPostProcessor
 from .schemas import TableStructureRecognizerSchema
@@ -101,11 +101,21 @@ class TableStructureRecognizer(BaseModule):
         cells = filter_contained_cells_within_spancell(cells, [e["box"] for e in elements["span"]])
         return cells, rows, cols, spans
 
-    def __call__(self, img, table_boxes, vis=None):
+    def _infer(self, img, table_boxes, pages_dev=None):
+        """(outputs on the host, per table {"size", "offset"}) for every table of the page in one batch: resized on the
+        device when rtdetr_device_forward applies, else `preprocess` on the host."""
+        boxes = [[int(v) for v in box] for box in table_boxes]
+        dev = rtdetr_device_forward(self.model, [img], [(0, b) for b in boxes], pages_dev)
+        if dev is not None:
+            return dev[0], [{"size": s, "offset": (b[0], b[1])} for s, b in zip(dev[1], boxes)]
         data = self.preprocess(img, table_boxes)
+        return self.model(torch.cat([d["tensor"] for d in data])), data
+
+    def __call__(self, img, table_boxes, vis=None, pages_dev=None):
+        """pages_dev (optional): `img` already on the device as upload_pages([img], ...) made it."""
         outputs = []
-        if data:
-            preds = self.model(torch.cat([d["tensor"] for d in data]))       # every table of the page in one batch
+        if len(table_boxes):
+            preds, data = self._infer(img, table_boxes, pages_dev)
             for i, d in enumerate(data):
                 table = self.postprocess({k: v[i:i + 1] for k, v in preds.items()}, d)
                 if table.n_row > 0 and table.n_col > 0:
