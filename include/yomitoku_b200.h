@@ -81,6 +81,28 @@ int ytk_op_attention_f16(const void* Q, long long ldq, long long q_rows, const v
  * Asynchronous on the stream. */
 int ytk_op_topk_f32(const float* scores_dev, int n, int L, int K, int* out_idx_dev, void* cuda_stream);
 
+/* Multi-scale deformable attention core of the RT-DETRv2 decoder (reference models/layers/rtdetrv2_decoder.py:306-388,
+ * grid_sample bilinear, zero padding, align_corners=False), rows = n_img * K queries.  All pointers on the device:
+ *   ow    fp32 [rows, ldo]: per row heads * P * 2 sampling offsets (x, y per point), then heads * P attention logits
+ *   ref   fp32 [rows, 4]: reference boxes (cx, cy, w, h); sampling location = ref.xy + off / points[l] * ref.wh * offset_scale
+ *   value fp16 level-major: level l of image i is rows [off[l] * n_img + i * h[l] * w[l], ...) with off = prefix sum of
+ *         h * w; head hd reads columns [voff + hd * head_dim, ...) of rows with pitch ldv
+ *   out   fp16 [rows, ldout]: columns [0, heads * head_dim) are written, nothing else
+ * level_h / level_w / level_points: host arrays of n_levels (1..4) entries; head_dim 32 and 12 points per head in all.
+ * Asynchronous on the stream; invalid arguments are an error, not a launch. */
+int ytk_op_deform_attn_f16(const float* ow, long long ldo, const float* ref, const void* value, long long ldv, int voff,
+                           const int* level_h, const int* level_w, const int* level_points, int n_levels, int n_img, int K,
+                           int heads, int head_dim, float offset_scale, void* out, long long ldout, void* cuda_stream);
+
+/* LayerNorm over the rows of x fp32 [M, D] (device).  If addvec != NULL every row first gets
+ * addvec[(row % period) + r0, :] added, r0 = *add_row0_dev if that is non-NULL, else add_row0; writeback != 0 stores the
+ * sum back to x.  Statistics run over the first d_real features (the rest is zero padding: zero in x, gamma, beta and
+ * addvec).  Outputs, each optional: out_f16 [M, D] fp16, out_f32 [M, D] fp32.  D <= 1024, D and d_real multiples of 4,
+ * 16-byte aligned fp32 pointers.  Asynchronous on the stream; invalid arguments are an error, not a launch. */
+int ytk_op_layernorm_f32(float* x, int M, int D, int d_real, const float* gamma, const float* beta, float eps,
+                         void* out_f16, float* out_f32, const float* addvec, int period, const int* add_row0_dev,
+                         int add_row0, int writeback, void* cuda_stream);
+
 /* ---- Device-side front half of the DBNet post-processing (reference postprocessor/dbnet_postporcessor.py:39-82:
  * binarize, findContours, and the pixel work of minAreaRect / box_score_fast).  One record per horizontal run of an
  * 8-connected component of (prob > thresh). ---- */
@@ -188,6 +210,18 @@ double ytk_parseq_last_flops(ytk_parseq* h);
 int ytk_parseq_last_steps(ytk_parseq* h);
 /* CUDA-event times (ms) of the last forward: encoder, AR decode, refinement, output copies */
 void ytk_parseq_last_phase_ms(ytk_parseq* h, float* ms4);
+
+/* op level, for the parity tests: the single-query attention of the AR decoder.  One query per (row, head), head dim
+ * D / heads in {32, 48, 64, 96}, fp16 operands with rows of D (queries) and [K | V] rows of 2 * D (keys / values),
+ * 16-byte aligned; out [B, D] fp16.
+ *   mode 0 (self-attention of AR step i = *step_dev, a device int with 0 <= i < S <= 800): q [S, D], kv [B][S][2D]; row b
+ *          attends with q[i] to its keys 0..i
+ *   mode 1 (cross-attention): q [B, D], kv = encoder memory [tokens][2D]; row b attends with q[b] to the ntok rows from
+ *          tok_off of crops[b] (host records; 1 <= ntok <= 800, the other fields are not read); S and step_dev are unused
+ * Asynchronous on the stream (mode 1 uploads the records to a buffer it allocates and frees on the stream); invalid
+ * arguments are an error, not a launch. */
+int ytk_op_single_query_attn_f16(int mode, const void* q, const void* kv, int B, int S, int D, int heads,
+                                 const int* step_dev, const ytk_crop* crops, void* out, void* cuda_stream);
 
 /* ---- Device-side crop extraction: replaces the pixel work of ParseqDataset._preprocess_on (reference
  * src/yomitoku/data/dataset.py:106-123): extract_roi_with_perspective (data/functions.py:301-333, cv2.warpPerspective),

@@ -217,7 +217,10 @@ def _attn_case(hd, heads, lens, masked, impl, seed=0, q_shared=None, kpads=None,
 
 @pytest.mark.parametrize("impl", [1, 2])     # 1: mma.sync kernel, 2: wgmma kernel (default)
 @pytest.mark.parametrize("hd,heads,lens", [(96, 8, [132, 92, 48, 200, 400, 129, 128, 4]), (32, 6, [800, 320, 64, 8, 72]),
-                                           (48, 8, [100, 260]), (64, 8, [160, 96, 31])])
+                                           (48, 8, [100, 260]), (64, 8, [160, 96, 31]),
+                                           # RT-DETRv2: AIFI at 960 / 640, cell decoder (1500 queries), layout decoder
+                                           (32, 8, [900, 900]), (32, 8, [400] * 3), (32, 8, [1500, 1500]),
+                                           (32, 8, [300] * 4)])
 def test_attention_tc_vs_torch(hd, heads, lens, impl):
     """Both attention kernels (parseq_ops.cu mma.sync, attn_tc.cu wgmma) vs fp32 softmax attention on the same fp16 operands: the only rounding the
     kernel adds is P and O in fp16 (2^-11 relative)."""

@@ -40,6 +40,15 @@ def _declare(lib):
                                          c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]
     lib.ytk_op_topk_f32.restype = c_int
     lib.ytk_op_topk_f32.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]
+    lib.ytk_op_deform_attn_f16.restype = c_int
+    lib.ytk_op_deform_attn_f16.argtypes = [c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_int, c_void_p, c_void_p, c_void_p,
+                                           c_int, c_int, c_int, c_int, c_int, ctypes.c_float, c_void_p, c_ll, c_void_p]
+    lib.ytk_op_layernorm_f32.restype = c_int
+    lib.ytk_op_layernorm_f32.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, ctypes.c_float, c_void_p,
+                                         c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_void_p]
+    lib.ytk_op_single_query_attn_f16.restype = c_int
+    lib.ytk_op_single_query_attn_f16.argtypes = [c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
+                                                 c_void_p, c_void_p, c_void_p]
 
 
 class YtkAttnSeq(ctypes.Structure):

@@ -184,6 +184,128 @@ int ytk_op_topk_f32(const float* scores_dev, int n, int L, int K, int* out_idx_d
                                                                                                          : YTK_OK;
 }
 
+static bool misaligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; }
+
+int ytk_op_deform_attn_f16(const float* ow, long long ldo, const float* ref, const void* value, long long ldv, int voff,
+                           const int* level_h, const int* level_w, const int* level_points, int n_levels, int n_img, int K,
+                           int heads, int head_dim, float offset_scale, void* out, long long ldout, void* cuda_stream) {
+    if (!ow || !ref || !value || !out || !level_h || !level_w || !level_points) {
+        ytk::set_error("ytk_op_deform_attn_f16: null argument");
+        return YTK_ERR;
+    }
+    if (n_levels < 1 || n_levels > ytk::RtLevels::kMax) {
+        ytk::set_error("ytk_op_deform_attn_f16: %d levels unsupported (1..%d)", n_levels, ytk::RtLevels::kMax);
+        return YTK_ERR;
+    }
+    if (n_img < 1 || K < 1 || heads < 1 || head_dim < 1 || voff < 0) {
+        ytk::set_error("ytk_op_deform_attn_f16: non-positive size (n_img %d, K %d, heads %d, head_dim %d, voff %d)", n_img,
+                       K, heads, head_dim, voff);
+        return YTK_ERR;
+    }
+    ytk::RtLevels lv;
+    lv.n = n_levels;
+    lv.off[0] = 0;
+    int P = 0;
+    for (int l = 0; l < n_levels; ++l) {
+        if (level_h[l] < 1 || level_w[l] < 1 || level_points[l] < 1) {
+            ytk::set_error("ytk_op_deform_attn_f16: level %d is %dx%d with %d points", l, level_h[l], level_w[l],
+                           level_points[l]);
+            return YTK_ERR;
+        }
+        lv.h[l] = level_h[l];
+        lv.w[l] = level_w[l];
+        lv.points[l] = level_points[l];
+        lv.off[l + 1] = lv.off[l] + level_h[l] * level_w[l];
+        P += level_points[l];
+    }
+    lv.total = lv.off[n_levels];
+    if (ldo < 3LL * heads * P || ldv < (long long)voff + (long long)heads * head_dim || ldout < (long long)heads * head_dim ||
+        misaligned(ref, 16)) {
+        ytk::set_error("ytk_op_deform_attn_f16: pitches too small (ldo %lld, ldv %lld with voff %d, ldout %lld) or ref not "
+                       "16-byte aligned", ldo, ldv, voff, ldout);
+        return YTK_ERR;
+    }
+    return ytk::launch_rt_deform_attn(ow, ldo, ref, value, ldv, voff, lv, n_img, K, heads, head_dim, offset_scale, out,
+                                      ldout, static_cast<cudaStream_t>(cuda_stream))
+               ? YTK_ERR
+               : YTK_OK;
+}
+
+int ytk_op_layernorm_f32(float* x, int M, int D, int d_real, const float* gamma, const float* beta, float eps,
+                         void* out_f16, float* out_f32, const float* addvec, int period, const int* add_row0_dev,
+                         int add_row0, int writeback, void* cuda_stream) {
+    if (!x || !gamma || !beta) {
+        ytk::set_error("ytk_op_layernorm_f32: null argument");
+        return YTK_ERR;
+    }
+    // the first table row comes from *add_row0_dev when that is given: add_row0 is read only without it
+    if (M < 1 || (addvec && (period < 1 || (!add_row0_dev && add_row0 < 0)))) {
+        ytk::set_error("ytk_op_layernorm_f32: %d rows, addvec period %d / first row %d unsupported", M, period, add_row0);
+        return YTK_ERR;
+    }
+    if (misaligned(x, 16) || misaligned(gamma, 16) || misaligned(beta, 16) || misaligned(out_f32, 16) ||
+        misaligned(addvec, 16) || misaligned(out_f16, 8)) {
+        ytk::set_error("ytk_op_layernorm_f32: fp32 pointers must be 16-byte and out_f16 8-byte aligned");
+        return YTK_ERR;
+    }
+    return ytk::launch_layernorm(x, M, D, d_real, gamma, beta, eps, out_f16, out_f32, addvec, period, add_row0_dev,
+                                 add_row0, writeback, static_cast<cudaStream_t>(cuda_stream))
+               ? YTK_ERR
+               : YTK_OK;
+}
+
+int ytk_op_single_query_attn_f16(int mode, const void* q, const void* kv, int B, int S, int D, int heads,
+                                 const int* step_dev, const ytk_crop* crops, void* out, void* cuda_stream) {
+    constexpr int kMaxTokens = ytk::kMaxMem;   // keys per (row, head) the kernel's shared-memory score row holds
+    if (mode != 0 && mode != 1) {
+        ytk::set_error("ytk_op_single_query_attn_f16: mode %d unknown (0 = self, 1 = cross)", mode);
+        return YTK_ERR;
+    }
+    if (!q || !kv || !out || (mode == 0 && !step_dev) || (mode == 1 && !crops)) {
+        ytk::set_error("ytk_op_single_query_attn_f16: null argument");
+        return YTK_ERR;
+    }
+    const int hd = heads > 0 ? D / heads : 0;
+    if (B < 1 || heads < 1 || D % heads != 0 || (hd != 32 && hd != 48 && hd != 64 && hd != 96)) {
+        ytk::set_error("ytk_op_single_query_attn_f16: B %d, D %d, %d heads unsupported (head dim 32/48/64/96)", B, D,
+                       heads);
+        return YTK_ERR;
+    }
+    if (mode == 0 && (S < 1 || S > kMaxTokens)) {
+        ytk::set_error("ytk_op_single_query_attn_f16: S %d unsupported (1..%d)", S, kMaxTokens);
+        return YTK_ERR;
+    }
+    if (misaligned(q, 16) || misaligned(kv, 16) || misaligned(out, 16)) {
+        ytk::set_error("ytk_op_single_query_attn_f16: q, kv and out must be 16-byte aligned");
+        return YTK_ERR;
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    if (mode == 0) return ytk::launch_dec_self_attn(q, kv, B, S, D, heads, step_dev, out, st) ? YTK_ERR : YTK_OK;
+    std::vector<ytk::CropDesc> descs(B);
+    for (int i = 0; i < B; ++i) {
+        const ytk_crop& c = crops[i];
+        if (c.ntok < 1 || c.ntok > kMaxTokens || c.tok_off < 0) {
+            ytk::set_error("ytk_op_single_query_attn_f16: crop %d has %d tokens from row %d (1..%d tokens)", i, c.ntok,
+                           c.tok_off, kMaxTokens);
+            return YTK_ERR;
+        }
+        descs[i] = ytk::CropDesc{c.pix_off, c.w, c.wp, c.tok_off, c.ntok, c.group};
+    }
+    const size_t bytes = descs.size() * sizeof(ytk::CropDesc);
+    void* descs_dev = nullptr;
+    if (cudaMallocAsync(&descs_dev, bytes, st) != cudaSuccess) {
+        cudaGetLastError();
+        ytk::set_error("ytk_op_single_query_attn_f16: cudaMallocAsync(%zu) failed", bytes);
+        return YTK_ERR;
+    }
+    // pageable source: the call returns after the records are staged, so `descs` may go out of scope
+    int rc = cudaMemcpyAsync(descs_dev, descs.data(), bytes, cudaMemcpyHostToDevice, st) != cudaSuccess;
+    if (rc) ytk::set_error("ytk_op_single_query_attn_f16: record upload failed");
+    if (!rc) rc = ytk::launch_dec_cross_attn(q, kv, reinterpret_cast<const ytk::CropDesc*>(descs_dev), B, D, heads, out, st);
+    cudaFreeAsync(descs_dev, st);
+    return rc ? YTK_ERR : YTK_OK;
+}
+
 static_assert(sizeof(ytk_db_run) == sizeof(ytk::DbRun), "ytk_db_run and ytk::DbRun must have one layout");
 
 int ytk_dbnet_post_front(const float* prob_dev, int n_pages, int H, int W, float thresh, void* scratch_dev,

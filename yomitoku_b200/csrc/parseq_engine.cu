@@ -434,8 +434,8 @@ int ParseqEngine::forward(const ParseqBatch& b, int* ids_out, float* probs_out, 
     for (const CropDesc& d : b.descs) {
         T = std::max<long long>(T, (long long)d.tok_off + d.ntok);
         max_ntok = std::max(max_ntok, d.ntok);
-        if (d.ntok > 800) {
-            set_error("crop with %d encoder tokens exceeds the supported 800", d.ntok);
+        if (d.ntok > kMaxMem) {
+            set_error("crop with %d encoder tokens exceeds the supported %d", d.ntok, kMaxMem);
             return 1;
         }
     }

@@ -188,7 +188,8 @@ int launch_layernorm(float* x, int M, int D, int d_real, const float* gamma, con
                      void* out_bf16, float* out_f32, const float* addvec, int period, const int* add_row0_dev,
                      int add_row0, int writeback, cudaStream_t st) {
     if (D > 128 * kLnVec || (D & 3) != 0 || (d_real & 3) != 0 || d_real > D || d_real <= 0) {
-        set_error("layernorm: D=%d unsupported (multiple of 4, <= %d)", D, 128 * kLnVec);
+        set_error("layernorm: D=%d / d_real=%d unsupported (multiples of 4, 0 < d_real <= D <= %d)", D, d_real,
+                  128 * kLnVec);
         return 1;
     }
     if (M <= 0) return 0;
@@ -497,7 +498,6 @@ int launch_flash_attention(const void* Q, long long ldq, long long q_rows, const
 // =================================================================================================== decoder attention
 constexpr int kMaxS = 101;
 constexpr int kMaxHd = 96;
-constexpr int kMaxMem = 800;
 
 // =================================================================================================== single-query attention
 // Both attentions of an AR step have ONE query per (row, head) against a strided list of cached K/V rows:

@@ -52,6 +52,10 @@ int launch_attention_tc(const void* Q, long long ldq, long long q_rows, const vo
                         long long kv_rows, void* O, long long ldo, const SeqDesc* seqs, int nseq, int heads,
                         int head_dim, int masked, cudaStream_t st);
 
+// Keys per (row, head) the single-query attention holds scores for (its shared-memory row): the most encoder tokens a
+// crop may have, and the most AR positions.
+constexpr int kMaxMem = 800;
+
 // AR attention, one query per (row, head) (single_query_attn_kernel):
 //  self : step i = *step_dev, q = q_shared[i], keys 0..i of the row's content K/V cache [row][S positions][2D] -> out[row]
 //  cross: q = qc[row], keys = the row's encoder memory K/V (projected once)                                  -> out[row]
