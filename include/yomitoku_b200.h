@@ -223,6 +223,36 @@ void ytk_parseq_last_phase_ms(ytk_parseq* h, float* ms4);
 int ytk_op_single_query_attn_f16(int mode, const void* q, const void* kv, int B, int S, int D, int heads,
                                  const int* step_dev, const ytk_crop* crops, void* out, void* cuda_stream);
 
+/* op level, for the parity tests: the DBNet detector's own kernels, each called as the engine calls it.  Activations
+ * are NHWC fp16 on the device, 16-byte aligned; weights are the reference's fp32 layouts on the host, packed by the
+ * code the engine's loader uses (with no BatchNorm: the bias is the whole shift).  Asynchronous on the stream (weights
+ * and scratch go to buffers allocated and freed on it); invalid arguments are an error, not a launch.
+ *   preprocess  n BGR u8 pages [n, H0, W0, 3] -> the stem's canvas [n, Hn+6, Wn+8, 8], all of it written: pixel (h, w)
+ *               at (h+3, w+3), channels 0..2 = cv2.resize(INTER_AREA) / 255 with the mean / std applied by position
+ *               to B, G, R, zero border and zero channels 3..7.  Hn <= H0 and Wn <= W0 (decimation only).
+ *   stem        7x7 / stride 2 / pad 3 conv (w [64][3][7][7], bias [64]) + ReLU over that canvas -> out
+ *               [n, Hn/2, Wn/2, 64]; Hn and Wn multiples of 32.
+ *   maxpool     max_pool2d(3, 2, 1): in [n, H, W, C] -> out [n, (H+1)/2, (W+1)/2, C]; C a multiple of 8.
+ *   upsample    bilinear, align_corners=False: src [n, Hs, Ws, C] -> channels [coff, coff+C) of dst [n, Hd, Wd, ldd],
+ *               written (accumulate = 0) or added (accumulate != 0); coff and ldd multiples of 8, coff + C <= ldd.
+ *   asf         the scale fusion after its 3x3 conv: a [n, H, W, 64], fuse [n, H, W, 256] rescaled in place by group;
+ *               w1 [16][64] / w2 [64][16] fp32 on the device, sp3 [9] / att [4][64] on the host.  Optional outputs
+ *               (device, or NULL): gvec [n, 64] = the channel gate, m [n, H, W] fp32 = the channel-mean map.
+ *   head        ConvT(64->64, 2, 2) + ReLU, then ConvT(64->1, 2, 2) + sigmoid in one GEMM epilogue: x [n, H, W, 64]
+ *               -> prob [n, 4H, 4W] fp32 (8-byte aligned); w1 [64][64][2][2], b1 [64], w2 [64][1][2][2], b2. */
+int ytk_op_dbnet_preprocess_u8(const uint8_t* src_dev, int n, int H0, int W0, int Hn, int Wn, void* canvas_dev,
+                               void* cuda_stream);
+int ytk_op_dbnet_stem_f16(const void* canvas_dev, int n, int Hn, int Wn, const float* w_host, const float* bias_host,
+                          void* out_dev, void* cuda_stream);
+int ytk_op_maxpool3x3s2_f16(const void* in, int n, int H, int W, int C, void* out, void* cuda_stream);
+int ytk_op_upsample_bilinear_f16(const void* src, int n, int Hs, int Ws, int C, void* dst, int Hd, int Wd, long long ldd,
+                                 int coff, int accumulate, void* cuda_stream);
+int ytk_op_asf_f16(const void* a, void* fuse, int n, int H, int W, const float* w1_dev, const float* w2_dev,
+                   const float* sp3_host, float sp1, const float* att_host, float* gvec_out, float* m_out,
+                   void* cuda_stream);
+int ytk_op_dbnet_head_f32(const void* x_dev, int n, int H, int W, const float* w1_host, const float* b1_host,
+                          const float* w2_host, float b2, float* prob_dev, void* cuda_stream);
+
 /* ---- Device-side crop extraction: replaces the pixel work of ParseqDataset._preprocess_on (reference
  * src/yomitoku/data/dataset.py:106-123): extract_roi_with_perspective (data/functions.py:301-333, cv2.warpPerspective),
  * rotate_text_image (:336-350) and resize_with_padding / resize_with_dynamic_padding (:379-439, cv2.resize INTER_AREA +

@@ -1,6 +1,6 @@
-"""CPU: the op-level entries of the deformable attention, LayerNorm and single-query attention kernels refuse invalid
-arguments on the host - a nonzero status, a message that names the problem, and no kernel launch.  The pointers are
-never dereferenced on these paths, so plain addresses stand in for device buffers."""
+"""CPU: the op-level entries of the deformable attention, LayerNorm and single-query attention kernels and of the DBNet
+detector's kernels refuse invalid arguments on the host - a nonzero status, a message that names the problem, and no
+kernel launch.  The pointers are never dereferenced on these paths, so plain addresses stand in for device buffers."""
 import ctypes
 
 import pytest
@@ -107,4 +107,114 @@ def _sqa(lib, mode=0, q=P, kv=P, B=4, S=26, D=384, heads=8, step=P, crops=None, 
 def test_single_query_attn_refusals(lib, kwargs, fragment):
     before = lib.ytk_launch_count()
     _refused(lib, _sqa(lib, **kwargs), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+# ======================================================================================================== DBNet
+W_HOST = (ctypes.c_float * (64 * 64 * 4))()      # host weights: large enough for every entry, never read on refusal
+
+
+def _prep(lib, src=P, n=1, H0=1200, W0=1600, Hn=1184, Wn=1600, canvas=P):
+    return lib.ytk_op_dbnet_preprocess_u8(src, n, H0, W0, Hn, Wn, canvas, None)
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(src=None), b"null argument"), (dict(canvas=None), b"null argument"),
+    (dict(n=0), b"non-positive size"), (dict(H0=0), b"non-positive size"), (dict(W0=-1), b"non-positive size"),
+    (dict(Hn=0), b"non-positive size"), (dict(Wn=0), b"non-positive size"),
+    # the upscale that ytk_dbnet_forward_u8 refuses too
+    (dict(Hn=1216), b"1200x1600 -> 1216x1600 is an upscale"), (dict(Wn=1632), b"1200x1600 -> 1184x1632 is an upscale"),
+    (dict(canvas=P + 8), b"16-byte aligned"),
+])
+def test_dbnet_preprocess_refusals(lib, kwargs, fragment):
+    before = lib.ytk_launch_count()
+    _refused(lib, _prep(lib, **kwargs), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+def _stem(lib, canvas=P, n=1, Hn=96, Wn=160, w=W_HOST, bias=W_HOST, out=P):
+    return lib.ytk_op_dbnet_stem_f16(canvas, n, Hn, Wn, w, bias, out, None)
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(canvas=None), b"null argument"), (dict(w=None), b"null argument"), (dict(bias=None), b"null argument"),
+    (dict(out=None), b"null argument"),
+    (dict(n=0), b"n 0, input 96x160 unsupported"), (dict(Hn=80), b"input 80x160 unsupported (multiples of 32)"),
+    (dict(Wn=100), b"input 96x100 unsupported"), (dict(Hn=0), b"input 0x160 unsupported"),
+    (dict(Wn=-32), b"input 96x-32 unsupported"),
+    (dict(canvas=P + 8), b"16-byte aligned"), (dict(out=P + 2), b"16-byte aligned"),
+])
+def test_dbnet_stem_refusals(lib, kwargs, fragment):
+    before = lib.ytk_launch_count()
+    _refused(lib, _stem(lib, **kwargs), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+def _pool(lib, src=P, n=1, H=320, W=320, C=64, out=P):
+    return lib.ytk_op_maxpool3x3s2_f16(src, n, H, W, C, out, None)
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(src=None), b"null argument"), (dict(out=None), b"null argument"),
+    (dict(n=0), b"n 0, 320x320, C 64 unsupported"), (dict(H=0), b"0x320"), (dict(W=0), b"320x0"),
+    (dict(C=12), b"C 12 unsupported"), (dict(C=0), b"C 0 unsupported"),
+    (dict(src=P + 8), b"16-byte aligned"), (dict(out=P + 4), b"16-byte aligned"),
+])
+def test_maxpool_refusals(lib, kwargs, fragment):
+    before = lib.ytk_launch_count()
+    _refused(lib, _pool(lib, **kwargs), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+def _up(lib, src=P, n=1, Hs=37, Ws=50, C=64, dst=P, Hd=74, Wd=100, ldd=256, coff=64, acc=0):
+    return lib.ytk_op_upsample_bilinear_f16(src, n, Hs, Ws, C, dst, Hd, Wd, ldd, coff, acc, None)
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(src=None), b"null argument"), (dict(dst=None), b"null argument"),
+    (dict(n=0), b"n 0, 37x50 -> 74x100"), (dict(Hs=0), b"0x50 -> 74x100"), (dict(Wd=0), b"37x50 -> 74x0"),
+    (dict(C=20), b"C 20 unsupported"),
+    (dict(coff=200), b"channels [200, 264) do not fit a pitch of 256"),
+    (dict(C=64, coff=192, ldd=248), b"channels [192, 256) do not fit a pitch of 248"),
+    (dict(coff=4), b"channels [4, 68) do not fit"), (dict(coff=-8), b"channels [-8, 56) do not fit"),
+    (dict(ldd=260), b"a pitch of 260"),
+    (dict(src=P + 8), b"16-byte aligned"), (dict(dst=P + 2), b"16-byte aligned"),
+])
+def test_upsample_refusals(lib, kwargs, fragment):
+    before = lib.ytk_launch_count()
+    _refused(lib, _up(lib, **kwargs), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+def _asf(lib, a=P, fuse=P, n=1, H=296, W=400, w1=P, w2=P, sp3=W_HOST, att=W_HOST):
+    return lib.ytk_op_asf_f16(a, fuse, n, H, W, w1, w2, sp3, 0.5, att, None, None, None)
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(a=None), b"null argument"), (dict(fuse=None), b"null argument"), (dict(w1=None), b"null argument"),
+    (dict(w2=None), b"null argument"), (dict(sp3=None), b"null argument"), (dict(att=None), b"null argument"),
+    (dict(n=0), b"n 0, 296x400 unsupported"), (dict(n=65536), b"n 65536, 296x400 unsupported"),
+    (dict(H=0), b"0x400 unsupported"), (dict(W=-1), b"296x-1 unsupported"),
+    (dict(H=65536, W=32768), b"65536x32768 unsupported"),
+    (dict(a=P + 8), b"16-byte aligned"), (dict(fuse=P + 2), b"16-byte aligned"),
+])
+def test_asf_refusals(lib, kwargs, fragment):
+    before = lib.ytk_launch_count()
+    _refused(lib, _asf(lib, **kwargs), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+def _head(lib, x=P, n=1, H=37, W=50, w1=W_HOST, b1=W_HOST, w2=W_HOST, prob=P):
+    return lib.ytk_op_dbnet_head_f32(x, n, H, W, w1, b1, w2, 0.1, prob, None)
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(x=None), b"null argument"), (dict(w1=None), b"null argument"), (dict(b1=None), b"null argument"),
+    (dict(w2=None), b"null argument"), (dict(prob=None), b"null argument"),
+    (dict(n=0), b"non-positive size (n 0, 37x50)"), (dict(H=0), b"non-positive size"), (dict(W=-4), b"non-positive size"),
+    (dict(x=P + 8), b"x_dev must be 16-byte"), (dict(prob=P + 4), b"prob_dev 8-byte aligned"),
+])
+def test_dbnet_head_refusals(lib, kwargs, fragment):
+    before = lib.ytk_launch_count()
+    _refused(lib, _head(lib, **kwargs), fragment)
     assert lib.ytk_launch_count() == before

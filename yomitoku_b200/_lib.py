@@ -49,6 +49,21 @@ def _declare(lib):
     lib.ytk_op_single_query_attn_f16.restype = c_int
     lib.ytk_op_single_query_attn_f16.argtypes = [c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
                                                  c_void_p, c_void_p, c_void_p]
+    lib.ytk_op_dbnet_preprocess_u8.restype = c_int
+    lib.ytk_op_dbnet_preprocess_u8.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
+    lib.ytk_op_dbnet_stem_f16.restype = c_int
+    lib.ytk_op_dbnet_stem_f16.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
+    lib.ytk_op_maxpool3x3s2_f16.restype = c_int
+    lib.ytk_op_maxpool3x3s2_f16.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
+    lib.ytk_op_upsample_bilinear_f16.restype = c_int
+    lib.ytk_op_upsample_bilinear_f16.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_ll,
+                                                 c_int, c_int, c_void_p]
+    lib.ytk_op_asf_f16.restype = c_int
+    lib.ytk_op_asf_f16.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, ctypes.c_float,
+                                   c_void_p, c_void_p, c_void_p, c_void_p]
+    lib.ytk_op_dbnet_head_f32.restype = c_int
+    lib.ytk_op_dbnet_head_f32.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, ctypes.c_float,
+                                          c_void_p, c_void_p]
 
 
 class YtkAttnSeq(ctypes.Structure):

@@ -5,10 +5,12 @@
 #include <climits>
 #include <cmath>
 #include <cstdlib>
+#include <cstring>
 #include <map>
 #include <memory>
 #include <mutex>
 #include <tuple>
+#include <vector>
 
 #include "crop_ops.h"
 #include "dbnet_engine.h"
@@ -303,6 +305,199 @@ int ytk_op_single_query_attn_f16(int mode, const void* q, const void* kv, int B,
     if (rc) ytk::set_error("ytk_op_single_query_attn_f16: record upload failed");
     if (!rc) rc = ytk::launch_dec_cross_attn(q, kv, reinterpret_cast<const ytk::CropDesc*>(descs_dev), B, D, heads, out, st);
     cudaFreeAsync(descs_dev, st);
+    return rc ? YTK_ERR : YTK_OK;
+}
+
+// Allocates `bytes` on the stream and, if `host` is given, uploads it.  The copy is from pageable memory: the call
+// returns after the data is staged, so `host` may go out of scope.  The caller frees the buffer with cudaFreeAsync.
+static void* stream_buffer(const void* host, size_t bytes, cudaStream_t st, const char* who) {
+    void* d = nullptr;
+    if (cudaMallocAsync(&d, bytes, st) != cudaSuccess) {
+        cudaGetLastError();
+        ytk::set_error("%s: cudaMallocAsync(%zu) failed", who, bytes);
+        return nullptr;
+    }
+    if (host && cudaMemcpyAsync(d, host, bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) {
+        cudaGetLastError();
+        cudaFreeAsync(d, st);
+        ytk::set_error("%s: upload of %zu bytes failed", who, bytes);
+        return nullptr;
+    }
+    return d;
+}
+
+int ytk_op_dbnet_preprocess_u8(const uint8_t* src_dev, int n, int H0, int W0, int Hn, int Wn, void* canvas_dev,
+                               void* cuda_stream) {
+    if (!src_dev || !canvas_dev) {
+        ytk::set_error("ytk_op_dbnet_preprocess_u8: null argument");
+        return YTK_ERR;
+    }
+    if (n < 1 || H0 < 1 || W0 < 1 || Hn < 1 || Wn < 1) {
+        ytk::set_error("ytk_op_dbnet_preprocess_u8: non-positive size (n %d, page %dx%d, input %dx%d)", n, H0, W0, Hn, Wn);
+        return YTK_ERR;
+    }
+    if (Hn > H0 || Wn > W0) {
+        ytk::set_error("ytk_op_dbnet_preprocess_u8: %dx%d -> %dx%d is an upscale; INTER_AREA decimation only", H0, W0, Hn,
+                       Wn);
+        return YTK_ERR;
+    }
+    if (misaligned(canvas_dev, 16)) {
+        ytk::set_error("ytk_op_dbnet_preprocess_u8: canvas_dev must be 16-byte aligned");
+        return YTK_ERR;
+    }
+    return ytk::launch_preprocess(src_dev, n, H0, W0, Hn, Wn, canvas_dev, static_cast<cudaStream_t>(cuda_stream))
+               ? YTK_ERR
+               : YTK_OK;
+}
+
+int ytk_op_dbnet_stem_f16(const void* canvas_dev, int n, int Hn, int Wn, const float* w_host, const float* bias_host,
+                          void* out_dev, void* cuda_stream) {
+    if (!canvas_dev || !w_host || !bias_host || !out_dev) {
+        ytk::set_error("ytk_op_dbnet_stem_f16: null argument");
+        return YTK_ERR;
+    }
+    if (n < 1 || Hn < 32 || Wn < 32 || Hn % 32 || Wn % 32) {
+        ytk::set_error("ytk_op_dbnet_stem_f16: n %d, input %dx%d unsupported (multiples of 32)", n, Hn, Wn);
+        return YTK_ERR;
+    }
+    if (misaligned(canvas_dev, 16) || misaligned(out_dev, 16)) {
+        ytk::set_error("ytk_op_dbnet_stem_f16: canvas_dev and out_dev must be 16-byte aligned");
+        return YTK_ERR;
+    }
+    // one buffer: packed weights [64][7][64] 16-bit, then the bias [64] fp32
+    std::vector<uint16_t> wp;
+    ytk::pack_stem_weights(w_host, nullptr, &wp);
+    const size_t wbytes = wp.size() * 2;
+    std::vector<uint8_t> blob(wbytes + 64 * 4);
+    memcpy(blob.data(), wp.data(), wbytes);
+    memcpy(blob.data() + wbytes, bias_host, 64 * 4);
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    uint8_t* d = static_cast<uint8_t*>(stream_buffer(blob.data(), blob.size(), st, "ytk_op_dbnet_stem_f16"));
+    if (!d) return YTK_ERR;
+    ytk::Epilogue e;
+    e.bias = reinterpret_cast<const float*>(d + wbytes);
+    e.out = out_dev;
+    e.ldc = 64;
+    e.act = ytk::ACT_RELU;
+    ytk::GemmPlan plan;
+    int rc = ytk::stem_plan_create(&plan, canvas_dev, n, Hn, Wn, d, e);
+    if (!rc) rc = ytk::gemm_plan_launch(&plan, st);
+    cudaFreeAsync(d, st);
+    return rc ? YTK_ERR : YTK_OK;
+}
+
+int ytk_op_maxpool3x3s2_f16(const void* in, int n, int H, int W, int C, void* out, void* cuda_stream) {
+    if (!in || !out) {
+        ytk::set_error("ytk_op_maxpool3x3s2_f16: null argument");
+        return YTK_ERR;
+    }
+    if (n < 1 || H < 1 || W < 1 || C < 8 || C % 8) {
+        ytk::set_error("ytk_op_maxpool3x3s2_f16: n %d, %dx%d, C %d unsupported (C a positive multiple of 8)", n, H, W, C);
+        return YTK_ERR;
+    }
+    if (misaligned(in, 16) || misaligned(out, 16)) {
+        ytk::set_error("ytk_op_maxpool3x3s2_f16: in and out must be 16-byte aligned");
+        return YTK_ERR;
+    }
+    return ytk::launch_maxpool(in, out, n, H, W, C, static_cast<cudaStream_t>(cuda_stream)) ? YTK_ERR : YTK_OK;
+}
+
+int ytk_op_upsample_bilinear_f16(const void* src, int n, int Hs, int Ws, int C, void* dst, int Hd, int Wd, long long ldd,
+                                 int coff, int accumulate, void* cuda_stream) {
+    if (!src || !dst) {
+        ytk::set_error("ytk_op_upsample_bilinear_f16: null argument");
+        return YTK_ERR;
+    }
+    if (n < 1 || Hs < 1 || Ws < 1 || Hd < 1 || Wd < 1 || C < 8 || C % 8) {
+        ytk::set_error("ytk_op_upsample_bilinear_f16: n %d, %dx%d -> %dx%d, C %d unsupported (C a positive multiple of 8)",
+                       n, Hs, Ws, Hd, Wd, C);
+        return YTK_ERR;
+    }
+    if (coff < 0 || coff % 8 || ldd % 8 || (long long)coff + C > ldd) {
+        ytk::set_error("ytk_op_upsample_bilinear_f16: channels [%d, %d) do not fit a pitch of %lld (coff and ldd multiples "
+                       "of 8)", coff, coff + C, ldd);
+        return YTK_ERR;
+    }
+    if (misaligned(src, 16) || misaligned(dst, 16)) {
+        ytk::set_error("ytk_op_upsample_bilinear_f16: src and dst must be 16-byte aligned");
+        return YTK_ERR;
+    }
+    return ytk::launch_upsample(src, n, Hs, Ws, C, dst, Hd, Wd, ldd, coff, accumulate,
+                                static_cast<cudaStream_t>(cuda_stream))
+               ? YTK_ERR
+               : YTK_OK;
+}
+
+int ytk_op_asf_f16(const void* a, void* fuse, int n, int H, int W, const float* w1_dev, const float* w2_dev,
+                   const float* sp3_host, float sp1, const float* att_host, float* gvec_out, float* m_out,
+                   void* cuda_stream) {
+    if (!a || !fuse || !w1_dev || !w2_dev || !sp3_host || !att_host) {
+        ytk::set_error("ytk_op_asf_f16: null argument");
+        return YTK_ERR;
+    }
+    // the pooling grid is (chunks, n): n is bounded by gridDim.y
+    if (n < 1 || n > 65535 || H < 1 || W < 1 || (long long)H * W > INT_MAX) {
+        ytk::set_error("ytk_op_asf_f16: n %d, %dx%d unsupported (1 <= n <= 65535)", n, H, W);
+        return YTK_ERR;
+    }
+    if (misaligned(a, 16) || misaligned(fuse, 16)) {
+        ytk::set_error("ytk_op_asf_f16: a and fuse must be 16-byte aligned");
+        return YTK_ERR;
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    // fp32 scratch on the stream: gsum partials, gmean, and the outputs the caller does not want
+    const size_t n_gsum = (size_t)n * ytk::kAsfPoolChunks * 64, n_gvec = gvec_out ? 0 : (size_t)n * 64,
+                 n_m = m_out ? 0 : (size_t)n * H * W;
+    float* d = static_cast<float*>(stream_buffer(nullptr, (n_gsum + n + n_gvec + n_m) * 4, st, "ytk_op_asf_f16"));
+    if (!d) return YTK_ERR;
+    float* gsum = d;
+    float* gmean = gsum + n_gsum;
+    float* gvec = gvec_out ? gvec_out : gmean + n;
+    float* m = m_out ? m_out : gmean + n + n_gvec;
+    const int rc = ytk::launch_asf(a, fuse, n, H, W, w1_dev, w2_dev, sp3_host, sp1, att_host, gsum, gvec, gmean, m, st);
+    cudaFreeAsync(d, st);
+    return rc ? YTK_ERR : YTK_OK;
+}
+
+int ytk_op_dbnet_head_f32(const void* x_dev, int n, int H, int W, const float* w1_host, const float* b1_host,
+                          const float* w2_host, float b2, float* prob_dev, void* cuda_stream) {
+    if (!x_dev || !w1_host || !b1_host || !w2_host || !prob_dev) {
+        ytk::set_error("ytk_op_dbnet_head_f32: null argument");
+        return YTK_ERR;
+    }
+    if (n < 1 || H < 1 || W < 1) {
+        ytk::set_error("ytk_op_dbnet_head_f32: non-positive size (n %d, %dx%d)", n, H, W);
+        return YTK_ERR;
+    }
+    if (misaligned(x_dev, 16) || misaligned(prob_dev, 8)) {
+        ytk::set_error("ytk_op_dbnet_head_f32: x_dev must be 16-byte and prob_dev 8-byte aligned");
+        return YTK_ERR;
+    }
+    // one buffer: GEMM rows [256][64] 16-bit, bias [256] fp32, final conv weights [4][64] fp32
+    std::vector<uint16_t> wp;
+    std::vector<float> bias, fin;
+    ytk::pack_convt_head(w1_host, b1_host, nullptr, nullptr, w2_host, &wp, &bias, &fin);
+    const size_t wbytes = wp.size() * 2, bbytes = bias.size() * 4;
+    std::vector<uint8_t> blob(wbytes + bbytes + fin.size() * 4);
+    memcpy(blob.data(), wp.data(), wbytes);
+    memcpy(blob.data() + wbytes, bias.data(), bbytes);
+    memcpy(blob.data() + wbytes + bbytes, fin.data(), fin.size() * 4);
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    uint8_t* d = static_cast<uint8_t*>(stream_buffer(blob.data(), blob.size(), st, "ytk_op_dbnet_head_f32"));
+    if (!d) return YTK_ERR;
+    ytk::ConvGeom g{n, H, W, 64, 64, 1, 1, 1, 0, 1, 256};
+    ytk::Epilogue e;
+    e.bias = reinterpret_cast<const float*>(d + wbytes);
+    e.out = prob_dev;
+    e.out_f32 = 1;
+    e.ldc = 4;
+    e.mode = ytk::EPI_CONVT_FINAL;
+    e.fin_w = reinterpret_cast<const float*>(d + wbytes + bbytes);
+    e.fin_b = b2;
+    ytk::GemmPlan plan;
+    int rc = ytk::conv_plan_create(&plan, x_dev, g, d, e);
+    if (!rc) rc = ytk::gemm_plan_launch(&plan, st);
+    cudaFreeAsync(d, st);
     return rc ? YTK_ERR : YTK_OK;
 }
 

@@ -78,6 +78,37 @@ static int pack_conv(const TensorView* w, int Cout, int Cin, int kh, int kw, con
     return upload(p.data(), p.size() * 2, dev);
 }
 
+void pack_stem_weights(const float* w, const float* scale, std::vector<uint16_t>* out) {
+    std::vector<uint16_t>& p = *out;
+    p.assign((size_t)64 * 7 * 64, 0);
+    for (int co = 0; co < 64; ++co)
+        for (int c = 0; c < 3; ++c)
+            for (int r = 0; r < 7; ++r)
+                for (int s = 0; s < 7; ++s)
+                    p[((size_t)co * 7 + r) * 64 + s * 8 + c] =
+                        f2op_host(w[(((size_t)co * 3 + c) * 7 + r) * 7 + s] * (scale ? scale[co] : 1.f));
+}
+
+void pack_convt_head(const float* w1, const float* b1, const float* scale, const float* shift, const float* w2,
+                     std::vector<uint16_t>* w_rows, std::vector<float>* bias, std::vector<float>* fin_w) {
+    std::vector<uint16_t>& p = *w_rows;
+    p.resize((size_t)256 * 64);
+    bias->resize(256);
+    for (int i = 0; i < 2; ++i)
+        for (int j = 0; j < 2; ++j)
+            for (int co = 0; co < 64; ++co) {
+                const int row = (i * 2 + j) * 64 + co;
+                const float sc = scale ? scale[co] : 1.f;
+                for (int ci = 0; ci < 64; ++ci)
+                    p[(size_t)row * 64 + ci] = f2op_host(w1[(((size_t)ci * 64 + co) * 2 + i) * 2 + j] * sc);
+                (*bias)[row] = b1[co] * sc + (shift ? shift[co] : 0.f);
+            }
+    // [ci][1][i'][j'] -> [k = i'*2+j'][ci] for the fused epilogue
+    fin_w->resize(4 * 64);
+    for (int ci = 0; ci < 64; ++ci)
+        for (int k = 0; k < 4; ++k) (*fin_w)[k * 64 + ci] = w2[ci * 4 + k];
+}
+
 int DbnetModel::load_conv(const WeightSet& ws, const std::string& wname, const std::string& bnname, int Cout, int Cin,
                           int k, int stride, int pad, int dil, const std::string& biasname, ConvW* out) {
     const TensorView* w = ws.need(wname, (long long)Cout * Cin * k * k);
@@ -122,13 +153,8 @@ int DbnetModel::load(const WeightSet& ws) {
         if (!w) return 1;
         std::vector<float> scale, shift;
         if (bn_fold(ws, bb + "bn1", 64, scale, shift)) return 1;
-        std::vector<uint16_t> p((size_t)64 * 7 * 64, 0);
-        for (int co = 0; co < 64; ++co)
-            for (int c = 0; c < 3; ++c)
-                for (int r = 0; r < 7; ++r)
-                    for (int s = 0; s < 7; ++s)
-                        p[((size_t)co * 7 + r) * 64 + s * 8 + c] =
-                            f2op_host(w->data[(((size_t)co * 3 + c) * 7 + r) * 7 + s] * scale[co]);
+        std::vector<uint16_t> p;
+        pack_stem_weights(w->data, scale.data(), &p);
         if (upload(p.data(), p.size() * 2, &stem.w)) return 1;
         void* d = nullptr;
         if (upload(shift.data(), 64 * 4, &d)) return 1;
@@ -190,21 +216,15 @@ int DbnetModel::load(const WeightSet& ws) {
     const std::string bz = d + "binarize.";
     if (load_conv(ws, bz + "0.weight", bz + "1", 64, 256, 3, 1, 1, 1, "", &bin_conv)) return 1;
     {
-        // ConvTranspose2d(64,64,2,2) weight [ci][co][i][j] + bias, BN folded: GEMM rows ordered (i, j, co)
+        // ConvTranspose2d(64,64,2,2) + BN (folded) + ReLU, then ConvTranspose2d(64,1,2,2): see pack_convt_head
         const TensorView *w = ws.need(bz + "3.weight", 64LL * 64 * 4), *b = ws.need(bz + "3.bias", 64);
-        if (!w || !b) return 1;
+        const TensorView *w2 = ws.need(bz + "6.weight", 64 * 4), *b2 = ws.need(bz + "6.bias", 1);
+        if (!w || !b || !w2 || !b2) return 1;
         std::vector<float> scale, shift;
         if (bn_fold(ws, bz + "4", 64, scale, shift)) return 1;
-        std::vector<uint16_t> p((size_t)256 * 64);
-        std::vector<float> bias(256);
-        for (int i = 0; i < 2; ++i)
-            for (int j = 0; j < 2; ++j)
-                for (int co = 0; co < 64; ++co) {
-                    const int row = (i * 2 + j) * 64 + co;
-                    for (int ci = 0; ci < 64; ++ci)
-                        p[(size_t)row * 64 + ci] = f2op_host(w->data[(((size_t)ci * 64 + co) * 2 + i) * 2 + j] * scale[co]);
-                    bias[row] = b->data[co] * scale[co] + shift[co];
-                }
+        std::vector<uint16_t> p;
+        std::vector<float> bias, fw;
+        pack_convt_head(w->data, b->data, scale.data(), shift.data(), w2->data, &p, &bias, &fw);
         if (upload(p.data(), p.size() * 2, &convt1.w)) return 1;
         void* q = nullptr;
         if (upload(bias.data(), 256 * 4, &q)) return 1;
@@ -213,12 +233,6 @@ int DbnetModel::load(const WeightSet& ws) {
         convt1.Cin = 64;
         owned.push_back(convt1.w);
         owned.push_back(convt1.bias);
-        const TensorView *w2 = ws.need(bz + "6.weight", 64 * 4), *b2 = ws.need(bz + "6.bias", 1);
-        if (!w2 || !b2) return 1;
-        // [ci][1][i'][j'] -> [k = i'*2+j'][ci] for the fused epilogue
-        std::vector<float> fw(4 * 64);
-        for (int ci = 0; ci < 64; ++ci)
-            for (int k = 0; k < 4; ++k) fw[k * 64 + ci] = w2->data[ci * 4 + k];
         void* fd = nullptr;
         if (upload(fw.data(), fw.size() * 4, &fd)) return 1;
         convt2_w_dev = reinterpret_cast<float*>(fd);

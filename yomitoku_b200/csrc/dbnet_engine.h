@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <cstdint>
 #include <functional>
 #include <map>
 #include <string>
@@ -80,5 +81,14 @@ struct DbnetEngine {
 };
 
 void dbnet_input_size(int H0, int W0, int shortest, int limit, int* Hn, int* Wn);
+
+// Weight packing shared by DbnetModel::load (BatchNorm folded in: per-channel scale / shift) and the op-level entries
+// (identity: scale and shift null).
+// Stem: conv1.weight [64][3][7][7] fp32 -> [64][7 rows][8 px * 8 ch] 16-bit (pixel 7 and channels 3..7 zero).
+void pack_stem_weights(const float* w, const float* scale, std::vector<uint16_t>* out);
+// Binarize head: ConvTranspose2d(64,64,2,2) weight [ci][co][i][j] and bias -> GEMM rows ordered (i, j, co), w_rows
+// [256][64] 16-bit and bias [256] fp32; ConvTranspose2d(64,1,2,2) weight [ci][1][i'][j'] -> fin_w [k = i'*2+j'][ci] fp32.
+void pack_convt_head(const float* w1, const float* b1, const float* scale, const float* shift, const float* w2,
+                     std::vector<uint16_t>* w_rows, std::vector<float>* bias, std::vector<float>* fin_w);
 
 }  // namespace ytk

@@ -383,55 +383,6 @@ int launch_asf(const void* a, void* fuse, int n_img, int H, int W, const float* 
     return cudaGetLastError() != cudaSuccess;
 }
 
-// ------------------------------------------------------------------------------------------------------------------
-// Final ConvTranspose2d(64 -> 1, kernel 2, stride 2) + Sigmoid (reference dbnet_plus.py:114-115): each input pixel
-// produces a 2x2 block of probabilities.  8 threads per input pixel.
-// ------------------------------------------------------------------------------------------------------------------
-struct ConvT2W { float w[4][64]; float b; };
-
-__global__ void convt2_sigmoid_kernel(const uint4* __restrict__ x, long long npix, int H, int W, const ConvT2W wts,
-                                      float* __restrict__ prob /* [N, 2H, 2W] */) {
-    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long pix = t >> 3;
-    const int cg = (int)(t & 7);
-    float part[4] = {0.f, 0.f, 0.f, 0.f};
-    if (pix < npix) {
-        float f[8];
-        unpack8(__ldg(x + pix * 8 + cg), f);
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-#pragma unroll
-            for (int j = 0; j < 8; ++j) part[k] += wts.w[k][cg * 8 + j] * f[j];
-    }
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        part[k] += __shfl_xor_sync(0xffffffffu, part[k], 1);
-        part[k] += __shfl_xor_sync(0xffffffffu, part[k], 2);
-        part[k] += __shfl_xor_sync(0xffffffffu, part[k], 4);
-    }
-    if (pix >= npix || cg >= 4) return;
-    const int w = (int)(pix % W);
-    const int h = (int)((pix / W) % H);
-    const long long img = pix / ((long long)W * H);
-    const int i = cg >> 1, j = cg & 1;
-    const float v = 1.f / (1.f + __expf(-(part[cg] + wts.b)));
-    prob[(img * (2 * H) + (2 * h + i)) * (2LL * W) + 2 * w + j] = v;
-}
-
-int launch_convt2_sigmoid(const void* x, int n_img, int H, int W, const float* host_w /* [64][1][2][2] */, float bias,
-                          float* prob, cudaStream_t st) {
-    ConvT2W wts;
-    for (int c = 0; c < 64; ++c)
-        for (int k = 0; k < 4; ++k) wts.w[k][c] = host_w[c * 4 + k];
-    wts.b = bias;
-    const long long npix = (long long)n_img * H * W;
-    const long long thr = npix * 8;
-    convt2_sigmoid_kernel<<<(unsigned)((thr + 255) / 256), 256, 0, st>>>(reinterpret_cast<const uint4*>(x), npix, H, W,
-                                                                         wts, prob);
-    count_launch();
-    return cudaGetLastError() != cudaSuccess;
-}
-
 // fp32 -> bf16 conversion helper for weight upload / debug
 __global__ void op_to_f32_kernel(const op_t* __restrict__ in, float* __restrict__ out, long long n) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
