@@ -223,6 +223,61 @@ void ytk_parseq_last_phase_ms(ytk_parseq* h, float* ms4);
 int ytk_op_single_query_attn_f16(int mode, const void* q, const void* kv, int B, int S, int D, int heads,
                                  const int* step_dev, const ytk_crop* crops, void* out, void* cuda_stream);
 
+/* op level, for the parity tests: the recognizer's decoding tail, each entry called as the engine calls it.  Device
+ * pointers; asynchronous on the stream; invalid arguments are an error, not a launch.  An output row r of the softmax
+ * statistics goes to index g = r * g_stride + g_off of ids / probs (crop g / S, position g % S); when rep_cut is given
+ * and rep_cut[g / S] == g % S, the position gets eos_id with probability 1 (the repetition patch).
+ *   linear_rowmax    the head GEMM with the row-max epilogue: per row of A [M, lda] fp16 times W [N, K] fp16 plus bias
+ *                    [N] fp32 (or NULL), npart = 2 * tiles_n float4 partials {max, sum exp(x - max), bit-cast arg-max,
+ *                    0} at partials[row * npart ...]; argmax_only != 0 leaves the sums 0 (the AR loop's mode when
+ *                    refinement follows).  npart_out / block_n_out (host, optional) receive the layout the plan chose:
+ *                    it depends on the SM count.  partials_capacity (float4s) must hold M * npart.
+ *   softmax_max      ids / probs from fp32 logits [rows, ldl] (C valid columns, ldl % 4 == 0, 16-byte aligned).
+ *   rowmax_finalize  the same from the partials [rows, ldp] of linear_rowmax (npart <= ldp valid per row).
+ *   ar_control       one AR step of the engine's loop: arg-max of the step's logits (npart == 0: fp32 logits [B, ldl];
+ *                    npart > 0: the partials, ldl float4s per row), the repetition stop, EOS bookkeeping, the ends of
+ *                    groups g0 .. g0 + ngroups - 1 (row_group holds global group ids), and cin [B, D] fp16 =
+ *                    LN_c(pos_q[j - 1] + sqrt(D) * embed[token]) for the token entering position j = step + 1.  embed is
+ *                    the engine's table: rows of D fp32, zero padded from d_real and pre-multiplied by sqrt(d_real / D),
+ *                    so sqrt(D) * embed = sqrt(d_real) * E; pos_q [S - 1, D], g_c / b_c [D] likewise zero padded.
+ *                    The state (tgt, raw [B][S]; rep_cut, rep_done, has_eos [B]; group_len, open_rows [g0 + ngroups];
+ *                    n_active, step, ticket [1]) is read and updated on the device; open_rows and ticket are zero
+ *                    between steps.
+ *   refine_embed     the refinement context [BOS, raw[0 .. L-2]] of each row, L = group_len[row_group[row]]: cin
+ *                    [B][S][D] fp16 (positions >= L get EOS), klen [B] = L, kpad [B] = first EOS position in the
+ *                    context (L if none).  Same embedding tables as ar_control; B <= 65535.
+ *   apply_rep_cut    the repetition patch alone (refine_iters == 0): ids / probs [B, S], rep_cut [B] (-1 = none). */
+typedef struct {
+    int32_t* tgt;
+    int32_t* raw;
+    int32_t* rep_cut;
+    int32_t* rep_done;
+    int32_t* has_eos;
+    int32_t* group_len;
+    int32_t* n_active;
+    int32_t* step;
+    int32_t* open_rows;
+    int32_t* ticket;
+} ytk_ar_state;   /* ten device pointers, the layout of ytk::ArState (csrc/parseq_ops.h) */
+
+int ytk_op_linear_rowmax_f16(const void* A, long long lda, int M, int K, const void* W, int N, const float* bias,
+                             int argmax_only, void* partials, long long partials_capacity, int* npart_out,
+                             int* block_n_out, void* cuda_stream);
+int ytk_op_softmax_max_f32(const float* logits, long long ldl, int C, int rows, int S, long long g_stride,
+                           long long g_off, const int* rep_cut, int eos_id, int* ids, float* probs, void* cuda_stream);
+int ytk_op_rowmax_finalize_f32(const void* partials, long long ldp, int npart, int C, int rows, int S,
+                               long long g_stride, long long g_off, const int* rep_cut, int eos_id, int* ids,
+                               float* probs, void* cuda_stream);
+int ytk_op_ar_control(const float* logits, long long ldl, int C, int npart, int B, int S, const int* row_group, int g0,
+                      int ngroups, const ytk_ar_state* state, int eos_id, int rep_on, int rep_period_max,
+                      int rep_min_run_p1, int rep_min_repeats, const float* embed, const float* pos_q, int D,
+                      int d_real, const float* g_c, const float* b_c, void* cin, void* cuda_stream);
+int ytk_op_refine_embed(const int* raw, const int* row_group, const int* group_len, int B, int S, int bos_id,
+                        int eos_id, const float* embed, const float* pos_q, int D, int d_real, const float* g_c,
+                        const float* b_c, void* cin, int* klen, int* kpad, void* cuda_stream);
+int ytk_op_apply_rep_cut(const int* rep_cut, int B, int S, int C, int eos_id, int* ids, float* probs,
+                         void* cuda_stream);
+
 /* op level, for the parity tests: the DBNet detector's own kernels, each called as the engine calls it.  Activations
  * are NHWC fp16 on the device, 16-byte aligned; weights are the reference's fp32 layouts on the host, packed by the
  * code the engine's loader uses (with no BatchNorm: the bias is the whole shift).  Asynchronous on the stream (weights

@@ -28,3 +28,4 @@ def test_struct_layouts_match_header():
     assert ctypes.sizeof(_lib.YtkTensor) == 8 + 8 + 8 + 32
     assert ctypes.sizeof(_lib.YtkAttnSeq) == 32          # 4 ints + long long + 2 ints
     assert ctypes.sizeof(_lib.YtkDbRun) == 24            # 4 ints + double
+    assert ctypes.sizeof(_lib.YtkArState) == 10 * 8      # ten device pointers

@@ -183,3 +183,52 @@ def test_engine_reuse_smaller_batch_after_larger():
     ids, probs, glen = rec.model.recognize_crops(small, [320] * 5, [0] * 5, 1)
     assert np.array_equal(ids, ids_ref) and np.array_equal(glen, glen_ref)
     assert np.allclose(probs, probs_ref, atol=1e-6)
+
+
+def _engine_crops(n=200, n_groups=4, seed=21):
+    """~200 crops in sorted groups of different padded widths (the layout the two-part AR loop splits)"""
+    rng = np.random.default_rng(seed)
+    per = n // n_groups
+    groups = [min(i // per, n_groups - 1) for i in range(n)]
+    widths = [8 * int(w) for w in rng.integers(6, 40, size=n)]
+    canv = [rng.integers(0, 256, size=(32, w, 3), dtype=np.uint8) for w in widths]
+    padded = [max(widths[j] for j in range(n) if groups[j] == g) for g in groups]
+    return canv, padded, groups, n_groups
+
+
+def test_two_part_ar_loop_matches_one_part(monkeypatch):
+    """YTK_AR_SPLIT_MIN=1 runs the AR loop as two row ranges on two streams (second part: g0 > 0, offset state
+    pointers, global group ids).  Ids and group lengths must be those of the one-part loop, probabilities within
+    1e-6 (test_large_model_ragged_vs_seam_consistency's standard)."""
+    name = "parseq-tiny-dynw-v4"
+    sd = weights.make_parseq_state_dict(ops.SPECS[name], seed=11, peaked=True)
+    rec = _rec(name, sd)
+    canv, padded, groups, ng = _engine_crops()
+    monkeypatch.delenv("YTK_AR_SPLIT_MIN", raising=False)
+    ids_a, probs_a, glen_a = rec.model.recognize_crops(canv, padded, groups, ng)
+    monkeypatch.setenv("YTK_AR_SPLIT_MIN", "1")
+    ids_b, probs_b, glen_b = rec.model.recognize_crops(canv, padded, groups, ng)
+    assert np.array_equal(glen_a, glen_b)
+    assert np.array_equal(ids_a, ids_b)
+    assert np.allclose(probs_a, probs_b, atol=1e-6)
+
+
+def test_unfused_head_matches_fused(monkeypatch):
+    """YTK_NO_FUSED_HEAD=1 materialises the head logits and runs softmax_max / the logits path of ar_control instead
+    of the row-max epilogue.  Both read the same fp32 logits (same plan, same accumulators), so the ids are equal and
+    the probabilities agree within the fp32 chain bound of tests/test_gpu_parseq_decode_kernels.py, taken at its
+    worst over a row: twice 48 2^-21 + 65 2^-24 + (C - 1) 2^-22 / e."""
+    name = "parseq-tiny-dynw-v4"
+    spec = ops.SPECS[name]
+    sd = weights.make_parseq_state_dict(spec, seed=12, peaked=True)
+    rec = _rec(name, sd)
+    canv, padded, groups, ng = _engine_crops(seed=22)
+    monkeypatch.delenv("YTK_NO_FUSED_HEAD", raising=False)
+    ids_a, probs_a, glen_a = rec.model.recognize_crops(canv, padded, groups, ng)
+    monkeypatch.setenv("YTK_NO_FUSED_HEAD", "1")
+    ids_b, probs_b, glen_b = rec.model.recognize_crops(canv, padded, groups, ng)
+    assert np.array_equal(glen_a, glen_b) and np.array_equal(ids_a, ids_b)
+    rel = 2 * (48 * 2.0 ** -21 + 65 * 2.0 ** -24 + (spec.num_classes - 1) * 2.0 ** -22 / np.e)
+    d = np.abs(probs_a.astype(np.float64) - probs_b) / (rel * probs_b)
+    print("[engine] fused vs unfused head: worst |dp| / (rel p) %.3g (rel %.3g)" % (d.max(), rel))
+    assert d.max() <= 1.0, d.max()

@@ -218,3 +218,126 @@ def test_dbnet_head_refusals(lib, kwargs, fragment):
     before = lib.ytk_launch_count()
     _refused(lib, _head(lib, **kwargs), fragment)
     assert lib.ytk_launch_count() == before
+
+
+# ======================================================================================================== PARSeq decoding tail
+def _rowmax(lib, A=P, lda=384, M=129, K=384, W=P, N=7119, bias=P, part=P, cap=129 * 2 * 28):
+    npart, bn = ctypes.c_int(-1), ctypes.c_int(-1)
+    st = lib.ytk_op_linear_rowmax_f16(A, lda, M, K, W, N, bias, 0, part, cap, ctypes.byref(npart), ctypes.byref(bn),
+                                      None)
+    assert npart.value == -1 and bn.value == -1                       # nothing reported on a refusal
+    return st
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(A=None), b"null argument"), (dict(W=None), b"null argument"), (dict(part=None), b"null argument"),
+    (dict(M=0), b"M 0, K 384, N 7119"), (dict(N=0), b"N 0"), (dict(K=0, lda=0), b"K 0"),
+    (dict(K=100, lda=104), b"K 100"), (dict(lda=320), b"lda 320 unsupported"), (dict(lda=388), b"lda 388"),
+    (dict(A=P + 8), b"16-byte aligned"), (dict(W=P + 2), b"16-byte aligned"), (dict(bias=P + 4), b"16-byte aligned"),
+    (dict(part=P + 8), b"16-byte aligned"),
+    # fewer float4s than M x 2 x ceil(N / 256), the fewest partials any N tile gives
+    (dict(cap=129 * 2 * 28 - 1), b"partials_capacity 7223 float4s < 7224"), (dict(cap=0), b"partials_capacity 0"),
+    (dict(M=1, N=64, cap=1), b"partials_capacity 1 float4s < 2"),
+])
+def test_linear_rowmax_refusals(lib, kwargs, fragment):
+    before = lib.ytk_launch_count()
+    _refused(lib, _rowmax(lib, **kwargs), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+def _smax(lib, logits=P, ldl=7168, C=7119, rows=101, S=101, g_stride=1, g_off=0, rep_cut=None, eos=0, ids=P,
+          probs=P):
+    return lib.ytk_op_softmax_max_f32(logits, ldl, C, rows, S, g_stride, g_off, rep_cut, eos, ids, probs, None)
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(logits=None), b"null argument"), (dict(ids=None), b"null argument"), (dict(probs=None), b"null argument"),
+    (dict(ldl=7118), b"ldl 7118 for C 7119"), (dict(ldl=7122), b"ldl 7122 for C 7119"),
+    (dict(logits=P + 4), b"not 16-byte aligned"), (dict(C=0), b"C 0"), (dict(rows=0), b"0 rows"),
+    (dict(S=0), b"S 0"), (dict(g_stride=-1), b"g_stride -1"), (dict(g_off=-5), b"g_off -5"),
+    (dict(eos=-1), b"eos_id -1"),
+])
+def test_softmax_max_refusals(lib, kwargs, fragment):
+    before = lib.ytk_launch_count()
+    _refused(lib, _smax(lib, **kwargs), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+def _fin(lib, part=P, ldp=56, npart=56, C=7119, rows=101, S=101, g_stride=1, g_off=0, eos=0, ids=P, probs=P):
+    return lib.ytk_op_rowmax_finalize_f32(part, ldp, npart, C, rows, S, g_stride, g_off, None, eos, ids, probs, None)
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(part=None), b"null argument"), (dict(ids=None), b"null argument"), (dict(probs=None), b"null argument"),
+    (dict(npart=57), b"npart 57, ldp 56"), (dict(npart=0), b"npart 0"), (dict(part=P + 8), b"not 16-byte aligned"),
+    (dict(rows=0), b"0 rows"), (dict(C=-1), b"C -1"), (dict(S=0), b"S 0"), (dict(g_off=-1), b"g_off -1"),
+])
+def test_rowmax_finalize_refusals(lib, kwargs, fragment):
+    before = lib.ytk_launch_count()
+    _refused(lib, _fin(lib, **kwargs), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+def _state(**none):
+    names = [n for n, _ in _lib.YtkArState._fields_]
+    return _lib.YtkArState(*[None if n in none else P + 64 * i for i, n in enumerate(names)])
+
+
+def _arc(lib, logits=P, ldl=7168, C=7119, npart=0, B=8, S=101, row_group=P, g0=0, ngroups=2, state=None, eos=0,
+         rep_on=1, pmax=8, run_p1=8, reps=3, embed=P, pos_q=P, D=384, d_real=368, g_c=P, b_c=P, cin=P):
+    state = _state() if state is None else state
+    return lib.ytk_op_ar_control(logits, ldl, C, npart, B, S, row_group, g0, ngroups, ctypes.byref(state), eos, rep_on,
+                                 pmax, run_p1, reps, embed, pos_q, D, d_real, g_c, b_c, cin, None)
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(D=1028, d_real=1028), b"D 1028 / d_real 1028 unsupported"), (dict(d_real=385), b"D 384 / d_real 385"),
+    (dict(d_real=0), b"d_real 0"), (dict(D=0, d_real=0), b"D 0"),
+    (dict(npart=-1), b"npart -1"), (dict(B=0), b"B 0"), (dict(S=0), b"S 0"), (dict(C=0, eos=0), b"C 0"),
+    (dict(ldl=7116), b"ldl 7116 too small for C 7119"), (dict(ldl=7121), b"ldl 7121"),
+    (dict(npart=56, ldl=55), b"ldl 55 too small for C 7119 / npart 56"), (dict(logits=P + 4), b"not 16-byte aligned"),
+    (dict(eos=7119), b"eos_id 7119 outside [0, 7119)"), (dict(eos=-1), b"eos_id -1 outside"),
+    (dict(ngroups=0), b"0 groups from g0 0"), (dict(g0=-1), b"2 groups from g0 -1"),
+    (dict(pmax=0), b"period_max 0"), (dict(run_p1=0), b"min_run_p1 0"), (dict(reps=0), b"min_repeats 0"),
+    (dict(logits=None), b"null argument"), (dict(row_group=None), b"null argument"), (dict(embed=None), b"null argument"),
+    (dict(pos_q=None), b"null argument"), (dict(g_c=None), b"null argument"), (dict(b_c=None), b"null argument"),
+    (dict(cin=None), b"null argument"),
+] + [(dict(state=_state(**{n: 1})), b"null argument") for n, _ in _lib.YtkArState._fields_])
+def test_ar_control_refusals(lib, kwargs, fragment):
+    before = lib.ytk_launch_count()
+    _refused(lib, _arc(lib, **kwargs), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+def _ref(lib, raw=P, row_group=P, glen=P, B=8, S=101, bos=7119, eos=0, embed=P, pos_q=P, D=384, d_real=368, g_c=P,
+         b_c=P, cin=P, klen=P, kpad=P):
+    return lib.ytk_op_refine_embed(raw, row_group, glen, B, S, bos, eos, embed, pos_q, D, d_real, g_c, b_c, cin, klen,
+                                   kpad, None)
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(raw=None), b"null argument"), (dict(row_group=None), b"null argument"), (dict(glen=None), b"null argument"),
+    (dict(klen=None), b"null argument"), (dict(kpad=None), b"null argument"), (dict(embed=None), b"null argument"),
+    (dict(pos_q=None), b"null argument"), (dict(g_c=None), b"null argument"), (dict(b_c=None), b"null argument"),
+    (dict(cin=None), b"null argument"),
+    (dict(D=1040, d_real=1040), b"D 1040 / d_real 1040"), (dict(d_real=400), b"D 384 / d_real 400"),
+    (dict(B=0), b"B 0"), (dict(B=65536), b"B 65536"), (dict(S=0), b"S 0"), (dict(bos=-1), b"bos_id -1"),
+    (dict(eos=-2), b"eos_id -2"),
+])
+def test_refine_embed_refusals(lib, kwargs, fragment):
+    before = lib.ytk_launch_count()
+    _refused(lib, _ref(lib, **kwargs), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(rep_cut=None), b"null argument"), (dict(ids=None), b"null argument"), (dict(probs=None), b"null argument"),
+    (dict(B=0), b"B 0"), (dict(S=0), b"S 0"), (dict(C=0), b"C 0"), (dict(eos=-1), b"eos_id -1"),
+])
+def test_apply_rep_cut_refusals(lib, kwargs, fragment):
+    a = dict(rep_cut=P, B=8, S=101, C=7119, eos=0, ids=P, probs=P)
+    a.update(kwargs)
+    before = lib.ytk_launch_count()
+    _refused(lib, lib.ytk_op_apply_rep_cut(a["rep_cut"], a["B"], a["S"], a["C"], a["eos"], a["ids"], a["probs"], None),
+             fragment)
+    assert lib.ytk_launch_count() == before

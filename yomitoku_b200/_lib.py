@@ -19,6 +19,12 @@ class YtkError(RuntimeError):
     pass
 
 
+class YtkArState(ctypes.Structure):
+    """ytk_ar_state: the AR loop's device state, ten int32 device pointers."""
+    _fields_ = [(n, c_void_p) for n in ("tgt", "raw", "rep_cut", "rep_done", "has_eos", "group_len", "n_active", "step",
+                                        "open_rows", "ticket")]
+
+
 def _declare(lib):
     lib.ytk_last_error.restype = ctypes.c_char_p
     lib.ytk_last_error.argtypes = []
@@ -49,6 +55,24 @@ def _declare(lib):
     lib.ytk_op_single_query_attn_f16.restype = c_int
     lib.ytk_op_single_query_attn_f16.argtypes = [c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p,
                                                  c_void_p, c_void_p, c_void_p]
+    lib.ytk_op_linear_rowmax_f16.restype = c_int
+    lib.ytk_op_linear_rowmax_f16.argtypes = [c_void_p, c_ll, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p,
+                                             c_ll, ctypes.POINTER(c_int), ctypes.POINTER(c_int), c_void_p]
+    lib.ytk_op_softmax_max_f32.restype = c_int
+    lib.ytk_op_softmax_max_f32.argtypes = [c_void_p, c_ll, c_int, c_int, c_int, c_ll, c_ll, c_void_p, c_int, c_void_p,
+                                           c_void_p, c_void_p]
+    lib.ytk_op_rowmax_finalize_f32.restype = c_int
+    lib.ytk_op_rowmax_finalize_f32.argtypes = [c_void_p, c_ll, c_int, c_int, c_int, c_int, c_ll, c_ll, c_void_p, c_int,
+                                               c_void_p, c_void_p, c_void_p]
+    lib.ytk_op_ar_control.restype = c_int
+    lib.ytk_op_ar_control.argtypes = [c_void_p, c_ll, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int,
+                                      ctypes.POINTER(YtkArState), c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                      c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
+    lib.ytk_op_refine_embed.restype = c_int
+    lib.ytk_op_refine_embed.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                                        c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
+    lib.ytk_op_apply_rep_cut.restype = c_int
+    lib.ytk_op_apply_rep_cut.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]
     lib.ytk_op_dbnet_preprocess_u8.restype = c_int
     lib.ytk_op_dbnet_preprocess_u8.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
     lib.ytk_op_dbnet_stem_f16.restype = c_int

@@ -4,6 +4,7 @@
 #include <algorithm>
 #include <climits>
 #include <cmath>
+#include <cstddef>
 #include <cstdlib>
 #include <cstring>
 #include <map>
@@ -306,6 +307,204 @@ int ytk_op_single_query_attn_f16(int mode, const void* q, const void* kv, int B,
     if (!rc) rc = ytk::launch_dec_cross_attn(q, kv, reinterpret_cast<const ytk::CropDesc*>(descs_dev), B, D, heads, out, st);
     cudaFreeAsync(descs_dev, st);
     return rc ? YTK_ERR : YTK_OK;
+}
+
+// ---- the recognizer's decoding tail (parseq_ops.cu, gemm_tc.cu EPI_ROWMAX), each entry called as the engine calls it
+int ytk_op_linear_rowmax_f16(const void* A, long long lda, int M, int K, const void* W, int N, const float* bias,
+                             int argmax_only, void* partials, long long partials_capacity, int* npart_out,
+                             int* block_n_out, void* cuda_stream) {
+    if (!A || !W || !partials) {
+        ytk::set_error("ytk_op_linear_rowmax_f16: null argument");
+        return YTK_ERR;
+    }
+    if (M < 1 || N < 1 || K < 64 || K % 64 != 0 || lda < K || lda % 8 != 0) {
+        ytk::set_error("ytk_op_linear_rowmax_f16: M %d, K %d, N %d, lda %lld unsupported (K a multiple of 64, lda >= K "
+                       "and a multiple of 8)", M, K, N, lda);
+        return YTK_ERR;
+    }
+    if (misaligned(A, 16) || misaligned(W, 16) || misaligned(bias, 16) || misaligned(partials, 16)) {
+        ytk::set_error("ytk_op_linear_rowmax_f16: A, W, bias and partials must be 16-byte aligned");
+        return YTK_ERR;
+    }
+    // the widest N tile (256) gives the fewest partials: a capacity below that is too small whatever the plan picks
+    const long long least = (long long)M * 2 * ((N + 255) / 256);
+    if (partials_capacity < least) {
+        ytk::set_error("ytk_op_linear_rowmax_f16: partials_capacity %lld float4s < %lld (M %d x at least %lld partials)",
+                       partials_capacity, least, M, least / M);
+        return YTK_ERR;
+    }
+    ytk::Epilogue e;
+    e.bias = bias;
+    e.out = partials;
+    e.out_f32 = 1;
+    e.mode = ytk::EPI_ROWMAX;
+    e.act = argmax_only ? ytk::ACT_RELU : ytk::ACT_NONE;   // ACT_RELU: the sum-free mode of the AR loop
+    ytk::GemmPlan plan;
+    if (ytk::gemm_plan_create(&plan, A, lda, M, K, W, N, e)) return YTK_ERR;
+    const long long npart = plan.args.ldc;                // 2 * tiles_n float4s per row
+    if (partials_capacity < (long long)M * npart) {
+        ytk::set_error("ytk_op_linear_rowmax_f16: partials_capacity %lld float4s < %lld (M %d x %lld partials at "
+                       "block_n %d)", partials_capacity, (long long)M * npart, M, npart, plan.block_n);
+        return YTK_ERR;
+    }
+    if (npart_out) *npart_out = (int)npart;
+    if (block_n_out) *block_n_out = plan.block_n;
+    return ytk::gemm_plan_launch(&plan, static_cast<cudaStream_t>(cuda_stream)) ? YTK_ERR : YTK_OK;
+}
+
+// rows / positions / output indices shared by the two softmax-statistics entries
+static bool bad_stat_rows(const char* who, int C, int rows, int S, long long g_stride, long long g_off, int eos_id) {
+    if (C < 1 || rows < 1 || S < 1 || g_stride < 0 || g_off < 0 || eos_id < 0) {
+        ytk::set_error("%s: C %d, %d rows, S %d, g_stride %lld, g_off %lld, eos_id %d unsupported", who, C, rows, S,
+                       g_stride, g_off, eos_id);
+        return true;
+    }
+    return false;
+}
+
+int ytk_op_softmax_max_f32(const float* logits, long long ldl, int C, int rows, int S, long long g_stride,
+                           long long g_off, const int* rep_cut, int eos_id, int* ids, float* probs, void* cuda_stream) {
+    if (!logits || !ids || !probs) {
+        ytk::set_error("ytk_op_softmax_max_f32: null argument");
+        return YTK_ERR;
+    }
+    if (bad_stat_rows("ytk_op_softmax_max_f32", C, rows, S, g_stride, g_off, eos_id)) return YTK_ERR;
+    // the kernel reads rows as float4: 16-byte aligned rows of at least C floats
+    if (ldl < C || ldl % 4 != 0 || misaligned(logits, 16)) {
+        ytk::set_error("ytk_op_softmax_max_f32: ldl %lld for C %d (ldl >= C, a multiple of 4) or logits not 16-byte "
+                       "aligned", ldl, C);
+        return YTK_ERR;
+    }
+    return ytk::launch_softmax_max(logits, ldl, C, rows, S, g_stride, g_off, rep_cut, eos_id, ids, probs,
+                                   static_cast<cudaStream_t>(cuda_stream))
+               ? YTK_ERR
+               : YTK_OK;
+}
+
+int ytk_op_rowmax_finalize_f32(const void* partials, long long ldp, int npart, int C, int rows, int S,
+                               long long g_stride, long long g_off, const int* rep_cut, int eos_id, int* ids,
+                               float* probs, void* cuda_stream) {
+    if (!partials || !ids || !probs) {
+        ytk::set_error("ytk_op_rowmax_finalize_f32: null argument");
+        return YTK_ERR;
+    }
+    if (bad_stat_rows("ytk_op_rowmax_finalize_f32", C, rows, S, g_stride, g_off, eos_id)) return YTK_ERR;
+    if (npart < 1 || npart > ldp || misaligned(partials, 16)) {
+        ytk::set_error("ytk_op_rowmax_finalize_f32: npart %d, ldp %lld (1 <= npart <= ldp) or partials not 16-byte "
+                       "aligned", npart, ldp);
+        return YTK_ERR;
+    }
+    return ytk::launch_rowmax_finalize(static_cast<const float*>(partials), ldp, npart, C, rows, S, g_stride, g_off,
+                                       rep_cut, eos_id, ids, probs, static_cast<cudaStream_t>(cuda_stream))
+               ? YTK_ERR
+               : YTK_OK;
+}
+
+static_assert(sizeof(ytk_ar_state) == sizeof(ytk::ArState), "ytk_ar_state and ytk::ArState must have one layout");
+static_assert(offsetof(ytk_ar_state, ticket) == offsetof(ytk::ArState, ticket) &&
+                  offsetof(ytk_ar_state, group_len) == offsetof(ytk::ArState, group_len),
+              "ytk_ar_state and ytk::ArState must have one layout");
+
+// content embedding + LN_c arguments shared by ar_control and refine_embed
+static bool bad_embed(const char* who, const float* embed, const float* pos_q, int D, int d_real, const float* g_c,
+                      const float* b_c, const void* cin) {
+    if (!embed || !pos_q || !g_c || !b_c || !cin) {
+        ytk::set_error("%s: null argument", who);
+        return true;
+    }
+    if (D < 1 || D > 1024 || d_real < 1 || d_real > D) {   // 256 threads x 4 features per row
+        ytk::set_error("%s: D %d / d_real %d unsupported (1 <= d_real <= D <= 1024)", who, D, d_real);
+        return true;
+    }
+    return false;
+}
+
+int ytk_op_ar_control(const float* logits, long long ldl, int C, int npart, int B, int S, const int* row_group, int g0,
+                      int ngroups, const ytk_ar_state* state, int eos_id, int rep_on, int rep_period_max,
+                      int rep_min_run_p1, int rep_min_repeats, const float* embed, const float* pos_q, int D,
+                      int d_real, const float* g_c, const float* b_c, void* cin, void* cuda_stream) {
+    const char* who = "ytk_op_ar_control";
+    if (!logits || !row_group || !state || !state->tgt || !state->raw || !state->rep_cut || !state->rep_done ||
+        !state->has_eos || !state->group_len || !state->n_active || !state->step || !state->open_rows ||
+        !state->ticket) {
+        ytk::set_error("%s: null argument", who);
+        return YTK_ERR;
+    }
+    if (bad_embed(who, embed, pos_q, D, d_real, g_c, b_c, cin)) return YTK_ERR;
+    if (B < 1 || S < 1 || C < 1 || npart < 0) {
+        ytk::set_error("%s: B %d, S %d, C %d, npart %d unsupported", who, B, S, C, npart);
+        return YTK_ERR;
+    }
+    // npart > 0: rows of ldl float4 partials; npart == 0: rows of ldl fp32 logits read as float4
+    if ((npart > 0 ? ldl < npart : (ldl < C || ldl % 4 != 0)) || misaligned(logits, 16)) {
+        ytk::set_error("%s: ldl %lld too small for C %d / npart %d (or not a multiple of 4), or logits not 16-byte "
+                       "aligned", who, ldl, C, npart);
+        return YTK_ERR;
+    }
+    if (eos_id < 0 || eos_id >= C) {
+        ytk::set_error("%s: eos_id %d outside [0, %d)", who, eos_id, C);
+        return YTK_ERR;
+    }
+    if (ngroups < 1 || g0 < 0) {
+        ytk::set_error("%s: %d groups from g0 %d unsupported", who, ngroups, g0);
+        return YTK_ERR;
+    }
+    if (rep_on && (rep_period_max < 1 || rep_min_run_p1 < 1 || rep_min_repeats < 1)) {
+        ytk::set_error("%s: repetition stop with period_max %d, min_run_p1 %d, min_repeats %d unsupported", who,
+                       rep_period_max, rep_min_run_p1, rep_min_repeats);
+        return YTK_ERR;
+    }
+    ytk::ArState a;
+    a.tgt = state->tgt;
+    a.raw = state->raw;
+    a.rep_cut = state->rep_cut;
+    a.rep_done = state->rep_done;
+    a.has_eos = state->has_eos;
+    a.group_len = state->group_len;
+    a.n_active = state->n_active;
+    a.step = state->step;
+    a.open_rows = state->open_rows;
+    a.ticket = state->ticket;
+    return ytk::launch_ar_control(logits, ldl, C, npart, B, S, row_group, g0, ngroups, a, eos_id, rep_on, rep_period_max,
+                                  rep_min_run_p1, rep_min_repeats, embed, pos_q, D, d_real, g_c, b_c, cin,
+                                  static_cast<cudaStream_t>(cuda_stream))
+               ? YTK_ERR
+               : YTK_OK;
+}
+
+int ytk_op_refine_embed(const int* raw, const int* row_group, const int* group_len, int B, int S, int bos_id,
+                        int eos_id, const float* embed, const float* pos_q, int D, int d_real, const float* g_c,
+                        const float* b_c, void* cin, int* klen, int* kpad, void* cuda_stream) {
+    const char* who = "ytk_op_refine_embed";
+    if (!raw || !row_group || !group_len || !klen || !kpad) {
+        ytk::set_error("%s: null argument", who);
+        return YTK_ERR;
+    }
+    if (bad_embed(who, embed, pos_q, D, d_real, g_c, b_c, cin)) return YTK_ERR;
+    if (B < 1 || B > 65535 || S < 1 || bos_id < 0 || eos_id < 0) {   // grid (S, B)
+        ytk::set_error("%s: B %d, S %d, bos_id %d, eos_id %d unsupported (1 <= B <= 65535)", who, B, S, bos_id,
+                       eos_id);
+        return YTK_ERR;
+    }
+    return ytk::launch_refine_embed(raw, row_group, group_len, B, S, bos_id, eos_id, embed, pos_q, D, d_real, g_c, b_c,
+                                    cin, klen, kpad, static_cast<cudaStream_t>(cuda_stream))
+               ? YTK_ERR
+               : YTK_OK;
+}
+
+int ytk_op_apply_rep_cut(const int* rep_cut, int B, int S, int C, int eos_id, int* ids, float* probs,
+                         void* cuda_stream) {
+    if (!rep_cut || !ids || !probs) {
+        ytk::set_error("ytk_op_apply_rep_cut: null argument");
+        return YTK_ERR;
+    }
+    if (B < 1 || S < 1 || C < 1 || eos_id < 0) {
+        ytk::set_error("ytk_op_apply_rep_cut: B %d, S %d, C %d, eos_id %d unsupported", B, S, C, eos_id);
+        return YTK_ERR;
+    }
+    return ytk::launch_apply_rep_cut(rep_cut, B, S, C, eos_id, ids, probs, static_cast<cudaStream_t>(cuda_stream))
+               ? YTK_ERR
+               : YTK_OK;
 }
 
 // Allocates `bytes` on the stream and, if `host` is given, uploads it.  The copy is from pageable memory: the call

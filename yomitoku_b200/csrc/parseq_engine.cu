@@ -526,7 +526,7 @@ int ParseqEngine::forward(const ParseqBatch& b, int* ids_out, float* probs_out, 
         // The decode loop can run as two PARTS (row ranges that end on a group boundary), each on its own stream, so
         // that one part's GEMMs overlap the other part's HBM-bound attention.  The step's kernels are latency-bound: halving
         // M does not halve their time, and the persistent GEMM CTAs (over 200 KB of shared memory each) do not co-reside -
-        // so it is OFF unless YTK_AR_SPLIT_MIN=<rows> asks for it (the GPU tests run both ways).  Parts share nothing but read-only weights / memory K/V.
+        // so it is OFF unless YTK_AR_SPLIT_MIN=<rows> asks for it (tests/test_gpu_parseq.py runs both ways and compares them).  Parts share nothing but read-only weights / memory K/V.
         struct Part {
             int r0, rows, g0, ng;
             ArState a;
