@@ -147,7 +147,8 @@ int ytk_dbnet_device(const ytk_dbnet* h);
 /* network input size for an H0 x W0 page = reference resize_shortest_edge (data/functions.py:212-224) */
 int ytk_dbnet_input_size(const ytk_dbnet* h, int H0, int W0, int* Hn, int* Wn);
 /* pages: [n_pages, H0, W0, 3] uint8 BGR (caller-owned; device pointer iff pages_on_device, else host - pinned for
- * async copies).  prob_out: [n_pages, Hn, Wn] fp32 sigmoid map = preds["binary"][:, 0] of the reference. */
+ * async copies), any size: the resize to (Hn, Wn) is cv2.resize(INTER_AREA) whether the page shrinks or grows.
+ * prob_out: [n_pages, Hn, Wn] fp32 sigmoid map = preds["binary"][:, 0] of the reference. */
 int ytk_dbnet_forward_u8(ytk_dbnet* h, const uint8_t* pages, int pages_on_device, int n_pages, int H0, int W0,
                          float* prob_out, int out_on_device, void* cuda_stream);
 /* model-level seam: x = normalised (n,3,H,W) fp32 exactly as the reference feeds DBNet.forward; H, W % 32 == 0 */
@@ -284,7 +285,9 @@ int ytk_op_apply_rep_cut(const int* rep_cut, int B, int S, int C, int eos_id, in
  * and scratch go to buffers allocated and freed on it); invalid arguments are an error, not a launch.
  *   preprocess  n BGR u8 pages [n, H0, W0, 3] -> the stem's canvas [n, Hn+6, Wn+8, 8], all of it written: pixel (h, w)
  *               at (h+3, w+3), channels 0..2 = cv2.resize(INTER_AREA) / 255 with the mean / std applied by position
- *               to B, G, R, zero border and zero channels 3..7.  Hn <= H0 and Wn <= W0 (decimation only).
+ *               to B, G, R, zero border and zero channels 3..7.  Hn <= H0 and Wn <= W0 (OpenCV's area decimation).
+ *   preprocess_up  the same for the shapes where some axis grows (Hn > H0 or Wn > W0), which OpenCV's INTER_AREA
+ *               resamples bilinearly on both axes with its "area-mode" coefficients.
  *   stem        7x7 / stride 2 / pad 3 conv (w [64][3][7][7], bias [64]) + ReLU over that canvas -> out
  *               [n, Hn/2, Wn/2, 64]; Hn and Wn multiples of 32.
  *   maxpool     max_pool2d(3, 2, 1): in [n, H, W, C] -> out [n, (H+1)/2, (W+1)/2, C]; C a multiple of 8.
@@ -297,6 +300,8 @@ int ytk_op_apply_rep_cut(const int* rep_cut, int B, int S, int C, int eos_id, in
  *               -> prob [n, 4H, 4W] fp32 (8-byte aligned); w1 [64][64][2][2], b1 [64], w2 [64][1][2][2], b2. */
 int ytk_op_dbnet_preprocess_u8(const uint8_t* src_dev, int n, int H0, int W0, int Hn, int Wn, void* canvas_dev,
                                void* cuda_stream);
+int ytk_op_dbnet_preprocess_up_u8(const uint8_t* src_dev, int n, int H0, int W0, int Hn, int Wn, void* canvas_dev,
+                                  void* cuda_stream);
 int ytk_op_dbnet_stem_f16(const void* canvas_dev, int n, int Hn, int Wn, const float* w_host, const float* bias_host,
                           void* out_dev, void* cuda_stream);
 int ytk_op_maxpool3x3s2_f16(const void* in, int n, int H, int W, int C, void* out, void* cuda_stream);

@@ -75,6 +75,8 @@ def _declare(lib):
     lib.ytk_op_apply_rep_cut.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]
     lib.ytk_op_dbnet_preprocess_u8.restype = c_int
     lib.ytk_op_dbnet_preprocess_u8.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
+    lib.ytk_op_dbnet_preprocess_up_u8.restype = c_int
+    lib.ytk_op_dbnet_preprocess_up_u8.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
     lib.ytk_op_dbnet_stem_f16.restype = c_int
     lib.ytk_op_dbnet_stem_f16.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
     lib.ytk_op_maxpool3x3s2_f16.restype = c_int

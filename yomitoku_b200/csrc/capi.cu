@@ -525,28 +525,46 @@ static void* stream_buffer(const void* host, size_t bytes, cudaStream_t st, cons
     return d;
 }
 
-int ytk_op_dbnet_preprocess_u8(const uint8_t* src_dev, int n, int H0, int W0, int Hn, int Wn, void* canvas_dev,
-                               void* cuda_stream) {
+// The two pre-processing entries: `up` = 0 takes the shapes OpenCV decimates with its area tables (no axis grows),
+// `up` = 1 the shapes it up-scales bilinearly (some axis grows).  One launcher serves both and picks by the same rule.
+static int op_dbnet_preprocess(const char* who, int up, const uint8_t* src_dev, int n, int H0, int W0, int Hn, int Wn,
+                               void* canvas_dev, void* cuda_stream) {
     if (!src_dev || !canvas_dev) {
-        ytk::set_error("ytk_op_dbnet_preprocess_u8: null argument");
+        ytk::set_error("%s: null argument", who);
         return YTK_ERR;
     }
     if (n < 1 || H0 < 1 || W0 < 1 || Hn < 1 || Wn < 1) {
-        ytk::set_error("ytk_op_dbnet_preprocess_u8: non-positive size (n %d, page %dx%d, input %dx%d)", n, H0, W0, Hn, Wn);
+        ytk::set_error("%s: non-positive size (n %d, page %dx%d, input %dx%d)", who, n, H0, W0, Hn, Wn);
         return YTK_ERR;
     }
-    if (Hn > H0 || Wn > W0) {
-        ytk::set_error("ytk_op_dbnet_preprocess_u8: %dx%d -> %dx%d is an upscale; INTER_AREA decimation only", H0, W0, Hn,
-                       Wn);
+    const bool grows = Hn > H0 || Wn > W0;
+    if (grows && !up) {
+        ytk::set_error("%s: %dx%d -> %dx%d is an upscale; INTER_AREA decimation only (ytk_op_dbnet_preprocess_up_u8 "
+                       "takes it)", who, H0, W0, Hn, Wn);
+        return YTK_ERR;
+    }
+    if (!grows && up) {
+        ytk::set_error("%s: %dx%d -> %dx%d grows no axis; INTER_AREA decimation is ytk_op_dbnet_preprocess_u8", who, H0,
+                       W0, Hn, Wn);
         return YTK_ERR;
     }
     if (misaligned(canvas_dev, 16)) {
-        ytk::set_error("ytk_op_dbnet_preprocess_u8: canvas_dev must be 16-byte aligned");
+        ytk::set_error("%s: canvas_dev must be 16-byte aligned", who);
         return YTK_ERR;
     }
     return ytk::launch_preprocess(src_dev, n, H0, W0, Hn, Wn, canvas_dev, static_cast<cudaStream_t>(cuda_stream))
                ? YTK_ERR
                : YTK_OK;
+}
+
+int ytk_op_dbnet_preprocess_u8(const uint8_t* src_dev, int n, int H0, int W0, int Hn, int Wn, void* canvas_dev,
+                               void* cuda_stream) {
+    return op_dbnet_preprocess("ytk_op_dbnet_preprocess_u8", 0, src_dev, n, H0, W0, Hn, Wn, canvas_dev, cuda_stream);
+}
+
+int ytk_op_dbnet_preprocess_up_u8(const uint8_t* src_dev, int n, int H0, int W0, int Hn, int Wn, void* canvas_dev,
+                                  void* cuda_stream) {
+    return op_dbnet_preprocess("ytk_op_dbnet_preprocess_up_u8", 1, src_dev, n, H0, W0, Hn, Wn, canvas_dev, cuda_stream);
 }
 
 int ytk_op_dbnet_stem_f16(const void* canvas_dev, int n, int Hn, int Wn, const float* w_host, const float* bias_host,
@@ -780,12 +798,6 @@ int ytk_dbnet_forward_u8(ytk_dbnet* h, const uint8_t* pages, int pages_on_device
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
     int Hn, Wn;
     ytk::dbnet_input_size(H0, W0, h->shortest, h->limit, &Hn, &Wn);
-    if (Hn > H0 || Wn > W0) {
-        ytk::set_error("ytk_dbnet_forward_u8: page %dx%d would be upscaled to %dx%d; the fused u8 path implements "
-                       "OpenCV's INTER_AREA decimation only - resize on the host and call ytk_dbnet_forward_f32",
-                       H0, W0, Hn, Wn);
-        return YTK_ERR;
-    }
     ytk::DbnetEngine* e = get_engine(h, n_pages, Hn, Wn);
     if (!e) return YTK_ERR;
     order_after_previous(h, st);

@@ -23,7 +23,9 @@ __device__ __forceinline__ uint4 pack8(const float* f) {
 // BGR u8 page -> float -> cv2.resize(INTER_AREA) to (Hn, Wn) -> /255 -> (x - mean[c]) / std[c] applied positionally
 // to the B,G,R planes (SURVEY.md Appendix A2) -> network input.  Output layout: zero-padded NHWC with 8 channels,
 // pixel (h, w) at padded position (h + 3, w + 3) of a [Hn+6, Wn+8] canvas (the 7x7/stride-2 stem reads it through
-// overlapping TMA boxes, see dbnet_engine.cu).  The area resampling restates OpenCV's ResizeArea tables in fp32.
+// overlapping TMA boxes, see dbnet_engine.cu).  One kernel body, templated on the resampler, which OpenCV picks by the
+// scales: AreaSampler (ResizeArea tables) when both axes shrink or keep their size, AreaUpSampler (bilinear with
+// "area-mode" coefficients) when some axis grows.  Both restate OpenCV's tables in fp32.
 // ------------------------------------------------------------------------------------------------------------------
 struct AreaTap { int lo; int hi; float w_lo; float w_mid; float w_hi; };  // src indices [lo, hi], edge weights
 
@@ -51,21 +53,13 @@ __device__ __forceinline__ AreaTap area_tap(int d, double scale, int ssize) {
     return t;
 }
 
-__global__ void preprocess_kernel(const uint8_t* __restrict__ src, int n_img, int H0, int W0, int Hn, int Wn,
-                                  op_t* __restrict__ dst) {
-    const int Hp = Hn + 6, Wp = Wn + 8;
-    const long long total = (long long)n_img * Hp * Wp;
-    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= total) return;
-    const int wp = (int)(idx % Wp);
-    const int hp = (int)((idx / Wp) % Hp);
-    const int img = (int)(idx / ((long long)Wp * Hp));
-    float o[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    const int h = hp - 3, w = wp - 3;
-    if (h >= 0 && h < Hn && w >= 0 && w < Wn) {
+// OpenCV's ResizeArea: pixel (h, w) of page img as fp32 B, G, R on the 0..255 scale
+struct AreaSampler {
+    __device__ __forceinline__ static void sample(const uint8_t* src, int img, int H0, int W0, int Hn, int Wn, int h,
+                                                  int w, float* acc) {
         const double sy = (double)H0 / Hn, sx = (double)W0 / Wn;
         const AreaTap ty = area_tap(h, sy, H0), tx = area_tap(w, sx, W0);
-        float acc[3] = {0.f, 0.f, 0.f};
+        acc[0] = acc[1] = acc[2] = 0.f;
         const uint8_t* base = src + (size_t)img * H0 * W0 * 3;
         for (int y = ty.lo; y <= ty.hi; ++y) {
             const float wy = (y == ty.lo && ty.w_lo > 0.f) ? ty.w_lo : ((y == ty.hi && ty.w_hi > 0.f) ? ty.w_hi : ty.w_mid);
@@ -82,6 +76,64 @@ __global__ void preprocess_kernel(const uint8_t* __restrict__ src, int n_img, in
             acc[1] += wy * row[1];
             acc[2] += wy * row[2];
         }
+    }
+};
+
+struct UpTap { int s0; int s1; float f; };  // value = S[s0] (1 - f) + S[s1] f
+
+__device__ __forceinline__ UpTap area_up_tap(int d, int ssize, int dsize) {
+    // OpenCV resize() with INTER_AREA when some axis grows, for destination index d of one axis (either axis: a
+    // shrinking one is sampled the same way).  scale must be 1 / (dsize / ssize) as in OpenCV, not ssize / dsize: where
+    // d * scale lands on an integer the two can floor to neighbouring pixels.  The products are rounded on their own
+    // (no FMA), as OpenCV's host code computes them.
+    const double inv = (double)dsize / ssize, scale = 1.0 / inv;
+    int s = (int)floor(__dmul_rn((double)d, scale));          // >= 0: d >= 0
+    float f = (float)((double)(d + 1) - __dmul_rn((double)(s + 1), inv));
+    f = f <= 0.f ? 0.f : f - floorf(f);
+    if (s >= ssize - 1) {
+        s = ssize - 1;
+        f = 0.f;
+    }
+    UpTap t;
+    t.s0 = s;
+    t.s1 = min(s + 1, ssize - 1);  // with f = 0 the second tap adds exactly 0
+    t.f = f;
+    return t;
+}
+
+// OpenCV's INTER_AREA up-scaling: a horizontal pass over two source rows, then a vertical one, in fp32
+struct AreaUpSampler {
+    __device__ __forceinline__ static void sample(const uint8_t* src, int img, int H0, int W0, int Hn, int Wn, int h,
+                                                  int w, float* acc) {
+        const UpTap ty = area_up_tap(h, H0, Hn), tx = area_up_tap(w, W0, Wn);
+        const uint8_t* base = src + (size_t)img * H0 * W0 * 3;
+        const uint8_t* r0 = base + (size_t)ty.s0 * W0 * 3;
+        const uint8_t* r1 = base + (size_t)ty.s1 * W0 * 3;
+        const float ax = 1.f - tx.f, ay = 1.f - ty.f;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            const float v0 = r0[tx.s0 * 3 + c] * ax + r0[tx.s1 * 3 + c] * tx.f;
+            const float v1 = r1[tx.s0 * 3 + c] * ax + r1[tx.s1 * 3 + c] * tx.f;
+            acc[c] = v0 * ay + v1 * ty.f;
+        }
+    }
+};
+
+template <class Sampler>
+__global__ void preprocess_kernel(const uint8_t* __restrict__ src, int n_img, int H0, int W0, int Hn, int Wn,
+                                  op_t* __restrict__ dst) {
+    const int Hp = Hn + 6, Wp = Wn + 8;
+    const long long total = (long long)n_img * Hp * Wp;
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= total) return;
+    const int wp = (int)(idx % Wp);
+    const int hp = (int)((idx / Wp) % Hp);
+    const int img = (int)(idx / ((long long)Wp * Hp));
+    float o[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    const int h = hp - 3, w = wp - 3;
+    if (h >= 0 && h < Hn && w >= 0 && w < Wn) {
+        float acc[3];
+        Sampler::sample(src, img, H0, W0, Hn, Wn, h, w, acc);
         // channel order seen by the network is B,G,R with the ImageNet RGB mean/std applied positionally
         const float mean[3] = {0.485f, 0.456f, 0.406f}, stdv[3] = {0.229f, 0.224f, 0.225f};
 #pragma unroll
@@ -93,8 +145,13 @@ __global__ void preprocess_kernel(const uint8_t* __restrict__ src, int n_img, in
 int launch_preprocess(const uint8_t* src, int n_img, int H0, int W0, int Hn, int Wn, void* dst, cudaStream_t st) {
     const long long total = (long long)n_img * (Hn + 6) * (Wn + 8);
     const int threads = 256;
-    preprocess_kernel<<<(unsigned)((total + threads - 1) / threads), threads, 0, st>>>(
-        src, n_img, H0, W0, Hn, Wn, reinterpret_cast<op_t*>(dst));
+    const unsigned blocks = (unsigned)((total + threads - 1) / threads);
+    op_t* out = reinterpret_cast<op_t*>(dst);
+    // OpenCV's rule: true area resampling only when neither axis grows
+    if (Hn <= H0 && Wn <= W0)
+        preprocess_kernel<AreaSampler><<<blocks, threads, 0, st>>>(src, n_img, H0, W0, Hn, Wn, out);
+    else
+        preprocess_kernel<AreaUpSampler><<<blocks, threads, 0, st>>>(src, n_img, H0, W0, Hn, Wn, out);
     count_launch();
     return cudaGetLastError() != cudaSuccess;
 }

@@ -7,6 +7,7 @@ namespace ytk {
 
 constexpr int kAsfPoolChunks = 64;   // launch_asf: gsum holds n_img * kAsfPoolChunks * 64 floats (partial channel sums)
 
+// cv2.resize(INTER_AREA) either way: area resampling when neither axis grows, OpenCV's bilinear up-scaling otherwise
 int launch_preprocess(const uint8_t* src_bgr, int n_img, int H0, int W0, int Hn, int Wn, void* dst_padded_nhwc8,
                       cudaStream_t st);
 int launch_pack_nchw_f32(const float* src_nchw, int n_img, int Hn, int Wn, void* dst_padded_nhwc8, cudaStream_t st);

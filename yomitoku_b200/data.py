@@ -2,8 +2,8 @@
 src/yomitoku/data/functions.py:196-439 and data/dataset.py:19-129.
 
 These are the host versions of rows R1 / R4 of SURVEY.md section 8a, exactly as the reference runs them; both rows also
-exist on the GPU: the detector's resize + normalisation fused in csrc/dbnet_ops.cu (preprocess_kernel; the functions
-here serve the model-level seam and pages that need up-scaling), and the crop extraction in csrc/crop_ops.cu, for which
+exist on the GPU: the detector's resize + normalisation fused in csrc/dbnet_ops.cu (preprocess_kernel, for pages that
+shrink or grow; the functions here serve the model-level seam), and the crop extraction in csrc/crop_ops.cu, for which
 `crop_geometry` / `crop_records` below compute the per-quad records (everything that follows from the quads alone).
 """
 from concurrent.futures import ThreadPoolExecutor

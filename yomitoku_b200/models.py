@@ -356,8 +356,9 @@ class DBNet(_DeviceModel):
         return OrderedDict(binary=out)
 
     def detect_pages_u8(self, pages, out=None, stream=None):
-        """Fused fast path: pages (n,H0,W0,3) uint8 BGR (numpy / torch, host or cuda) -> (n,Hn,Wn) fp32 probability
-        maps (pre-processing runs on the GPU).  Pages that would be up-scaled need the model-level seam."""
+        """Fused fast path: pages (n,H0,W0,3) uint8 BGR of any size (numpy / torch, host or cuda) -> (n,Hn,Wn) fp32
+        probability maps.  The pre-processing runs on the GPU: cv2.resize(INTER_AREA) to input_size, whether the page
+        shrinks or grows, then the normalisation of TextDetector.preprocess."""
         h = self._ensure()
         t = pages if isinstance(pages, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(pages))
         if t.dim() == 3:

@@ -304,14 +304,14 @@ class BatchedOCR:
 
     def _stage(self, pages, shared):
         """Host staging of a batch of same-size pages: (stage (n,H,W,3) u8 tensor, out (n,Hn,Wn) f32 tensor).  With
-        `shared` (pages that are only decimated) both live in the shared page-locked ring - the H2D/D2H copies are plain
-        DMAs and the workers read both without a copy; `self._last_shared` then holds the two buffers."""
+        `shared` both live in the shared page-locked ring - the H2D/D2H copies are plain DMAs and the workers read both
+        without a copy; `self._last_shared` then holds the two buffers."""
         import torch
         n = len(pages)
         h0, w0 = pages[0].shape[:2]
         hn, wn = self.detector.model.input_size(h0, w0)
         self._last_shared = None
-        if shared and hn <= h0 and wn <= w0:
+        if shared:
             pb = self._shared("pages", n * h0 * w0 * 3)
             ob = self._shared("prob", n * hn * wn * 4)
             sn = pb.view(0, (n, h0, w0, 3), np.uint8)

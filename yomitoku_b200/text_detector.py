@@ -1,8 +1,8 @@
 """TextDetector: DBNet++ behind the reference's module API.
 
 Mirrors reference src/yomitoku/text_detector.py:26-146 - same catalog names (`dbnet`, `dbnetv2`, `dbnetv2_1`),
-constructor kwargs, `preprocess` / `postprocess` / `__call__` contract and result schema.  The model forward (and,
-for pages that only need decimation, the resize + normalisation in front of it) runs as sm_90a kernels; contour
+constructor kwargs, `preprocess` / `postprocess` / `__call__` contract and result schema.  The resize + normalisation
+(cv2.resize INTER_AREA, whether the page shrinks or grows) and the model forward run as sm_90a kernels; contour
 extraction / unclip stay on the host like the reference (SURVEY.md R3).  `infer_onnx` is accepted and ignored:
 ONNX / multi-backend dispatch is out of scope for this path.
 """
@@ -13,7 +13,7 @@ import torch
 
 from .base import BaseModelCatalog, BaseModule, logger
 from .config import TextDetectorDBNetConfig, TextDetectorDBNetV2_1Config, TextDetectorDBNetV2Config
-from .data import array_to_tensor, resize_shortest_edge, shortest_edge_size, standardization_image
+from .data import array_to_tensor, resize_shortest_edge, standardization_image
 from .models import DBNet
 from .postprocessor import DBnetPostProcessor
 from .schemas import TextDetectorSchema
@@ -45,13 +45,19 @@ class TextDetector(BaseModule):
         self.load_model(model_name, path_cfg, from_pretrained=from_pretrained)
         self.model.eval().to(self.device)
         self.post_processor = DBnetPostProcessor(**self._cfg.post_process)
+        # the pre-processing is a CUDA kernel: a detector placed on the CPU (a stand-in model with only the reference's
+        # `model(tensor)` contract) runs the reference's host flow, preprocess + model + postprocess
+        self.on_cuda = torch.device(device).type == "cuda"
         # front half of the post-processing (threshold, connected components, per-component sums) on the device: only
         # the components' row runs come back instead of the probability map.  Pages that need OpenCV's view of the
         # bitmap (a component with a hole) fall back to the host path per page - the result is the same either way.
-        self.device_post = os.environ.get("YTK_DEVICE_POST", "1") != "0" and torch.cuda.is_available()
+        self.device_post = (self.on_cuda and os.environ.get("YTK_DEVICE_POST", "1") != "0"
+                            and torch.cuda.is_available())
 
     def preprocess(self, img):
-        """BGR u8 page -> normalised (1,3,H',W') fp32 tensor; reference text_detector.py:99-107 (host path)."""
+        """BGR u8 page -> normalised (1,3,H',W') fp32 tensor; reference text_detector.py:99-107 (host path: the
+        reference's API and the model-level seam `model(preprocess(img))`; on a CUDA device `__call__` pre-processes the
+        u8 page on the device instead)."""
         img = img.copy()
         img = img[:, :, ::-1].astype(np.float32)
         resized = resize_shortest_edge(img, self._cfg.data.shortest_size, self._cfg.data.limit_size)
@@ -77,30 +83,23 @@ class TextDetector(BaseModule):
         return out
 
     def _detect_device(self, pages_u8):
-        """(n, H0, W0, 3) u8 pages that are only decimated -> per page (quads, scores) through the device front half."""
+        """(n, H0, W0, 3) u8 pages -> per page (quads, scores) through the device front half."""
         t = torch.from_numpy(pages_u8).to(self.model.cuda_device(), non_blocking=False)
         prob = self.model.detect_pages_u8(t)
         return self.postprocess_device(prob, pages_u8.shape[1:3])
 
-    def _decimated(self, h, w):
-        hn, wn = shortest_edge_size(h, w, self._cfg.data.shortest_size, self._cfg.data.limit_size)
-        return hn <= h and wn <= w
-
     def _probability_map(self, img):
-        ori_h, ori_w = img.shape[:2]
-        hn, wn = shortest_edge_size(ori_h, ori_w, self._cfg.data.shortest_size, self._cfg.data.limit_size)
-        if hn <= ori_h and wn <= ori_w:
-            # decimation only: fused GPU pre-processing straight from the u8 page
-            prob = self.model.detect_pages_u8(np.ascontiguousarray(img))
-            return prob.cpu().numpy()[:, None] if prob.is_cuda else prob.numpy()[:, None]
-        tensor = self.preprocess(img)
-        with torch.inference_mode():
-            return self.model(tensor)["binary"].cpu().numpy()
+        if not self.on_cuda:
+            with torch.inference_mode():
+                return self.model(self.preprocess(img))["binary"].cpu().numpy()
+        # fused GPU pre-processing straight from the u8 page, whether it shrinks or grows
+        prob = self.model.detect_pages_u8(np.ascontiguousarray(img))
+        return prob.cpu().numpy()[:, None] if prob.is_cuda else prob.numpy()[:, None]
 
     def __call__(self, img):
         """Apply the detection model to a BGR page (np.ndarray HxWx3 u8); returns (TextDetectorSchema, vis)."""
         ori_h, ori_w = img.shape[:2]
-        if self.device_post and self._decimated(ori_h, ori_w):
+        if self.device_post:
             quads, scores = self._detect_device(np.ascontiguousarray(img)[None])[0]
         else:
             preds = {"binary": self._probability_map(img)}
@@ -115,7 +114,7 @@ class TextDetector(BaseModule):
         """Batched entry (new surface, SURVEY.md section 0): list of same-size BGR pages -> list of
         TextDetectorSchema.  One device launch sequence for the whole batch, host post-processing per page."""
         arr = np.stack([np.ascontiguousarray(p) for p in pages])
-        if self.device_post and self._decimated(*arr.shape[1:3]):
+        if self.device_post:
             return [TextDetectorSchema(points=q, scores=s) for q, s in self._detect_device(arr)]
         prob = self.model.detect_pages_u8(arr)
         prob = prob.cpu().numpy() if prob.is_cuda else prob.numpy()
