@@ -83,27 +83,43 @@ constexpr int kEpiStageBytes = 8 * 32 * kStagePitch;
 constexpr int kAccPitch = 68;
 constexpr int kAccBytes = 2 * 64 * kAccPitch * 4;
 
-// TMA epilogue (DIRECT == 2): every epilogue warp owns a ring of 2 KB buffers (32 tile rows x 64 bytes, 64-byte
-// swizzled = the layout a TMA box of that shape has in shared memory).  Two per warp: with a residual one box is in
-// flight (loaded by TMA while the MMAs of the tile run) while the other is being stored; without one they double-buffer
-// the TMA stores.  A deeper ring would cost the 256-wide tiles one of their three K stages.
-constexpr int kEpiBufBytes = 32 * 64;
-constexpr int epi_tma_nbuf(int /*resid*/) { return 2; }
+// TMA epilogue (DIRECT == 2): works on the accumulator fragments directly (no slice buffer).  Every epilogue warp owns
+// a ring of kEpiTmaBufs 2 KB buffers (16 tile rows x 128 bytes, 128-byte swizzled = the layout a TMA box of that shape
+// has in shared memory).  With a residual, the boxes of the next three passes are in flight (the first ones of a tile
+// load while its MMAs run) while one is being stored; without one they buffer the TMA stores.  Four boxes per warp
+// fit in the bytes the slice buffer used to take, so every tile width keeps its K stages.
+constexpr int kEpiBufBytes = 16 * 128;
+constexpr int kEpiTmaBufs = 4;
 constexpr int kSmemLimit = 232448;  // 227 KB of dynamic shared memory per CTA
 constexpr int kSmemFixed = 1024 /*final-conv weights*/ + 1024 /*align slack*/ + 512 /*barriers*/;
 
-template <int BLOCK_N, int EPI_BYTES = kEpiStageBytes>
+template <int BLOCK_N, int EPI_BYTES = kEpiStageBytes, int ACC_BYTES = kAccBytes>
 struct TileCfg {
     static constexpr int kBBytes = BLOCK_N * kBlockK * 2;
     static constexpr int kStageBytes = kABytes + kBBytes;
-    static constexpr int kRingBudget = kSmemLimit - kSmemFixed - kAccBytes - EPI_BYTES;
+    static constexpr int kAccB = ACC_BYTES;   // accumulator slice buffers (none in the TMA epilogue)
+    static constexpr int kRingBudget = kSmemLimit - kSmemFixed - ACC_BYTES - EPI_BYTES;
     static constexpr int kStages = (kRingBudget / kStageBytes) > 8 ? 8 : (kRingBudget / kStageBytes);
     static constexpr int kRingBytes = kStages * kStageBytes;
-    static constexpr int kSmemBytes = kRingBytes + kAccBytes + EPI_BYTES + kSmemFixed;
+    static constexpr int kSmemBytes = kRingBytes + ACC_BYTES + EPI_BYTES + kSmemFixed;
     static_assert(kStages >= 3, "K pipeline depth");
     static_assert(kSmemBytes <= kSmemLimit, "shared memory budget");
-    static_assert((kRingBytes + kAccBytes) % 2048 == 0, "epilogue buffers must stay 2 KB aligned");
+    static_assert((kRingBytes + ACC_BYTES) % 2048 == 0, "epilogue buffers must stay 2 KB aligned");
 };
+
+// 16-bit 8x8 matrix moves between shared memory and the mma fragment layout (thread t: row t / 4, columns 2 (t % 4),
+// +1); lane l gives the row address of matrix l / 8
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
+                 : "r"(addr)
+                 : "memory");
+}
+__device__ __forceinline__ void stsm_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+                 "r"(r2), "r"(r3)
+                 : "memory");
+}
 
 // ragged last columns of a row segment: element-wise copy (rare; kept out of line)
 __device__ __noinline__ void copy_elems(void* dst, const void* src, int n, int esz) {
@@ -156,7 +172,8 @@ __device__ __forceinline__ TileCoord decode_tile(const GemmArgs& a, int tile, in
 // so that each instantiation carries only its own store path - one kernel with every path inlined thrashes the
 // instruction cache.
 template <int BLOCK_N, int RESID, int DIRECT>
-using KernelCfg = TileCfg<BLOCK_N, DIRECT == 2 ? 8 * epi_tma_nbuf(RESID) * kEpiBufBytes : kEpiStageBytes>;
+using KernelCfg = TileCfg<BLOCK_N, DIRECT == 2 ? 8 * kEpiTmaBufs * kEpiBufBytes : kEpiStageBytes,
+                          DIRECT == 2 ? 0 : kAccBytes>;
 
 // DIRECT: 0 = staged epilogue (registers -> per-warp shared staging -> coalesced per-thread global accesses),
 //         1 = row per thread straight to global memory (A/B aid, not dispatched),
@@ -165,7 +182,7 @@ template <int BLOCK_N, int OUT_F32, int RESID, int MODE, int DIRECT>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ GemmMaps maps,
                                                               const __grid_constant__ GemmArgs args) {
     using Cfg = KernelCfg<BLOCK_N, RESID, DIRECT>;
-    constexpr int kEpiBytes = Cfg::kSmemBytes - Cfg::kRingBytes - kAccBytes - kSmemFixed;
+    constexpr int kEpiBytes = Cfg::kSmemBytes - Cfg::kRingBytes - Cfg::kAccB - kSmemFixed;
     constexpr int stage_bytes = Cfg::kStageBytes;
     constexpr int nstages = Cfg::kStages;
     extern __shared__ uint8_t smem_raw[];
@@ -175,7 +192,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     const int n_workers = static_cast<int>(gridDim.x);
 
     float* acc_smem = reinterpret_cast<float*>(smem + Cfg::kRingBytes);
-    uint8_t* epi_stage = smem + Cfg::kRingBytes + kAccBytes;
+    uint8_t* epi_stage = smem + Cfg::kRingBytes + Cfg::kAccB;
     float* fin_w = reinterpret_cast<float*>(epi_stage + kEpiBytes);  // [4][64] weights of the fused final conv
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_stage + kEpiBytes + 1024);
     uint64_t* empty_bar = full_bar + 8;
@@ -260,12 +277,12 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         }
     } else {
         // ------------------------------------------------------------------ consumers (warps 0..7)
-        // Warpgroup wg computes tile rows [64 wg, 64 wg + 64) with wgmma, then runs the epilogue on them: warp wl of the
+        // Warpgroup wg computes tile rows [64 wg, 64 wg + 64) with wgmma, then runs the epilogue on them.  The TMA
+        // epilogue (DIRECT == 2, below) works on each warp's own 16 fragment rows.  The staged one: warp wl of the
         // warpgroup stores the 32 rows of quadrant q (row per thread) and, of every 64-column slice, the 32-column chunk
         // of its set (the CONVT_FINAL epilogue pairs chunks instead, see below).  Values go registers -> slice buffer ->
-        // bias/residual/activation -> TMA boxes (residual in by cp.async.bulk.tensor, result out by TMA store) or, for
-        // the plans the TMA path does not cover, per-warp shared staging and coalesced 16-byte global accesses (4 lanes
-        // per 64-byte row segment), so DRAM sees whole sectors.
+        // bias/residual/activation -> per-warp shared staging and coalesced 16-byte global accesses (4 lanes per 64-byte
+        // row segment), so DRAM sees whole sectors.
         setmaxnreg_inc<232>();   // 2 x 128 x 232 + 128 x 40 <= 64 K registers
         const int wg = warp >> 2, wl = warp & 3;
         const int q = 2 * wg + (wl & 1);   // 32-row quadrant of the tile this warp stores
@@ -340,48 +357,58 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             }
         };
         if constexpr (DIRECT == 2) {
-            // ---- TMA epilogue.  A "pass" is one warp's share of 64 output bytes per row: 32 tile rows x CPP columns,
-            // one 2 KB box.  The warp's passes (units -> its chunks -> passes) form one sequence that indexes a ring of
-            // NBUF boxes: residual boxes are loaded LOOK passes ahead by lane 0 (the first ones of a tile while its MMAs
-            // run), a thread adds its own row in place, and lane 0 hands the box to a
-            // TMA store.  Rows / columns outside the tensor are zero-filled on load and dropped on store by the hardware.
+            // ---- TMA epilogue, straight from the wgmma fragments.  Warp w (= 4 wg + wl) holds tile rows 16 w + lane / 4
+            // (+ 8) and, of every 8-column group j, columns 8 j + 2 (lane % 4) (+ 1).  A "pass" is 128 bytes of columns of
+            // those 16 rows: one 2 KB box, 128-byte swizzled (16-byte chunk ^= row % 8), which the warp reads (residual)
+            // and writes (result) in the fragment layout - ldmatrix / stmatrix for 16-bit boxes, float2 accesses for
+            // fp32 ones, all conflict-free - before lane 0 hands it to a TMA store.  The warp's passes (units ->
+            // passes) form one sequence that indexes a ring of NBUF boxes: residual boxes are loaded LOOK passes ahead
+            // by lane 0 (the first ones of a tile while its MMAs run).  Rows / columns outside the tensor are
+            // zero-filled on load and dropped on store by the hardware.  Per element: (acc + bias) + residual, then the
+            // activation, then rounding - the order of the staged epilogue, so both give the same bits.
             static_assert(MODE == EPI_NORMAL, "TMA epilogue: plain stores only");
             static_assert(RESID == 0 || (RESID == 2) == (OUT_F32 != 0), "TMA epilogue: residual and output boxes match");
-            constexpr int NBUF = epi_tma_nbuf(RESID);
+            constexpr int NBUF = kEpiTmaBufs;
+            static_assert(NBUF <= 4, "residual barriers: 4 per warp");
             constexpr int LOOK = NBUF - 1;
-            constexpr int CPP = OUT_F32 ? 16 : 32;
-            constexpr int NPASS = 32 / CPP;
+            constexpr int CPB = OUT_F32 ? 32 : 64;   // columns per box (128 bytes)
+            constexpr int JPB = CPB / 8;             // 8-column fragment groups per box
+            constexpr int NPASS = BLOCK_N / CPB;
+            const int tr0 = warp * 16;               // first tile row of the warp
             const int bw_mask = (1 << args.bw_log2) - 1;
-            const int qw = (q * 32) & bw_mask;          // where the quadrant's 32 rows start inside the BH x BW patch
-            const int qh = (q * 32) >> args.bw_log2;
+            const int qw = tr0 & bw_mask;            // where the warp's 16 rows start inside the BH x BW patch
+            const int qh = tr0 >> args.bw_log2;
             uint8_t* bufs = epi_stage + warp * (NBUF * kEpiBufBytes);
             [[maybe_unused]] uint64_t* rbar = rbar_base + warp * 4;
-            const int sw = args.epi_swz ? ((lane >> 1) & 3) : 0;   // SWIZZLE_64B: 16 B chunk ^= (row / 2) % 4
-            const int row_off = lane * 64;
-            // residual prefetch cursor (lane 0 only): position (unit, chunk, pass) of the next box to load
-            [[maybe_unused]] int pf_u = worker, pf_c = wset, pf_p = 0, pf_g = 0;
+            const int swz = args.epi_swz ? 7 : 0;
+            const int fr = lane >> 2;                // fragment row (and fr + 8)
+            const int fc = (lane & 3) * 2;           // fragment column inside an 8-column group
+            // fp32 box: byte offset of (row fr, column 8 jj + fc) is f32_off + (((2 jj) ^ row) << 4) with the low chunk
+            // bit folded in below; row fr + 8 is 1024 bytes further (same swizzle phase)
+            const int f32_sub = (lane >> 1) & 1, f32_byte = (lane & 1) * 8;
+            // 16-bit box, ldmatrix / stmatrix x4 over groups (2 t, 2 t + 1): lane gives row mrow of 16-byte chunk
+            // 2 t + mchunk (matrices: rows 0-7 / 8-15 of group 2 t, then of group 2 t + 1)
+            const int mrow = ((lane >> 3) & 1) * 8 + (lane & 7), mchunk = lane >> 4;
+            // residual prefetch cursor (lane 0 only): position (unit, pass) of the next box to load
+            [[maybe_unused]] int pf_u = worker, pf_p = 0, pf_g = 0;
             [[maybe_unused]] TileCoord pf_tc{};
             [[maybe_unused]] auto pf_seek = [&]() {   // moves the cursor to the next existing pass at or after its position
                 while (pf_u < total_units) {
                     pf_tc = decode_tile(args, pf_u, BLOCK_N);
-                    if (pf_c < BLOCK_N / 32 && pf_tc.n0 + pf_c * 32 + pf_p * CPP < args.Cout) return;
-                    pf_c = wset;       // nothing (left) for this warp in the unit
-                    pf_p = 0;
+                    if (pf_p < NPASS && pf_tc.n0 + pf_p * CPB < args.Cout) return;
+                    pf_p = 0;          // nothing (left) in the unit
                     pf_u += n_workers;
                 }
             };
             [[maybe_unused]] auto pf_step = [&]() {
-                if (++pf_p == NPASS) {
-                    pf_p = 0;
-                    pf_c += 2;
-                }
+                ++pf_p;
                 pf_seek();
             };
             [[maybe_unused]] auto pf_issue = [&]() {
                 const int b = pf_g % NBUF;
                 mbar_expect_tx(&rbar[b], kEpiBufBytes);
-                tma_load_4d(bufs + b * kEpiBufBytes, &maps.resid, &rbar[b], pf_tc.n0 + pf_c * 32 + pf_p * CPP,
-                            pf_tc.w0 + qw, pf_tc.h0 + qh, pf_tc.img);
+                tma_load_4d(bufs + b * kEpiBufBytes, &maps.resid, &rbar[b], pf_tc.n0 + pf_p * CPB, pf_tc.w0 + qw,
+                            pf_tc.h0 + qh, pf_tc.img);
                 ++pf_g;
             };
             if constexpr (RESID != 0) {
@@ -397,111 +424,102 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             for (int u = worker; u < total_units; u += n_workers) {
                 const TileCoord tc = decode_tile(args, u, BLOCK_N);
                 mma_tile();
-#pragma unroll 1
-                for (int c = 0; c < BLOCK_N / 32; ++c) {
-                    const int col0 = tc.n0 + c * 32;
-                    if ((c & 1) == 0) {
-                        if (col0 >= args.Cout) break;  // warpgroup-uniform
-                        dump_slice(c >> 1);
-                    }
-                    if ((c & 1) != wset || col0 >= args.Cout) continue;
-                    float f[32];
-                    load_chunk(c, f);
-                    if (args.bias != nullptr) {
-                        if (col0 + 32 <= args.Cout) {
-                            const float4* b4 = reinterpret_cast<const float4*>(args.bias + col0);
+                // passes are unrolled: the fragment registers of a pass must be compile-time indices
 #pragma unroll
-                            for (int j = 0; j < 8; ++j) {
-                                const float4 b = __ldg(b4 + j);
-                                f[4 * j + 0] += b.x;
-                                f[4 * j + 1] += b.y;
-                                f[4 * j + 2] += b.z;
-                                f[4 * j + 3] += b.w;
+                for (int p = 0; p < NPASS; ++p) {
+                    const int col0 = tc.n0 + p * CPB;
+                    if (col0 >= args.Cout) break;   // warp-uniform; the cursor above skips the same passes
+                    const int b = gc % NBUF;
+                    uint8_t* box = bufs + b * kEpiBufBytes;
+                    const uint32_t box_s = smem_u32(box);
+                    float v[4 * JPB];
+#pragma unroll
+                    for (int i = 0; i < 4 * JPB; ++i) v[i] = acc[4 * JPB * p + i];
+                    if (args.bias != nullptr) {
+#pragma unroll
+                        for (int jj = 0; jj < JPB; ++jj) {
+                            const int col = col0 + 8 * jj + fc;   // Cout is even on this path: col < Cout covers col + 1
+                            const float2 bb = col < args.Cout ? __ldg(reinterpret_cast<const float2*>(args.bias + col))
+                                                              : make_float2(0.f, 0.f);
+                            v[4 * jj + 0] += bb.x;
+                            v[4 * jj + 1] += bb.y;
+                            v[4 * jj + 2] += bb.x;
+                            v[4 * jj + 3] += bb.y;
+                        }
+                    }
+                    if constexpr (RESID != 0) {
+                        mbar_wait(&rbar[b], static_cast<uint32_t>(gc / NBUF) & 1u);
+                        if constexpr (RESID == 2) {
+#pragma unroll
+                            for (int jj = 0; jj < JPB; ++jj) {
+                                const uint8_t* rp = box + fr * 128 + (((2 * jj + f32_sub) ^ (fr & swz)) << 4) + f32_byte;
+                                const float2 r0 = *reinterpret_cast<const float2*>(rp);
+                                const float2 r1 = *reinterpret_cast<const float2*>(rp + 1024);
+                                v[4 * jj + 0] += r0.x;
+                                v[4 * jj + 1] += r0.y;
+                                v[4 * jj + 2] += r1.x;
+                                v[4 * jj + 3] += r1.y;
                             }
                         } else {
 #pragma unroll
-                            for (int j = 0; j < 32; ++j) f[j] += __ldg(args.bias + min(col0 + j, args.Cout - 1));
+                            for (int t = 0; t < JPB / 2; ++t) {
+                                uint32_t r0, r1, r2, r3;
+                                ldsm_x4(box_s + mrow * 128 + (((2 * t + mchunk) ^ (mrow & swz)) << 4), r0, r1, r2, r3);
+                                v[8 * t + 0] += op_lo(r0); v[8 * t + 1] += op_hi(r0);
+                                v[8 * t + 2] += op_lo(r1); v[8 * t + 3] += op_hi(r1);
+                                v[8 * t + 4] += op_lo(r2); v[8 * t + 5] += op_hi(r2);
+                                v[8 * t + 6] += op_lo(r3); v[8 * t + 7] += op_hi(r3);
+                            }
+                        }
+                        __syncwarp();   // every lane has read the residual before the results overwrite the box
+                    } else {
+                        // the store that used this buffer NBUF passes ago must have read it
+                        if (lane == 0) bulk_wait_read<NBUF - 1>();
+                        __syncwarp();
+                    }
+                    if (args.act == ACT_RELU) {
+#pragma unroll
+                        for (int j = 0; j < 4 * JPB; ++j) v[j] = fmaxf(v[j], 0.f);
+                    } else if (args.act == ACT_GELU) {
+#pragma unroll
+                        for (int j = 0; j < 4 * JPB; j += 2) gelu_fast2(v[j], v[j + 1]);
+                    } else if (args.act == ACT_SIGMOID) {
+#pragma unroll
+                        for (int j = 0; j < 4 * JPB; ++j) v[j] = __fdividef(1.f, 1.f + __expf(-v[j]));
+                    } else if (args.act == ACT_SILU) {
+#pragma unroll
+                        for (int j = 0; j < 4 * JPB; ++j) v[j] = __fdividef(v[j], 1.f + __expf(-v[j]));
+                    }
+                    if constexpr (OUT_F32) {
+#pragma unroll
+                        for (int jj = 0; jj < JPB; ++jj) {
+                            uint8_t* wp = box + fr * 128 + (((2 * jj + f32_sub) ^ (fr & swz)) << 4) + f32_byte;
+                            *reinterpret_cast<float2*>(wp) = make_float2(v[4 * jj + 0], v[4 * jj + 1]);
+                            *reinterpret_cast<float2*>(wp + 1024) = make_float2(v[4 * jj + 2], v[4 * jj + 3]);
+                        }
+                    } else {
+#pragma unroll
+                        for (int t = 0; t < JPB / 2; ++t)
+                            stsm_x4(box_s + mrow * 128 + (((2 * t + mchunk) ^ (mrow & swz)) << 4),
+                                    pack_op(v[8 * t + 0], v[8 * t + 1]), pack_op(v[8 * t + 2], v[8 * t + 3]),
+                                    pack_op(v[8 * t + 4], v[8 * t + 5]), pack_op(v[8 * t + 6], v[8 * t + 7]));
+                    }
+                    fence_proxy_async_smem();   // the box just written -> visible to the TMA store
+                    __syncwarp();
+                    if (lane == 0) {
+                        tma_store_4d(&maps.out, box, col0, tc.w0 + qw, tc.h0 + qh, tc.img);
+                        bulk_commit();
+                        if constexpr (RESID != 0) {
+                            if (pf_u < total_units) {
+                                // the next box goes where pass gc - 1 was stored from: all but the store just
+                                // committed must have read their source
+                                bulk_wait_read<1>();
+                                pf_issue();
+                                pf_step();
+                            }
                         }
                     }
-#pragma unroll
-                    for (int p = 0; p < NPASS; ++p) {
-                        if (col0 + p * CPP < args.Cout) {   // warp-uniform; the cursor above skips the same passes
-                            const int b = gc % NBUF;
-                            uint8_t* box = bufs + b * kEpiBufBytes;
-                            uint8_t* my_row = box + row_off;
-                            if constexpr (RESID != 0) {
-                                mbar_wait(&rbar[b], static_cast<uint32_t>(gc / NBUF) & 1u);
-#pragma unroll
-                                for (int j = 0; j < 4; ++j) {
-                                    const uint4 r = *reinterpret_cast<const uint4*>(my_row + ((j ^ sw) << 4));
-                                    if constexpr (RESID == 2) {
-                                        f[p * 16 + 4 * j + 0] += __uint_as_float(r.x);
-                                        f[p * 16 + 4 * j + 1] += __uint_as_float(r.y);
-                                        f[p * 16 + 4 * j + 2] += __uint_as_float(r.z);
-                                        f[p * 16 + 4 * j + 3] += __uint_as_float(r.w);
-                                    } else {
-                                        const int e = p * CPP + 8 * j;
-                                        f[e + 0] += op_lo(r.x); f[e + 1] += op_hi(r.x);
-                                        f[e + 2] += op_lo(r.y); f[e + 3] += op_hi(r.y);
-                                        f[e + 4] += op_lo(r.z); f[e + 5] += op_hi(r.z);
-                                        f[e + 6] += op_lo(r.w); f[e + 7] += op_hi(r.w);
-                                    }
-                                }
-                            } else {
-                                // the store that used this buffer NBUF passes ago must have read it
-                                if (lane == 0) bulk_wait_read<NBUF - 1>();
-                                __syncwarp();
-                            }
-                            if (args.act == ACT_RELU) {
-#pragma unroll
-                                for (int j = 0; j < CPP; ++j) f[p * CPP + j] = fmaxf(f[p * CPP + j], 0.f);
-                            } else if (args.act == ACT_GELU) {
-#pragma unroll
-                                for (int j = 0; j < CPP; j += 2) gelu_fast2(f[p * CPP + j], f[p * CPP + j + 1]);
-                            } else if (args.act == ACT_SIGMOID) {
-#pragma unroll
-                                for (int j = 0; j < CPP; ++j)
-                                    f[p * CPP + j] = __fdividef(1.f, 1.f + __expf(-f[p * CPP + j]));
-                            } else if (args.act == ACT_SILU) {
-#pragma unroll
-                                for (int j = 0; j < CPP; ++j)
-                                    f[p * CPP + j] = __fdividef(f[p * CPP + j], 1.f + __expf(-f[p * CPP + j]));
-                            }
-#pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                uint4 o;
-                                if constexpr (OUT_F32) {
-                                    o.x = __float_as_uint(f[p * 16 + 4 * j + 0]);
-                                    o.y = __float_as_uint(f[p * 16 + 4 * j + 1]);
-                                    o.z = __float_as_uint(f[p * 16 + 4 * j + 2]);
-                                    o.w = __float_as_uint(f[p * 16 + 4 * j + 3]);
-                                } else {
-                                    const int e = p * CPP + 8 * j;
-                                    o.x = pack_op(f[e + 0], f[e + 1]);
-                                    o.y = pack_op(f[e + 2], f[e + 3]);
-                                    o.z = pack_op(f[e + 4], f[e + 5]);
-                                    o.w = pack_op(f[e + 6], f[e + 7]);
-                                }
-                                *reinterpret_cast<uint4*>(my_row + ((j ^ sw) << 4)) = o;
-                            }
-                            fence_proxy_async_smem();   // the rows just written -> visible to the TMA store
-                            __syncwarp();
-                            if (lane == 0) {
-                                tma_store_4d(&maps.out, box, col0 + p * CPP, tc.w0 + qw, tc.h0 + qh, tc.img);
-                                bulk_commit();
-                                if constexpr (RESID != 0) {
-                                    if (pf_u < total_units) {
-                                        // the next box goes where pass gc - 1 was stored from: all but the store just
-                                        // committed must have read their source
-                                        bulk_wait_read<1>();
-                                        pf_issue();
-                                        pf_step();
-                                    }
-                                }
-                            }
-                            ++gc;
-                        }
-                    }
+                    ++gc;
                 }
             }
             if (lane == 0) bulk_wait_read<0>();   // shared memory must outlive the last stores' reads
@@ -932,8 +950,8 @@ int make_tmap_op_4d(CUtensorMap* m, const void* base, const uint64_t dims[4], co
 }
 
 // Output / residual tensor [n_img][Ho][Wo][Cout] (row pitch ld elements) as a 4-D map whose box is one epilogue warp's
-// share of a pass: 64 bytes of columns x the 32 tile rows of a quadrant (32 consecutive pixels of a row when
-// the patch is at least 32 wide, else 32 / BW full patch rows).
+// pass: 128 bytes of columns x the warp's 16 tile rows (16 consecutive pixels of a row when the patch is at least 16
+// wide, else 16 / BW full patch rows).
 static int make_tmap_epi(CUtensorMap* m, const void* base, int f32, const GemmArgs& a, int Cout, long long ld, int swz,
                          int tile_cols = 0) {
     EncodeTiledFn fn = get_encode_fn();
@@ -945,7 +963,7 @@ static int make_tmap_epi(CUtensorMap* m, const void* base, int f32, const GemmAr
     const int bw = 1 << a.bw_log2;
     cuuint64_t gd[4] = {(cuuint64_t)Cout, (cuuint64_t)a.Wo, (cuuint64_t)a.Ho, (cuuint64_t)a.n_img};
     cuuint64_t gs[3] = {(cuuint64_t)ld * es, (cuuint64_t)ld * es * a.Wo, (cuuint64_t)ld * es * a.Wo * a.Ho};
-    cuuint32_t bx[4] = {(cuuint32_t)(64 / es), (cuuint32_t)(bw < 32 ? bw : 32), (cuuint32_t)(bw < 32 ? 32 / bw : 1), 1};
+    cuuint32_t bx[4] = {(cuuint32_t)(128 / es), (cuuint32_t)(bw < 16 ? bw : 16), (cuuint32_t)(bw < 16 ? 16 / bw : 1), 1};
     if (tile_cols > 0) {   // prefetch map: the whole BH x BW x BLOCK_N output tile
         bx[0] = (cuuint32_t)tile_cols;
         bx[1] = (cuuint32_t)bw;
@@ -958,7 +976,7 @@ static int make_tmap_epi(CUtensorMap* m, const void* base, int f32, const GemmAr
     const CUtensorMapDataType dt = f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
                                        : (kOpFmt ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
     CUresult r = fn(m, dt, 4, const_cast<void*>(base), gd, gs, bx, est, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                    swz ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_NONE,
+                    swz ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
                     l2_256 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B : CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {

@@ -43,7 +43,7 @@ struct alignas(64) GemmMaps {
     CUtensorMap a[4];
     CUtensorMap b;
     // TMA epilogue (args.epi_tma): the output tensor [n_img][Ho][Wo][Cout] and the residual tensor of the same shape,
-    // 64-byte-swizzled boxes of 32 tile rows x 64 bytes (one epilogue warp's share of a pass)
+    // 128-byte-swizzled boxes of 16 tile rows x 128 bytes (one epilogue warp's pass)
     CUtensorMap out;
     CUtensorMap resid;
     CUtensorMap resid_pf;   // the residual tensor again, box = a whole output tile (L2 prefetch one tile ahead)
@@ -70,7 +70,7 @@ struct GemmArgs {
     float fin_b;
     int epi_tma;                   // 1: the epilogue moves residual and output tiles with TMA (EPI_NORMAL plans whose
                                    // residual, if any, has the output's element size); 0: per-thread global accesses
-    int epi_swz;                   // 1: the TMA epilogue's boxes are 64-byte swizzled (conflict-free row accesses)
+    int epi_swz;                   // 1: the TMA epilogue's boxes are 128-byte swizzled (conflict-free row accesses)
     int epi_pf;                    // 1: the TMA producer prefetches the next tile's residual rows into L2 (whole rows of
                                    // the tile in one request instead of 64-byte pieces fetched from DRAM one by one)
 };
