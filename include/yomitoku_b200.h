@@ -380,6 +380,38 @@ typedef struct {
     int x0, y0, x1, y1;   /* the model input is page[y0:y1, x0:x1]; 0 <= x0 < x1 <= W, 0 <= y0 < y1 <= H */
 } ytk_rtdetr_src;         /* 32 bytes */
 
+/* ---- Page tables: pages of any sizes back to back in one flat uint8 buffer, one record per page, the same record and
+ * rules as the RT-DETRv2 sources above.  A same-size [n, H0, W0, 3] buffer is the table {i * H0 * W0 * 3, H0, W0, 0, 0,
+ * W0, H0}.  The record is read as a page (its rectangle must be the whole page) by the detector and the pyramid, and
+ * as the page a crop record's `page` indexes by the crop extraction.  The records are host arrays (pageable: reusable
+ * as soon as the call returns); invalid records (a page beyond pages_bytes, an empty page, a rectangle outside its
+ * page or, where whole pages are read, not the whole page) are an error, not a launch.  At most 65535 pages a call. ---- */
+typedef ytk_rtdetr_src ytk_page;
+
+/* ytk_dbnet_forward_u8 for a page table: every page is resized to the network input of its own size, and all pages of
+ * one call must map to the same input (Hn, Wn) (an error names both shapes otherwise); prob_out [n_pages, Hn, Wn].
+ * pages: pages_bytes bytes on the device iff pages_on_device, else on the host. */
+int ytk_dbnet_forward_table_u8(ytk_dbnet* h, const uint8_t* pages, int pages_on_device, long long pages_bytes,
+                               const ytk_page* table, int n_pages, float* prob_out, int out_on_device,
+                               void* cuda_stream);
+/* op level, for the parity tests: the pre-processing of ytk_dbnet_forward_table_u8 alone, each page resized to
+ * (Hn, Wn) by the rule OpenCV picks for its own scales, into the canvas of ytk_op_dbnet_preprocess_u8.  The records are
+ * uploaded to a buffer allocated and freed on the stream. */
+int ytk_op_dbnet_preprocess_table_u8(const uint8_t* pages_dev, long long pages_bytes, const ytk_page* table, int n,
+                                     int Hn, int Wn, void* canvas_dev, void* cuda_stream);
+/* ytk_extract_crops_u8 for a page table: geoms[i].page indexes `table`, the ROI lies inside that page.  scratch_dev
+ * also holds the page table after the records (one upload), so scratch_bytes >= align16(max(roi_off + w*h*3)) +
+ * n_crops * sizeof(ytk_crop_geom) + n_pages * sizeof(ytk_page): the call allocates nothing. */
+int ytk_extract_crops_table_u8(const uint8_t* pages_dev, long long pages_bytes, const ytk_page* table, int n_pages,
+                               const ytk_crop_geom* geoms, int n_crops, uint8_t* scratch_dev, long long scratch_bytes,
+                               uint8_t* canvases_dev, long long canvases_bytes, void* cuda_stream);
+/* ytk_halve_pages_u8 for a page table: page i of src_table -> page i of dst_table, which must be
+ * cvRound(H / 2) x cvRound(W / 2).  scratch_dev holds the two uploaded tables: scratch_bytes >= 2 * n_pages *
+ * sizeof(ytk_page). */
+int ytk_halve_pages_table_u8(const uint8_t* src_dev, long long src_bytes, const ytk_page* src_table, int n_pages,
+                             uint8_t* dst_dev, long long dst_bytes, const ytk_page* dst_table, uint8_t* scratch_dev,
+                             long long scratch_bytes, void* cuda_stream);
+
 /* The reference's whole input path on the device: per record, the rectangle as RGB,
  * Image.fromarray(rgb_crop).resize((img, img), Image.BILINEAR) bit for bit (Pillow's fixed-point separable resample,
  * horizontal pass first) and ToTensor, then the forward of ytk_rtdetr_forward_f32 with the same outputs, ordering and

@@ -77,6 +77,8 @@ def _declare(lib):
     lib.ytk_op_dbnet_preprocess_u8.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
     lib.ytk_op_dbnet_preprocess_up_u8.restype = c_int
     lib.ytk_op_dbnet_preprocess_up_u8.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
+    lib.ytk_op_dbnet_preprocess_table_u8.restype = c_int
+    lib.ytk_op_dbnet_preprocess_table_u8.argtypes = [c_void_p, c_ll, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]
     lib.ytk_op_dbnet_stem_f16.restype = c_int
     lib.ytk_op_dbnet_stem_f16.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]
     lib.ytk_op_maxpool3x3s2_f16.restype = c_int
@@ -115,6 +117,9 @@ def _declare_dbnet(lib):
     lib.ytk_dbnet_input_size.argtypes = [c_void_p, c_int, c_int, P(c_int), P(c_int)]
     lib.ytk_dbnet_forward_u8.restype = c_int
     lib.ytk_dbnet_forward_u8.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p]
+    lib.ytk_dbnet_forward_table_u8.restype = c_int
+    lib.ytk_dbnet_forward_table_u8.argtypes = [c_void_p, c_void_p, c_int, c_ll, c_void_p, c_int, c_void_p, c_int,
+                                               c_void_p]
     lib.ytk_dbnet_forward_f32.restype = c_int
     lib.ytk_dbnet_forward_f32.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p]
     lib.ytk_dbnet_flops.restype = ctypes.c_double
@@ -170,6 +175,12 @@ def _declare_crops(lib):
                                          c_void_p]
     lib.ytk_halve_pages_u8.restype = c_int
     lib.ytk_halve_pages_u8.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p]
+    lib.ytk_extract_crops_table_u8.restype = c_int
+    lib.ytk_extract_crops_table_u8.argtypes = [c_void_p, c_ll, c_void_p, c_int, c_void_p, c_int, c_void_p, c_ll,
+                                               c_void_p, c_ll, c_void_p]
+    lib.ytk_halve_pages_table_u8.restype = c_int
+    lib.ytk_halve_pages_table_u8.argtypes = [c_void_p, c_ll, c_void_p, c_int, c_void_p, c_ll, c_void_p, c_void_p, c_ll,
+                                             c_void_p]
 
 
 class YtkRtdetrSrc(ctypes.Structure):

@@ -525,6 +525,37 @@ static void* stream_buffer(const void* host, size_t bytes, cudaStream_t st, cons
     return d;
 }
 
+// A page table: n records {page_off, H, W, rectangle} of pages back to back in `pages_bytes` bytes (ytk_page).  Records
+// come from the caller: a page beyond the buffer, an empty page or a rectangle outside its page is an error, and so is
+// a rectangle other than the whole page where the entry reads whole pages.
+static int check_page_table(const ytk_page* t, int n, long long pages_bytes, bool whole, const char* who) {
+    if (!t || n < 1 || n > 65535 || pages_bytes < 1) {
+        ytk::set_error("%s: %d page records for %lld page bytes (1..65535 records, a non-empty buffer)", who, n,
+                       pages_bytes);
+        return 1;
+    }
+    for (int i = 0; i < n; ++i) {
+        const ytk_page& p = t[i];
+        const bool ok = p.page_off >= 0 && p.H >= 1 && p.W >= 1 && p.page_off <= pages_bytes &&
+                        (long long)p.H * p.W <= (pages_bytes - p.page_off) / 3 && p.x0 >= 0 && p.x0 < p.x1 &&
+                        p.x1 <= p.W && p.y0 >= 0 && p.y0 < p.y1 && p.y1 <= p.H;
+        if (!ok) {
+            ytk::set_error("%s: page %d (at %lld, %dx%d, rectangle x %d..%d y %d..%d) is empty, has a rectangle outside "
+                           "it, or overruns the %lld page bytes", who, i, p.page_off, p.H, p.W, p.x0, p.x1, p.y0, p.y1,
+                           pages_bytes);
+            return 1;
+        }
+        if (whole && (p.x0 != 0 || p.y0 != 0 || p.x1 != p.W || p.y1 != p.H)) {
+            ytk::set_error("%s: page %d (%dx%d) has the rectangle x %d..%d y %d..%d; the detector reads whole pages", who,
+                           i, p.H, p.W, p.x0, p.x1, p.y0, p.y1);
+            return 1;
+        }
+    }
+    return 0;
+}
+
+static_assert(sizeof(ytk_page) == sizeof(ytk::RtSrc), "ytk_page and ytk::RtSrc must have one layout");
+
 // The two pre-processing entries: `up` = 0 takes the shapes OpenCV decimates with its area tables (no axis grows),
 // `up` = 1 the shapes it up-scales bilinearly (some axis grows).  One launcher serves both and picks by the same rule.
 static int op_dbnet_preprocess(const char* who, int up, const uint8_t* src_dev, int n, int H0, int W0, int Hn, int Wn,
@@ -565,6 +596,30 @@ int ytk_op_dbnet_preprocess_u8(const uint8_t* src_dev, int n, int H0, int W0, in
 int ytk_op_dbnet_preprocess_up_u8(const uint8_t* src_dev, int n, int H0, int W0, int Hn, int Wn, void* canvas_dev,
                                   void* cuda_stream) {
     return op_dbnet_preprocess("ytk_op_dbnet_preprocess_up_u8", 1, src_dev, n, H0, W0, Hn, Wn, canvas_dev, cuda_stream);
+}
+
+int ytk_op_dbnet_preprocess_table_u8(const uint8_t* pages_dev, long long pages_bytes, const ytk_page* table, int n,
+                                     int Hn, int Wn, void* canvas_dev, void* cuda_stream) {
+    const char* who = "ytk_op_dbnet_preprocess_table_u8";
+    if (!pages_dev || !canvas_dev) {
+        ytk::set_error("%s: null argument", who);
+        return YTK_ERR;
+    }
+    if (Hn < 1 || Wn < 1) {
+        ytk::set_error("%s: non-positive input size %dx%d", who, Hn, Wn);
+        return YTK_ERR;
+    }
+    if (check_page_table(table, n, pages_bytes, true, who)) return YTK_ERR;
+    if (misaligned(canvas_dev, 16)) {
+        ytk::set_error("%s: canvas_dev must be 16-byte aligned", who);
+        return YTK_ERR;
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    void* d = stream_buffer(table, (size_t)n * sizeof(ytk_page), st, who);
+    if (!d) return YTK_ERR;
+    const int rc = ytk::launch_preprocess_table(pages_dev, static_cast<const ytk::RtSrc*>(d), n, Hn, Wn, canvas_dev, st);
+    cudaFreeAsync(d, st);
+    return rc ? YTK_ERR : YTK_OK;
 }
 
 int ytk_op_dbnet_stem_f16(const void* canvas_dev, int n, int Hn, int Wn, const float* w_host, const float* bias_host,
@@ -818,6 +873,59 @@ int ytk_dbnet_forward_u8(ytk_dbnet* h, const uint8_t* pages, int pages_on_device
     return finish_forward(h, e, prob_out, out_on_device, st);
 }
 
+int ytk_dbnet_forward_table_u8(ytk_dbnet* h, const uint8_t* pages, int pages_on_device, long long pages_bytes,
+                               const ytk_page* table, int n_pages, float* prob_out, int out_on_device,
+                               void* cuda_stream) {
+    const char* who = "ytk_dbnet_forward_table_u8";
+    if (!h || !pages || !prob_out) {
+        ytk::set_error("%s: null argument", who);
+        return YTK_ERR;
+    }
+    if (check_page_table(table, n_pages, pages_bytes, true, who)) return YTK_ERR;
+    // one engine per call: every page must map to the same network input
+    int Hn, Wn;
+    ytk::dbnet_input_size(table[0].H, table[0].W, h->shortest, h->limit, &Hn, &Wn);
+    for (int i = 1; i < n_pages; ++i) {
+        int hn, wn;
+        ytk::dbnet_input_size(table[i].H, table[i].W, h->shortest, h->limit, &hn, &wn);
+        if (hn != Hn || wn != Wn) {
+            ytk::set_error("%s: page 0 (%dx%d) maps to the input %dx%d but page %d (%dx%d) to %dx%d; one call takes pages "
+                           "of one input size", who, table[0].H, table[0].W, Hn, Wn, i, table[i].H, table[i].W, hn, wn);
+            return YTK_ERR;
+        }
+    }
+    std::lock_guard<std::mutex> lk(h->mu);
+    DevGuard dev_guard(h->device);  // host threads start on device 0: the handle's device is the one that counts
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    ytk::DbnetEngine* e = get_engine(h, n_pages, Hn, Wn);
+    if (!e) return YTK_ERR;
+    // the staging buffer holds [host pages (16-byte aligned) |] the page table
+    const size_t page_bytes = pages_on_device ? 0 : (size_t)(pages_bytes + 15) / 16 * 16;
+    const size_t table_bytes = (size_t)n_pages * sizeof(ytk_page);
+    if (ensure_stage(h, page_bytes + table_bytes)) return YTK_ERR;
+    order_after_previous(h, st);
+    const uint8_t* src = pages;
+    uint8_t* stage = reinterpret_cast<uint8_t*>(h->stage);
+    if (!pages_on_device) {
+        if (cudaMemcpyAsync(stage, pages, (size_t)pages_bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) {
+            ytk::set_error("%s: H2D copy of pages failed", who);
+            return YTK_ERR;
+        }
+        src = stage;
+    }
+    // pageable records: the call returns after they are staged, so the caller may reuse them at once
+    if (cudaMemcpyAsync(stage + page_bytes, table, table_bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) {
+        ytk::set_error("%s: page table upload failed", who);
+        return YTK_ERR;
+    }
+    if (ytk::launch_preprocess_table(src, reinterpret_cast<const ytk::RtSrc*>(stage + page_bytes), n_pages, Hn, Wn,
+                                     e->input, st)) {
+        ytk::set_error("%s: preprocess launch failed", who);
+        return YTK_ERR;
+    }
+    return finish_forward(h, e, prob_out, out_on_device, st);
+}
+
 int ytk_dbnet_forward_f32(ytk_dbnet* h, const float* x, int x_on_device, int n, int H, int W, float* prob_out,
                           int out_on_device, void* cuda_stream) {
     std::lock_guard<std::mutex> lk(h->mu);
@@ -939,6 +1047,70 @@ int ytk_extract_crops_u8(const uint8_t* pages_dev, int n_pages, int H0, int W0, 
     return YTK_OK;
 }
 
+int ytk_extract_crops_table_u8(const uint8_t* pages_dev, long long pages_bytes, const ytk_page* table, int n_pages,
+                               const ytk_crop_geom* geoms, int n_crops, uint8_t* scratch_dev, long long scratch_bytes,
+                               uint8_t* canvases_dev, long long canvases_bytes, void* cuda_stream) {
+    const char* who = "ytk_extract_crops_table_u8";
+    if (n_crops == 0) return YTK_OK;
+    if (!pages_dev || !geoms || !scratch_dev || !canvases_dev || n_crops < 0) {
+        ytk::set_error("%s: null or empty argument", who);
+        return YTK_ERR;
+    }
+    if (check_page_table(table, n_pages, pages_bytes, false, who)) return YTK_ERR;
+    long long roi_end = 0;
+    for (int i = 0; i < n_crops; ++i) {
+        const ytk_crop_geom& g = geoms[i];
+        const long long sw = (g.rot & 1) ? g.h : g.w, sh = (g.rot & 1) ? g.w : g.h;
+        // the ROI lies inside the crop's own page
+        const bool in_page = g.page >= 0 && g.page < n_pages && (long long)g.x0 + g.rw <= table[g.page].W &&
+                             (long long)g.y0 + g.rh <= table[g.page].H;
+        const bool ok = in_page && g.x0 >= 0 && g.y0 >= 0 && g.rw >= 1 && g.rh >= 1 && g.w >= 1 && g.h >= 1 &&
+                        g.rot >= 0 && g.rot <= 3 && g.cw >= 1 && g.ch >= 1 && g.cw <= sw && g.ch <= sh &&
+                        g.cw <= g.canvas_w && g.ch <= g.canvas_h && g.roi_off >= 0 &&
+                        g.roi_off + (long long)g.w * g.h * 3 <= scratch_bytes && g.pix_off >= 0 &&
+                        g.pix_off + (long long)g.canvas_w * g.canvas_h * 3 <= canvases_bytes;
+        if (!ok) {
+            ytk::set_error("%s: inconsistent crop record %d (page %d of %d, roi %d,%d %dx%d, out %dx%d rot %d, content "
+                           "%dx%d, canvas %dx%d)", who, i, g.page, n_pages, g.x0, g.y0, g.rw, g.rh, g.w, g.h, g.rot, g.cw,
+                           g.ch, g.canvas_w, g.canvas_h);
+            return YTK_ERR;
+        }
+        roi_end = std::max(roi_end, g.roi_off + (long long)g.w * g.h * 3);
+    }
+    // records and page table are staged in the caller's scratch buffer, 16-byte aligned after the ROIs, with ONE copy
+    const long long rec_off = (roi_end + 15) / 16 * 16;
+    const long long rec_bytes = (long long)n_crops * (long long)sizeof(ytk::CropGeom);
+    const long long tab_bytes = (long long)n_pages * (long long)sizeof(ytk_page);
+    if (rec_off + rec_bytes + tab_bytes > scratch_bytes) {
+        ytk::set_error("%s: scratch_dev holds %lld bytes, need %lld (ROIs) + %lld (records) + %lld (page table)", who,
+                       scratch_bytes, rec_off, rec_bytes, tab_bytes);
+        return YTK_ERR;
+    }
+    cudaPointerAttributes attr;
+    if (cudaPointerGetAttributes(&attr, pages_dev) != cudaSuccess || attr.type != cudaMemoryTypeDevice) {
+        cudaGetLastError();
+        ytk::set_error("%s: pages_dev is not a device pointer", who);
+        return YTK_ERR;
+    }
+    DevGuard dev_guard(attr.device);
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    std::vector<uint8_t> blob((size_t)(rec_bytes + tab_bytes));
+    memcpy(blob.data(), geoms, (size_t)rec_bytes);
+    memcpy(blob.data() + rec_bytes, table, (size_t)tab_bytes);
+    cudaError_t err = cudaMemcpyAsync(scratch_dev + rec_off, blob.data(), blob.size(), cudaMemcpyHostToDevice, st);
+    if (err != cudaSuccess) {
+        ytk::set_error("%s: record upload failed: %s", who, cudaGetErrorString(err));
+        return YTK_ERR;
+    }
+    const ytk::CropGeom* dev = reinterpret_cast<const ytk::CropGeom*>(scratch_dev + rec_off);
+    const ytk::RtSrc* tab = reinterpret_cast<const ytk::RtSrc*>(scratch_dev + rec_off + rec_bytes);
+    if (ytk::launch_extract_crops_table(pages_dev, tab, dev, n_crops, scratch_dev, canvases_dev, st)) {
+        ytk::set_error("%s: kernel launch failed", who);
+        return YTK_ERR;
+    }
+    return YTK_OK;
+}
+
 int ytk_halve_pages_u8(const uint8_t* src_dev, int n_pages, int H, int W, uint8_t* dst_dev, int dH, int dW,
                        void* cuda_stream) {
     // cv2.resize(..., fx=0.5, fy=0.5): dsize = (cvRound(W * 0.5), cvRound(H * 0.5)), round half to even
@@ -957,6 +1129,56 @@ int ytk_halve_pages_u8(const uint8_t* src_dev, int n_pages, int H, int W, uint8_
     DevGuard dev_guard(attr.device);
     if (ytk::launch_halve_pages(src_dev, n_pages, H, W, dst_dev, dH, dW, static_cast<cudaStream_t>(cuda_stream))) {
         ytk::set_error("ytk_halve_pages_u8: kernel launch failed");
+        return YTK_ERR;
+    }
+    return YTK_OK;
+}
+
+int ytk_halve_pages_table_u8(const uint8_t* src_dev, long long src_bytes, const ytk_page* src_table, int n_pages,
+                             uint8_t* dst_dev, long long dst_bytes, const ytk_page* dst_table, uint8_t* scratch_dev,
+                             long long scratch_bytes, void* cuda_stream) {
+    const char* who = "ytk_halve_pages_table_u8";
+    if (!src_dev || !dst_dev || !scratch_dev) {
+        ytk::set_error("%s: null argument", who);
+        return YTK_ERR;
+    }
+    if (check_page_table(src_table, n_pages, src_bytes, true, who) ||
+        check_page_table(dst_table, n_pages, dst_bytes, true, who))
+        return YTK_ERR;
+    long long max_pixels = 0;
+    for (int i = 0; i < n_pages; ++i) {
+        const int eh = (int)nearbyint(src_table[i].H * 0.5), ew = (int)nearbyint(src_table[i].W * 0.5);
+        if (dst_table[i].H != eh || dst_table[i].W != ew) {
+            ytk::set_error("%s: page %d %dx%d -> %dx%d, expected %dx%d", who, i, src_table[i].H, src_table[i].W,
+                           dst_table[i].H, dst_table[i].W, eh, ew);
+            return YTK_ERR;
+        }
+        max_pixels = std::max(max_pixels, (long long)eh * ew);
+    }
+    const long long tab_bytes = (long long)n_pages * (long long)sizeof(ytk_page);
+    if (scratch_bytes < 2 * tab_bytes) {
+        ytk::set_error("%s: scratch_dev holds %lld bytes, need %lld (two page tables)", who, scratch_bytes, 2 * tab_bytes);
+        return YTK_ERR;
+    }
+    cudaPointerAttributes attr;
+    if (cudaPointerGetAttributes(&attr, src_dev) != cudaSuccess || attr.type != cudaMemoryTypeDevice) {
+        cudaGetLastError();
+        ytk::set_error("%s: src_dev is not a device pointer", who);
+        return YTK_ERR;
+    }
+    DevGuard dev_guard(attr.device);
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    std::vector<uint8_t> blob((size_t)(2 * tab_bytes));
+    memcpy(blob.data(), src_table, (size_t)tab_bytes);
+    memcpy(blob.data() + tab_bytes, dst_table, (size_t)tab_bytes);
+    cudaError_t err = cudaMemcpyAsync(scratch_dev, blob.data(), blob.size(), cudaMemcpyHostToDevice, st);
+    if (err != cudaSuccess) {
+        ytk::set_error("%s: page table upload failed: %s", who, cudaGetErrorString(err));
+        return YTK_ERR;
+    }
+    const ytk::RtSrc* tabs = reinterpret_cast<const ytk::RtSrc*>(scratch_dev);
+    if (ytk::launch_halve_pages_table(src_dev, tabs, n_pages, dst_dev, tabs + n_pages, max_pixels, st)) {
+        ytk::set_error("%s: kernel launch failed", who);
         return YTK_ERR;
     }
     return YTK_OK;

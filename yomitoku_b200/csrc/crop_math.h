@@ -91,12 +91,13 @@ YTK_HD void warp_coord(const double* M, int x, int y, int bw0, int* ix, int* iy,
 }
 
 // Rectified pixel (x, y) of crop g, written at its rotated position into the scratch ROI (RGB order: the reference
-// hands ParseqDataset the page as img[:, :, ::-1], data/dataset.py:69).  pages: [n][H0][W0][3] BGR.
-YTK_HD void warp_store(const CropGeom& g, const uint8_t* pages, int H0, int W0, int x, int y, uint8_t* scratch) {
+// hands ParseqDataset the page as img[:, :, ::-1], data/dataset.py:69).  page: the crop's own BGR page, rows of W0 * 3
+// bytes (g.page has already been resolved by the caller).
+YTK_HD void warp_store_page(const CropGeom& g, const uint8_t* page, int W0, int x, int y, uint8_t* scratch) {
     int ix, iy, ax, ay;
     warp_coord(g.minv, x, y, warp_block_width(g.w, g.h), &ix, &iy, &ax, &ay);
     const int w00 = (32 - ax) * (32 - ay), w01 = ax * (32 - ay), w10 = (32 - ax) * ay, w11 = ax * ay;
-    const uint8_t* base = pages + ((long long)g.page * H0 + g.y0) * (long long)W0 * 3 + (long long)g.x0 * 3;
+    const uint8_t* base = page + (long long)g.y0 * W0 * 3 + (long long)g.x0 * 3;
     const bool x0ok = ix >= 0 && ix < g.rw, x1ok = ix + 1 >= 0 && ix + 1 < g.rw;
     const bool y0ok = iy >= 0 && iy < g.rh, y1ok = iy + 1 >= 0 && iy + 1 < g.rh;
     const uint8_t* r0 = base + (long long)iy * W0 * 3 + (long long)ix * 3;
@@ -129,6 +130,11 @@ YTK_HD void warp_store(const CropGeom& g, const uint8_t* pages, int H0, int W0, 
     o[0] = (uint8_t)v[2];  // BGR page -> RGB crop
     o[1] = (uint8_t)v[1];
     o[2] = (uint8_t)v[0];
+}
+
+// The same for same-size pages: [n][H0][W0][3] BGR, crop g on page g.page.
+YTK_HD void warp_store(const CropGeom& g, const uint8_t* pages, int H0, int W0, int x, int y, uint8_t* scratch) {
+    warp_store_page(g, pages + (long long)g.page * H0 * W0 * 3, W0, x, y, scratch);
 }
 
 // Taps of one destination index along one axis of cv2.resize(INTER_AREA) (computeResizeAreaTab): an optional partial

@@ -5,6 +5,7 @@
 
 #include "gemm_tc.h"
 #include "ptx.cuh"
+#include "resample_math.h"
 
 namespace ytk {
 
@@ -23,9 +24,10 @@ __device__ __forceinline__ uint4 pack8(const float* f) {
 // BGR u8 page -> float -> cv2.resize(INTER_AREA) to (Hn, Wn) -> /255 -> (x - mean[c]) / std[c] applied positionally
 // to the B,G,R planes (SURVEY.md Appendix A2) -> network input.  Output layout: zero-padded NHWC with 8 channels,
 // pixel (h, w) at padded position (h + 3, w + 3) of a [Hn+6, Wn+8] canvas (the 7x7/stride-2 stem reads it through
-// overlapping TMA boxes, see dbnet_engine.cu).  One kernel body, templated on the resampler, which OpenCV picks by the
-// scales: AreaSampler (ResizeArea tables) when both axes shrink or keep their size, AreaUpSampler (bilinear with
-// "area-mode" coefficients) when some axis grows.  Both restate OpenCV's tables in fp32.
+// overlapping TMA boxes, see dbnet_engine.cu).  One kernel body; the resampler is the one OpenCV picks by the scales
+// of each page: AreaSampler (ResizeArea tables) when both axes shrink or keep their size, AreaUpSampler (bilinear with
+// "area-mode" coefficients) when some axis grows.  Both restate OpenCV's tables in fp32.  One page per blockIdx.y, so
+// the choice is uniform in a block even when the pages of a launch have different sizes (a page table).
 // ------------------------------------------------------------------------------------------------------------------
 struct AreaTap { int lo; int hi; float w_lo; float w_mid; float w_hi; };  // src indices [lo, hi], edge weights
 
@@ -55,12 +57,11 @@ __device__ __forceinline__ AreaTap area_tap(int d, double scale, int ssize) {
 
 // OpenCV's ResizeArea: pixel (h, w) of page img as fp32 B, G, R on the 0..255 scale
 struct AreaSampler {
-    __device__ __forceinline__ static void sample(const uint8_t* src, int img, int H0, int W0, int Hn, int Wn, int h,
-                                                  int w, float* acc) {
+    __device__ __forceinline__ static void sample(const uint8_t* base, int H0, int W0, int Hn, int Wn, int h, int w,
+                                                  float* acc) {
         const double sy = (double)H0 / Hn, sx = (double)W0 / Wn;
         const AreaTap ty = area_tap(h, sy, H0), tx = area_tap(w, sx, W0);
         acc[0] = acc[1] = acc[2] = 0.f;
-        const uint8_t* base = src + (size_t)img * H0 * W0 * 3;
         for (int y = ty.lo; y <= ty.hi; ++y) {
             const float wy = (y == ty.lo && ty.w_lo > 0.f) ? ty.w_lo : ((y == ty.hi && ty.w_hi > 0.f) ? ty.w_hi : ty.w_mid);
             float row[3] = {0.f, 0.f, 0.f};
@@ -103,10 +104,9 @@ __device__ __forceinline__ UpTap area_up_tap(int d, int ssize, int dsize) {
 
 // OpenCV's INTER_AREA up-scaling: a horizontal pass over two source rows, then a vertical one, in fp32
 struct AreaUpSampler {
-    __device__ __forceinline__ static void sample(const uint8_t* src, int img, int H0, int W0, int Hn, int Wn, int h,
-                                                  int w, float* acc) {
+    __device__ __forceinline__ static void sample(const uint8_t* base, int H0, int W0, int Hn, int Wn, int h, int w,
+                                                  float* acc) {
         const UpTap ty = area_up_tap(h, H0, Hn), tx = area_up_tap(w, W0, Wn);
-        const uint8_t* base = src + (size_t)img * H0 * W0 * 3;
         const uint8_t* r0 = base + (size_t)ty.s0 * W0 * 3;
         const uint8_t* r1 = base + (size_t)ty.s1 * W0 * 3;
         const float ax = 1.f - tx.f, ay = 1.f - ty.f;
@@ -119,41 +119,57 @@ struct AreaUpSampler {
     }
 };
 
-template <class Sampler>
-__global__ void preprocess_kernel(const uint8_t* __restrict__ src, int n_img, int H0, int W0, int Hn, int Wn,
-                                  op_t* __restrict__ dst) {
+// Page img of the launch: from the page table when there is one, else page img of a same-size [n][H0][W0][3] batch.
+__global__ void preprocess_kernel(const uint8_t* __restrict__ src, const RtSrc* __restrict__ table, int H0, int W0,
+                                  int Hn, int Wn, op_t* __restrict__ dst) {
     const int Hp = Hn + 6, Wp = Wn + 8;
-    const long long total = (long long)n_img * Hp * Wp;
-    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= total) return;
-    const int wp = (int)(idx % Wp);
-    const int hp = (int)((idx / Wp) % Hp);
-    const int img = (int)(idx / ((long long)Wp * Hp));
+    const int img = blockIdx.y;
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= Hp * Wp) return;
+    const uint8_t* page = src + (size_t)img * H0 * W0 * 3;
+    int H = H0, W = W0;
+    if (table) {
+        const RtSrc p = table[img];
+        page = src + p.page_off;
+        H = p.H;
+        W = p.W;
+    }
+    const int wp = idx % Wp;
+    const int hp = idx / Wp;
     float o[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     const int h = hp - 3, w = wp - 3;
     if (h >= 0 && h < Hn && w >= 0 && w < Wn) {
         float acc[3];
-        Sampler::sample(src, img, H0, W0, Hn, Wn, h, w, acc);
+        // OpenCV's rule: true area resampling only when neither axis grows
+        if (Hn <= H && Wn <= W)
+            AreaSampler::sample(page, H, W, Hn, Wn, h, w, acc);
+        else
+            AreaUpSampler::sample(page, H, W, Hn, Wn, h, w, acc);
         // channel order seen by the network is B,G,R with the ImageNet RGB mean/std applied positionally
         const float mean[3] = {0.485f, 0.456f, 0.406f}, stdv[3] = {0.229f, 0.224f, 0.225f};
 #pragma unroll
         for (int c = 0; c < 3; ++c) o[c] = (float)(((double)acc[c] / 255.0 - (double)mean[c]) / (double)stdv[c]);
     }
-    reinterpret_cast<uint4*>(dst)[idx] = pack8(o);
+    reinterpret_cast<uint4*>(dst)[(size_t)img * Hp * Wp + idx] = pack8(o);
+}
+
+static int preprocess(const uint8_t* src, const RtSrc* table, int n_img, int H0, int W0, int Hn, int Wn, void* dst,
+                      cudaStream_t st) {
+    if (n_img < 1 || n_img > 65535) return 1;  // one page per blockIdx.y
+    const int threads = 256;
+    const dim3 grid((unsigned)(((long long)(Hn + 6) * (Wn + 8) + threads - 1) / threads), (unsigned)n_img);
+    preprocess_kernel<<<grid, threads, 0, st>>>(src, table, H0, W0, Hn, Wn, reinterpret_cast<op_t*>(dst));
+    count_launch();
+    return cudaGetLastError() != cudaSuccess;
 }
 
 int launch_preprocess(const uint8_t* src, int n_img, int H0, int W0, int Hn, int Wn, void* dst, cudaStream_t st) {
-    const long long total = (long long)n_img * (Hn + 6) * (Wn + 8);
-    const int threads = 256;
-    const unsigned blocks = (unsigned)((total + threads - 1) / threads);
-    op_t* out = reinterpret_cast<op_t*>(dst);
-    // OpenCV's rule: true area resampling only when neither axis grows
-    if (Hn <= H0 && Wn <= W0)
-        preprocess_kernel<AreaSampler><<<blocks, threads, 0, st>>>(src, n_img, H0, W0, Hn, Wn, out);
-    else
-        preprocess_kernel<AreaUpSampler><<<blocks, threads, 0, st>>>(src, n_img, H0, W0, Hn, Wn, out);
-    count_launch();
-    return cudaGetLastError() != cudaSuccess;
+    return preprocess(src, nullptr, n_img, H0, W0, Hn, Wn, dst, st);
+}
+
+int launch_preprocess_table(const uint8_t* pages, const RtSrc* table_dev, int n_img, int Hn, int Wn, void* dst,
+                            cudaStream_t st) {
+    return preprocess(pages, table_dev, n_img, 0, 0, Hn, Wn, dst, st);
 }
 
 // Model-level seam: the reference hands DBNet a normalised (N,3,H,W) fp32 tensor (text_detector.py:127-129).  Repack

@@ -125,6 +125,23 @@ def crop_to_tensor(crop_u8):
 
 
 # ------------------------------------------------------------------------------------------ device-side crop extraction
+# Layout of ytk_page / ytk_rtdetr_src (include/yomitoku_b200.h): one page of a flat buffer and a rectangle of it.
+PAGE_DTYPE = np.dtype([("page_off", "<i8"), ("H", "<i4"), ("W", "<i4"), ("x0", "<i4"), ("y0", "<i4"), ("x1", "<i4"),
+                       ("y1", "<i4")])
+
+
+def page_table(shapes):
+    """Pages of the given (h, w) shapes back to back in one flat BGR uint8 buffer: (PAGE_DTYPE records covering each
+    whole page, total bytes).  Same-size pages give the byte layout of their (n, h, w, 3) stack."""
+    hw = np.asarray([(int(s[0]), int(s[1])) for s in shapes], np.int64).reshape(-1, 2)
+    size = hw[:, 0] * hw[:, 1] * 3
+    t = np.zeros(len(hw), PAGE_DTYPE)
+    t["page_off"] = np.cumsum(size) - size
+    t["H"] = t["y1"] = hw[:, 0]
+    t["W"] = t["x1"] = hw[:, 1]
+    return t, int(size.sum())
+
+
 # Layout of ytk_crop_geom (include/yomitoku_b200.h) / ytk::CropGeom (csrc/crop_math.h).
 CROP_GEOM_DTYPE = np.dtype([
     ("minv", "<f8", (9,)), ("roi_off", "<i8"), ("pix_off", "<i8"), ("page", "<i4"), ("x0", "<i4"), ("y0", "<i4"),

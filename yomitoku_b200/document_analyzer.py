@@ -443,7 +443,7 @@ class DocumentAnalyzer:
 
     # -------------------------------------------------------------------------------------- many pages
     def analyze_pages(self, pages, layouts=None):
-        """Batched multi-page form (SURVEY.md section 8f row 3): `pages` = list of same-size BGR pages.  Detection and
+        """Batched multi-page form (SURVEY.md section 8f row 3): `pages` = list of BGR pages, of one size or of many.  Detection and
         recognition of ALL pages run through `pipeline.BatchedOCR` (detector batches, one packed recognizer call,
         host post-processing in the process pool) while the layout analyzer works through the pages in a thread pool;
         then `aggregate` per page.  `layouts` (optional list of LayoutAnalyzerSchema) replaces the layout analyzer.

@@ -97,30 +97,72 @@ class _DeviceModel:
         return m
 
 
-def extract_crops_device(pages_dev, geoms, stream=None):
-    """Device-side crop extraction (C ABI ytk_extract_crops_u8, csrc/crop_ops.cu).
+def uniform_pages(flat, table):
+    """(n, H, W, 3) view of the flat uint8 tensor `flat` when the page table (data.PAGE_DTYPE records) describes
+    same-size pages back to back - a stacked batch, from its first page's offset on - else None."""
+    n = len(table)
+    if n == 0:
+        return None
+    H, W, off0 = int(table["H"][0]), int(table["W"][0]), int(table["page_off"][0])
+    nb = H * W * 3
+    if not (np.all(table["H"] == H) and np.all(table["W"] == W)
+            and np.array_equal(table["page_off"], off0 + nb * np.arange(n, dtype=np.int64))):
+        return None
+    return flat[off0:off0 + n * nb].view(n, H, W, 3)
 
-    pages_dev: (n, H0, W0, 3) uint8 BGR cuda tensor; geoms: CROP_GEOM_DTYPE records (data.crop_geometry) - their
-    roi_off / pix_off are (re)assigned here, crops packed back to back in record order.  Returns (canvases, total
-    bytes): a flat uint8 cuda tensor holding every crop's (canvas_h, canvas_w, 3) RGB canvas at geoms["pix_off"], ready
-    for PARSeq.run_packed_ptr(..., on_device=1).  Asynchronous on `stream` (default: the current stream)."""
+
+def device_pages(flat, table):
+    """The pages of a batch in the form the device calls below take: the (n, H, W, 3) view of a same-size batch, else
+    the (flat buffer, page table) pair."""
+    v = uniform_pages(flat, table)
+    return v if v is not None else (flat, np.ascontiguousarray(table))
+
+
+def _check_table_pages(who, pages):
+    from .data import PAGE_DTYPE
+    flat, table = pages
+    if not (isinstance(flat, torch.Tensor) and flat.is_cuda and flat.dtype == torch.uint8 and flat.dim() == 1
+            and flat.is_contiguous()):
+        raise ValueError("%s: the page buffer must be a contiguous flat uint8 cuda tensor" % who)
+    if not (isinstance(table, np.ndarray) and table.dtype == PAGE_DTYPE and table.flags.c_contiguous):
+        raise ValueError("%s: the page table must be a contiguous PAGE_DTYPE array" % who)
+    return flat, table
+
+
+def extract_crops_device(pages_dev, geoms, stream=None):
+    """Device-side crop extraction (C ABI ytk_extract_crops_u8 / ytk_extract_crops_table_u8, csrc/crop_ops.cu).
+
+    pages_dev: (n, H0, W0, 3) uint8 BGR cuda tensor, or a (flat uint8 cuda tensor, page table) pair for pages of
+    different sizes (`device_pages`; geoms["page"] indexes the table); geoms: CROP_GEOM_DTYPE records
+    (data.crop_geometry) - their roi_off / pix_off are (re)assigned here, crops packed back to back in record order.
+    Returns (canvases, total bytes): a flat uint8 cuda tensor holding every crop's (canvas_h, canvas_w, 3) RGB canvas at
+    geoms["pix_off"], ready for PARSeq.run_packed_ptr(..., on_device=1).  Asynchronous on `stream` (default: the
+    current stream)."""
     from .data import CROP_GEOM_DTYPE, layout_crop_buffers
-    if not (isinstance(pages_dev, torch.Tensor) and pages_dev.is_cuda and pages_dev.dtype == torch.uint8
-            and pages_dev.dim() == 4 and pages_dev.shape[3] == 3 and pages_dev.is_contiguous()):
+    table = None
+    if isinstance(pages_dev, tuple):
+        pages_dev, table = _check_table_pages("extract_crops_device", pages_dev)
+    elif not (isinstance(pages_dev, torch.Tensor) and pages_dev.is_cuda and pages_dev.dtype == torch.uint8
+              and pages_dev.dim() == 4 and pages_dev.shape[3] == 3 and pages_dev.is_contiguous()):
         raise ValueError("extract_crops_device: pages_dev must be a contiguous (n, H, W, 3) uint8 cuda tensor")
     if not (isinstance(geoms, np.ndarray) and geoms.dtype == CROP_GEOM_DTYPE and geoms.flags.c_contiguous):
         raise ValueError("extract_crops_device: geoms must be a contiguous CROP_GEOM_DTYPE array")
     scratch_bytes, total = layout_crop_buffers(geoms)      # writes roi_off / pix_off into the caller's records
     ctx = torch.cuda.stream(stream) if stream is not None else torch.cuda.device(pages_dev.device)
-    # scratch = ROIs + (16-byte aligned) the device copy of the records (include/yomitoku_b200.h)
-    scratch_bytes = (scratch_bytes + 15) // 16 * 16 + geoms.nbytes
+    # scratch = ROIs + (16-byte aligned) the device copy of the records [+ the page table] (include/yomitoku_b200.h)
+    scratch_bytes = (scratch_bytes + 15) // 16 * 16 + geoms.nbytes + (0 if table is None else table.nbytes)
     with ctx:
         scratch = torch.empty(max(scratch_bytes, 1), dtype=torch.uint8, device=pages_dev.device)
         canv = torch.empty(max(total, 1), dtype=torch.uint8, device=pages_dev.device)
-    n, H0, W0, _ = pages_dev.shape
-    _lib.check(_lib.lib().ytk_extract_crops_u8(pages_dev.data_ptr(), n, H0, W0, geoms.ctypes.data, len(geoms),
-                                               scratch.data_ptr(), scratch_bytes, canv.data_ptr(), total,
-                                               _stream_ptr(stream)))
+    if table is None:
+        n, H0, W0, _ = pages_dev.shape
+        _lib.check(_lib.lib().ytk_extract_crops_u8(pages_dev.data_ptr(), n, H0, W0, geoms.ctypes.data, len(geoms),
+                                                   scratch.data_ptr(), scratch_bytes, canv.data_ptr(), total,
+                                                   _stream_ptr(stream)))
+    else:
+        _lib.check(_lib.lib().ytk_extract_crops_table_u8(pages_dev.data_ptr(), pages_dev.numel(), table.ctypes.data,
+                                                         len(table), geoms.ctypes.data, len(geoms), scratch.data_ptr(),
+                                                         scratch_bytes, canv.data_ptr(), total, _stream_ptr(stream)))
     if stream is not None:
         # the scratch buffer is only read by the canvas kernel queued on `stream`: hand it back to the allocator in
         # stream order
@@ -182,7 +224,26 @@ def dbnet_post_front(prob_dev, thresh, stream=None, max_runs=32768):
 
 def halve_pages_device(pages_dev, stream=None):
     """One level of the source_downscale pyramid on the GPU (C ABI ytk_halve_pages_u8): (n, H, W, 3) uint8 cuda tensor ->
-    (n, cvRound(H / 2), cvRound(W / 2), 3), equal to cv2.resize(page, None, fx=0.5, fy=0.5, INTER_AREA) per page."""
+    (n, cvRound(H / 2), cvRound(W / 2), 3), equal to cv2.resize(page, None, fx=0.5, fy=0.5, INTER_AREA) per page.  A
+    (flat buffer, page table) pair gives a new pair: the halved pages back to back with their own table
+    (ytk_halve_pages_table_u8)."""
+    if isinstance(pages_dev, tuple):
+        from .data import page_table
+        flat, table = _check_table_pages("halve_pages_device", pages_dev)
+        shapes = [(int(np.rint(h * 0.5)), int(np.rint(w * 0.5))) for h, w in zip(table["H"], table["W"])]
+        if min(min(hw) for hw in shapes) < 1:
+            raise ValueError("halve_pages_device: a page of the table cannot be halved")
+        dst_table, total = page_table(shapes)
+        ctx = torch.cuda.stream(stream) if stream is not None else torch.cuda.device(flat.device)
+        with ctx:
+            out = torch.empty(total, dtype=torch.uint8, device=flat.device)
+            scratch = torch.empty(2 * table.nbytes, dtype=torch.uint8, device=flat.device)
+        _lib.check(_lib.lib().ytk_halve_pages_table_u8(flat.data_ptr(), flat.numel(), table.ctypes.data, len(table),
+                                                       out.data_ptr(), total, dst_table.ctypes.data,
+                                                       scratch.data_ptr(), scratch.numel(), _stream_ptr(stream)))
+        if stream is not None:
+            scratch.record_stream(stream)
+        return out, dst_table
     n, H, W, _ = pages_dev.shape
     dH, dW = int(np.rint(H * 0.5)), int(np.rint(W * 0.5))      # round half to even, like cvRound
     if dH < 1 or dW < 1:
@@ -196,7 +257,7 @@ def halve_pages_device(pages_dev, stream=None):
 
 def extract_crops_pyramid(pages, geoms, levels, stream=None):
     """`extract_crops_device` for records that live on different pyramid levels (source_downscale).  pages: dict
-    level -> (n, H_k, W_k, 3) cuda tensor; missing levels are built on demand by halving the level below (the dict is
+    level -> (n, H_k, W_k, 3) cuda tensor or (flat buffer, page table) pair; missing levels are built on demand by halving the level below (the dict is
     filled in place).  geoms / levels: records in packing order and their levels.  Returns (canvases, total bytes,
     pix_off): one flat buffer, and every record's canvas offset in it (one extraction per level, back to back)."""
     levels = np.asarray(levels, np.int64)
@@ -371,6 +432,29 @@ class DBNet(_DeviceModel):
                               pin_memory=(not t.is_cuda) and torch.cuda.is_available())
         _lib.check(_lib.lib().ytk_dbnet_forward_u8(h, t.data_ptr(), 1 if t.is_cuda else 0, n, H0, W0, out.data_ptr(),
                                                    1 if out.is_cuda else 0, _stream_ptr(stream)))
+        return out
+
+    def detect_pages_table(self, flat, table, out=None, stream=None):
+        """Pages of any sizes that share one network input: `flat` a flat uint8 tensor (host or cuda) holding the pages
+        at the offsets of `table` (data.PAGE_DTYPE records, whole pages) -> (n, Hn, Wn) fp32 probability maps, each page
+        pre-processed exactly as `detect_pages_u8` does it alone.  Pages laid out as a same-size stack take
+        `detect_pages_u8` itself; otherwise ytk_dbnet_forward_table_u8 reads only the span of `flat` the table covers."""
+        same = uniform_pages(flat, table)
+        if same is not None:
+            return self.detect_pages_u8(same, out=out, stream=stream)
+        h = self._ensure()
+        Hn, Wn = self.input_size(int(table["H"][0]), int(table["W"][0]))
+        n = len(table)
+        if out is None:
+            out = torch.empty((n, Hn, Wn), dtype=torch.float32, device=flat.device,
+                              pin_memory=(not flat.is_cuda) and torch.cuda.is_available())
+        lo = int(table["page_off"].min())
+        hi = int((table["page_off"] + table["H"].astype(np.int64) * table["W"] * 3).max())
+        rel = np.array(table, copy=True)
+        rel["page_off"] -= lo
+        _lib.check(_lib.lib().ytk_dbnet_forward_table_u8(h, flat.data_ptr() + lo, 1 if flat.is_cuda else 0, hi - lo,
+                                                         rel.ctypes.data, n, out.data_ptr(), 1 if out.is_cuda else 0,
+                                                         _stream_ptr(stream)))
         return out
 
     def flops(self, n, Hn, Wn):

@@ -2,21 +2,22 @@
 (SURVEY.md section 0: "there is no multi-page or multi-GPU batching in the reference").
 
     ocr = BatchedOCR(TextDetector(...), TextRecognizer(...), workers=16)
-    results = ocr(pages)            # list of BGR pages of one size -> list of OCRSchema
+    results = ocr(pages)            # list of BGR pages, of any sizes -> list of OCRSchema
 
-Per page the results are what `OCR.__call__` (reference ocr.py:51-63) returns: detection runs for a whole batch of
-pages in one device launch sequence, the host stages the reference also has (contours/unclip, crop extraction:
-SURVEY.md R3/R4) fan out over a process pool, and ALL crops of ALL pages go to the recognizer as one packed ragged
-call in which every crop keeps the padded width and mini-batch group its own page would have given it - so per-page
-outputs do not depend on how many pages are batched.
+Per page the results are what `OCR.__call__` (reference ocr.py:51-63) returns: the pages of a batch sit back to back in
+one buffer described by a page table (data.page_table), detection runs in one device launch sequence per group of pages
+that share a detector input size (in chunks of `det_batch`; a same-size batch is one group), the host stages the
+reference also has (contours/unclip, crop extraction: SURVEY.md R3/R4) fan out over a process pool, and ALL crops of ALL
+pages go to the recognizer as one packed ragged call in which every crop keeps the padded width and mini-batch group its
+own page would have given it - so per-page outputs do not depend on how many pages are batched, or of which sizes.
 """
 import os
 from concurrent.futures import ProcessPoolExecutor
 
 import numpy as np
 
-from .data import CROP_GEOM_DTYPE, ParseqDataset, crop_records
-from .models import dbnet_post_front
+from .data import CROP_GEOM_DTYPE, ParseqDataset, crop_records, page_table
+from .models import dbnet_post_front, device_pages
 from .postprocessor import DBnetPostProcessor
 from .schemas import OCRSchema
 from .text_recognizer import plan_mini_batches
@@ -43,6 +44,44 @@ class _span:
             import threading
             import time
             TRACE.append((self.name, threading.current_thread().name, self.t0, time.perf_counter()))
+
+
+class BatchPlan:
+    """Layout and detector plan of one batch, pages in submission order.
+      table / page_bytes  the pages back to back in one flat uint8 buffer (data.page_table)
+      inputs              detector input size (Hn, Wn) per page
+      chunks              detector calls: (Hn, Wn, page indices), grouped by input size in order of first appearance,
+                          at most det_batch pages each, pages in submission order inside a group
+      prob_off / prob_len float offset of each page's probability map in the map buffer (maps in chunk order, so every
+                          chunk's maps are contiguous) and the buffer's length in floats
+    A same-size batch is one group: its chunks, offsets and byte layout are those of the (n, H, W, 3) stack."""
+
+    def __init__(self, shapes, input_size, det_batch):
+        self.shapes = [(int(s[0]), int(s[1])) for s in shapes]
+        self.table, self.page_bytes = page_table(self.shapes)
+        self.inputs = [tuple(int(v) for v in input_size(h, w)) for h, w in self.shapes]
+        groups = {}
+        for i, hw in enumerate(self.inputs):
+            groups.setdefault(hw, []).append(i)
+        self.chunks = [(hn, wn, idx[s:s + det_batch]) for (hn, wn), idx in groups.items()
+                       for s in range(0, len(idx), det_batch)]
+        self.prob_off = [0] * len(self.shapes)
+        off = 0
+        for hn, wn, idx in self.chunks:
+            for i in idx:
+                self.prob_off[i] = off
+                off += hn * wn
+        self.prob_len = off
+
+    def prob_map(self, buf, i):
+        """Page i's (Hn, Wn) map in a flat map buffer (numpy array or tensor)."""
+        hn, wn = self.inputs[i]
+        return buf[self.prob_off[i]:self.prob_off[i] + hn * wn].reshape(hn, wn)
+
+    def chunk_maps(self, buf, chunk):
+        hn, wn, idx = chunk
+        o = self.prob_off[idx[0]]
+        return buf[o:o + len(idx) * hn * wn].reshape(len(idx), hn, wn)
 
 
 class _SharedBuf:
@@ -295,44 +334,52 @@ class BatchedOCR:
 
     # ------------------------------------------------------------------------------------------ stages
     def _shared(self, kind, nbytes):
-        """Shared + page-locked staging buffer of the current ring slot (pages, probability maps or crop arena)."""
-        key = (kind, int(nbytes))
-        ring = self._prob_ring.setdefault(key, {})
-        if self._slot not in ring:
-            ring[self._slot] = _SharedBuf(nbytes)
-        return ring[self._slot]
+        """Shared + page-locked staging buffer of the current ring slot (pages, probability maps or crop arena).  One
+        buffer per (kind, slot), sized by capacity: it is reused while it is large enough and replaced by a larger one
+        otherwise (the slot's previous batch is finished by then, see `submit`), so batches with different byte totals
+        do not accumulate /dev/shm files and page-locked registrations."""
+        ring = self._prob_ring.setdefault(kind, {})
+        buf = ring.get(self._slot)
+        if buf is None or buf.nbytes < nbytes:
+            if buf is not None:
+                buf.close()
+            buf = ring[self._slot] = _SharedBuf(max(int(nbytes), 1))
+        return buf
 
     def _stage(self, pages, shared):
-        """Host staging of a batch of same-size pages: (stage (n,H,W,3) u8 tensor, out (n,Hn,Wn) f32 tensor).  With
+        """Host staging of a batch: (stage flat u8 tensor holding the pages back to back, out flat f32 tensor for the
+        probability maps, BatchPlan).  For same-size pages the stage is byte for byte their (n, H, W, 3) stack.  With
         `shared` both live in the shared page-locked ring - the H2D/D2H copies are plain DMAs and the workers read both
         without a copy; `self._last_shared` then holds the two buffers."""
         import torch
-        n = len(pages)
-        h0, w0 = pages[0].shape[:2]
-        hn, wn = self.detector.model.input_size(h0, w0)
+        plan = BatchPlan([p.shape[:2] for p in pages], self.detector.model.input_size, self.det_batch)
         self._last_shared = None
         if shared:
-            pb = self._shared("pages", n * h0 * w0 * 3)
-            ob = self._shared("prob", n * hn * wn * 4)
-            sn = pb.view(0, (n, h0, w0, 3), np.uint8)
+            pb = self._shared("pages", plan.page_bytes)
+            ob = self._shared("prob", plan.prob_len * 4)
             with _span("detect.stage_pages"):
-                for i, p in enumerate(pages):
-                    np.copyto(sn[i], p)
-            stage = pb.torch.view(n, h0, w0, 3)
-            out = ob.torch.view(torch.float32).view(n, hn, wn)
+                for (h, w), off, p in zip(plan.shapes, plan.table["page_off"], pages):
+                    np.copyto(pb.view(int(off), (h, w, 3), np.uint8), p)
+            stage = pb.torch[:plan.page_bytes]
+            out = ob.torch[:plan.prob_len * 4].view(torch.float32)
             self._last_shared = (pb, ob)
         else:
-            stage = torch.from_numpy(np.stack([np.ascontiguousarray(p) for p in pages]))
-            out = torch.empty((n, hn, wn), dtype=torch.float32)
-        return stage, out
+            stage = torch.from_numpy(np.concatenate([np.ascontiguousarray(p).reshape(-1) for p in pages]))
+            out = torch.empty(plan.prob_len, dtype=torch.float32)
+        return stage, out, plan
+
+    def _detect_chunk(self, stage, plan, chunk, maps, stream=None):
+        """One detector call: the chunk's pages of the flat stage (host or device) -> maps (n, Hn, Wn)."""
+        self.detector.model.detect_pages_table(stage, plan.table[chunk[2]], out=maps, stream=stream)
 
     def detect_prob(self, pages, shared=False, stream=None):
-        """Device stage 1: probability maps (n, Hn, Wn) float32 on the host for same-size pages."""
-        stage, out = self._stage(pages, shared)
-        for s in range(0, len(pages), self.det_batch):
-            e = min(len(pages), s + self.det_batch)
-            self.detector.model.detect_pages_u8(stage[s:e], out=out[s:e], stream=stream)
-        return out.numpy()
+        """Device stage 1: probability maps float32 on the host, per page in submission order (an (n, Hn, Wn) array when
+        all pages share the detector input size)."""
+        stage, out, plan = self._stage(pages, shared)
+        for ch in plan.chunks:
+            self._detect_chunk(stage, plan, ch, plan.chunk_maps(out, ch), stream)
+        maps = [plan.prob_map(out.numpy(), i) for i in range(len(pages))]
+        return np.stack(maps) if len(set(plan.inputs)) == 1 else maps
 
     def _run_groups_local(self, groups, stream=None):
         """groups: list of (canvases, padded_widths).  One packed device call per <= max_tokens chunk (chunks end on
@@ -517,7 +564,7 @@ class BatchedOCR:
                 assert total_d == total
                 parts.append((canv_d, total_d))
             some = next(iter(pages.values()))
-            device = getattr(some, "device", "cpu")
+            device = getattr(some[0] if isinstance(some, tuple) else some, "device", "cpu")
             if parts:
                 canv = concat_device_buffers(parts, stream)
                 if len(parts) == 1:
@@ -840,11 +887,10 @@ class BatchedOCR:
                         self._slot = self._ring
                         self._ring += 1
         n = len(pages)
-        stage, out = self._stage(pages, shared=pool is not None)
+        stage, out, plan = self._stage(pages, shared=pool is not None)
         prob = out.numpy()
         sh = self._last_shared if pool is not None else None
         arena, cap = None, self.crop_cap
-        h0, w0 = pages[0].shape[:2]
         pages_dev = None
         if self.device_crops or getattr(self.recognizer, "rec_orientation_fallback", False):
             # (the orientation fallback's second look is implemented on the device-crops path only: its crops are the
@@ -866,49 +912,55 @@ class BatchedOCR:
         if dev_post:
             import torch
             out_dev = torch.empty(out.shape, dtype=torch.float32, device=pages_dev.device)
-        futs = []
-        # detection in chunks of det_batch pages; a chunk's host jobs start while the next chunk is on the device
-        for s in range(0, n, self.det_batch):
-            e = min(n, s + self.det_batch)
+        futs = [None] * n       # submission order, whatever order the detector groups run in
+        # detection per chunk of pages that share a detector input size (plan.chunks); a chunk's host jobs start while
+        # the next chunk is on the device
+        for ch in plan.chunks:
+            hn, wn, idx = ch
+            maps = plan.chunk_maps(out_dev if dev_post else out, ch)
             with _span("submit.detect"):
-                self.detector.model.detect_pages_u8((stage if pages_dev is None else pages_dev)[s:e],
-                                                    out=(out_dev if dev_post else out)[s:e], stream=stream)
-            runs = [None] * (e - s)
+                self._detect_chunk(stage if pages_dev is None else pages_dev, plan, ch, maps, stream)
+            runs = [None] * len(idx)
             if dev_post:
                 with _span("submit.post_front"):
                     if prob_override is not None:      # benchmarks with random detector weights: replace the maps
-                        for i in range(s, e):
-                            self._override_prob(out_dev[i], prob_override[i], stream)
-                    runs, _ = dbnet_post_front(out_dev[s:e], self.detector.post_processor.thresh, stream)
+                        for j, i in enumerate(idx):
+                            self._override_prob(maps[j], prob_override[i], stream)
+                    runs, _ = dbnet_post_front(maps, self.detector.post_processor.thresh, stream)
                     self.post_front_pages += sum(r is not None for r in runs)
                     self.post_host_pages += sum(r is None for r in runs)
-                    self.post_d2h_bytes += 16 * (e - s) + sum(r.nbytes for r in runs if r is not None)
-                    for i in range(s, e):
-                        if runs[i - s] is None:
-                            out[i].copy_(out_dev[i])      # pageable or pinned host row; synchronous
-                            self.post_d2h_bytes += out[i].numel() * 4
+                    self.post_d2h_bytes += 16 * len(idx) + sum(r.nbytes for r in runs if r is not None)
+                    for j, i in enumerate(idx):
+                        if runs[j] is None:
+                            plan.prob_map(out, i).copy_(maps[j])      # pageable or pinned host map; synchronous
+                            self.post_d2h_bytes += hn * wn * 4
             else:
-                self.post_d2h_bytes += out[s:e].numel() * 4
-            for i in range(s, e):
+                self.post_d2h_bytes += maps.numel() * 4
+            for j, i in enumerate(idx):
+                h0, w0 = plan.shapes[i]
+                pm = plan.prob_map(prob, i)
                 qo = None if quads_override is None else quads_override[i]
-                if runs[i - s] is not None:
-                    job = (("shape", h0, w0), _Runs(runs[i - s], out.shape[1], out.shape[2]), qo, None, "geom")
+                if runs[j] is not None:
+                    job = (("shape", h0, w0), _Runs(runs[j], hn, wn), qo, None, "geom")
                 elif sh is None:
-                    job = (pages[i], prob[i] if (prob_override is None or dev_post) else prob_override[i], qo)
+                    job = (pages[i], pm if (prob_override is None or dev_post) else prob_override[i], qo)
                     if pages_dev is not None:
                         job = (("shape", h0, w0), job[1], qo, None, "geom")
                 elif pages_dev is not None:
                     if prob_override is not None and not dev_post:
-                        np.copyto(prob[i], prob_override[i])
-                    job = (("shape", h0, w0), ob.desc(i * prob[i].nbytes, prob[i].shape, np.float32), qo, None, "geom")
+                        np.copyto(pm, prob_override[i])
+                    job = (("shape", h0, w0), ob.desc(plan.prob_off[i] * 4, pm.shape, np.float32), qo, None, "geom")
                 else:
                     if prob_override is not None:   # benchmarks with random detector weights: overwrite the D2H result
-                        np.copyto(prob[i], prob_override[i])
+                        np.copyto(pm, prob_override[i])
                     # descriptors only: the workers map the three buffers themselves
-                    job = (pb.desc(i * h0 * w0 * 3, (h0, w0, 3), np.uint8),
-                           ob.desc(i * prob[i].nbytes, prob[i].shape, np.float32), qo,
+                    job = (pb.desc(int(plan.table["page_off"][i]), (h0, w0, 3), np.uint8),
+                           ob.desc(plan.prob_off[i] * 4, pm.shape, np.float32), qo,
                            arena.desc(i * cap, (cap,), np.uint8))
-                futs.append(_Done(_host_stage(job)) if pool is None else pool.submit(_host_stage, job))
+                futs[i] = _Done(_host_stage(job)) if pool is None else pool.submit(_host_stage, job)
+        if pages_dev is not None:
+            # what the crop kernels read: the (n, H, W, 3) view of a same-size batch, else (flat buffer, page table)
+            pages_dev = device_pages(pages_dev, plan.table)
         if pool is None:
             return _Handle(futs, None, 0, pages_dev)
         handle = _Handle(futs, arena, cap, pages_dev)
@@ -927,7 +979,7 @@ class BatchedOCR:
             dst.copy_(t, non_blocking=True)
 
     def _upload_pages(self, stage, stream=None):
-        """(n, H0, W0, 3) uint8 staging tensor -> the same pages in HBM of the detector's device (asynchronous on
+        """Flat uint8 staging tensor (the pages back to back) -> the same bytes in HBM of the detector's device (asynchronous on
         `stream`)."""
         import torch
         dev = self.detector.model.cuda_device() if hasattr(self.detector.model, "cuda_device") else "cuda"
@@ -1096,7 +1148,7 @@ class BatchedOCR:
         return _stream_impl(self, batches, lookahead, prob_override, quads_override)
 
     def __call__(self, pages, prob_override=None, quads_override=None):
-        """pages: list of same-size BGR uint8 arrays.  prob_override / quads_override (benchmarks with random
+        """pages: list of BGR uint8 arrays, of one size or of many.  prob_override / quads_override (benchmarks with random
         detector weights): the detector still runs, but post-processing sees the given probability maps / the
         recognizer the given quads."""
         return self.collect(self.submit(pages, prob_override, quads_override))

@@ -67,19 +67,19 @@ class TextDetector(BaseModule):
         return self.post_processor(preds, image_size)
 
     def postprocess_device(self, prob_dev, image_size, stream=None):
-        """prob_dev: (n, Hn, Wn) fp32 cuda probability maps of same-size pages -> per page (quads, scores), equal to
-        `postprocess` of the downloaded maps."""
+        """prob_dev: (n, Hn, Wn) fp32 cuda probability maps -> per page (quads, scores), equal to `postprocess` of the
+        downloaded maps.  image_size: the (h, w) of every page, or a list with one (h, w) per page."""
         from .models import dbnet_post_front
         pp = self.post_processor
         runs, _ = dbnet_post_front(prob_dev, pp.thresh, stream)
         hn, wn = prob_dev.shape[1:]
-        height, width = image_size
+        sizes = image_size if isinstance(image_size, list) else [image_size] * len(runs)
         out = []
-        for i, r in enumerate(runs):
+        for i, (r, size) in enumerate(zip(runs, sizes)):
             if r is None:
-                out.append(self.postprocess({"binary": prob_dev[i:i + 1, None].cpu().numpy()}, image_size))
+                out.append(self.postprocess({"binary": prob_dev[i:i + 1, None].cpu().numpy()}, size))
             else:
-                out.append(pp.boxes_from_runs(r, wn, hn, width, height))
+                out.append(pp.boxes_from_runs(r, wn, hn, size[1], size[0]))
         return out
 
     def _detect_device(self, pages_u8):
@@ -111,17 +111,26 @@ class TextDetector(BaseModule):
         return results, vis
 
     def detect_pages(self, pages):
-        """Batched entry (new surface, SURVEY.md section 0): list of same-size BGR pages -> list of
-        TextDetectorSchema.  One device launch sequence for the whole batch, host post-processing per page."""
-        arr = np.stack([np.ascontiguousarray(p) for p in pages])
+        """Batched entry (new surface, SURVEY.md section 0): list of BGR pages, of one size or of many -> list of
+        TextDetectorSchema.  The pages go to the device back to back with a page table (data.page_table); one device
+        launch sequence per group of pages that share a detector input size (a same-size batch is one group), host
+        post-processing per page."""
+        from .pipeline import BatchPlan
+        plan = BatchPlan([p.shape[:2] for p in pages], self.model.input_size, max(1, len(pages)))
+        flat = torch.from_numpy(np.concatenate([np.ascontiguousarray(p).reshape(-1) for p in pages]))
         if self.device_post:
-            return [TextDetectorSchema(points=q, scores=s) for q, s in self._detect_device(arr)]
-        prob = self.model.detect_pages_u8(arr)
-        prob = prob.cpu().numpy() if prob.is_cuda else prob.numpy()
-        out = []
-        for i, p in enumerate(pages):
-            quads, scores = self.postprocess({"binary": prob[i:i + 1, None]}, p.shape[:2])
-            out.append(TextDetectorSchema(points=quads, scores=scores))
+            flat = flat.to(self.model.cuda_device(), non_blocking=False)
+        out = [None] * len(pages)
+        for ch in plan.chunks:
+            idx = ch[2]
+            prob = self.model.detect_pages_table(flat, plan.table[idx])
+            if self.device_post:
+                res = self.postprocess_device(prob, [plan.shapes[i] for i in idx])
+            else:
+                prob = prob.cpu().numpy() if prob.is_cuda else prob.numpy()
+                res = [self.postprocess({"binary": prob[j:j + 1, None]}, plan.shapes[i]) for j, i in enumerate(idx)]
+            for i, (quads, scores) in zip(idx, res):
+                out[i] = TextDetectorSchema(points=quads, scores=scores)
         return out
 
 
