@@ -148,7 +148,8 @@ int ytk_dbnet_device(const ytk_dbnet* h);
 int ytk_dbnet_input_size(const ytk_dbnet* h, int H0, int W0, int* Hn, int* Wn);
 /* pages: [n_pages, H0, W0, 3] uint8 BGR (caller-owned; device pointer iff pages_on_device, else host - pinned for
  * async copies), any size: the resize to (Hn, Wn) is cv2.resize(INTER_AREA) whether the page shrinks or grows.
- * prob_out: [n_pages, Hn, Wn] fp32 sigmoid map = preds["binary"][:, 0] of the reference. */
+ * prob_out: [n_pages, Hn, Wn] fp32 sigmoid map = preds["binary"][:, 0] of the reference.  The same as
+ * ytk_dbnet_forward_table_u8 (below) with the table of n_pages evenly spaced whole pages. */
 int ytk_dbnet_forward_u8(ytk_dbnet* h, const uint8_t* pages, int pages_on_device, int n_pages, int H0, int W0,
                          float* prob_out, int out_on_device, void* cuda_stream);
 /* model-level seam: x = normalised (n,3,H,W) fp32 exactly as the reference feeds DBNet.forward; H, W % 32 == 0 */
@@ -283,12 +284,12 @@ int ytk_op_apply_rep_cut(const int* rep_cut, int B, int S, int C, int eos_id, in
  * are NHWC fp16 on the device, 16-byte aligned; weights are the reference's fp32 layouts on the host, packed by the
  * code the engine's loader uses (with no BatchNorm: the bias is the whole shift).  Asynchronous on the stream (weights
  * and scratch go to buffers allocated and freed on it); invalid arguments are an error, not a launch.
- *   preprocess  n BGR u8 pages [n, H0, W0, 3] -> the stem's canvas [n, Hn+6, Wn+8, 8], all of it written: pixel (h, w)
- *               at (h+3, w+3), channels 0..2 = cv2.resize(INTER_AREA) / 255 with the mean / std applied by position
- *               to B, G, R, zero border and zero channels 3..7.  Hn <= H0 and Wn <= W0 (OpenCV's area decimation).
- *   preprocess_up  the same for the shapes where some axis grows (Hn > H0 or Wn > W0), which OpenCV's INTER_AREA
- *               resamples bilinearly on both axes with its "area-mode" coefficients.
- *   stem        7x7 / stride 2 / pad 3 conv (w [64][3][7][7], bias [64]) + ReLU over that canvas -> out
+ *   preprocess  (ytk_op_dbnet_preprocess_table_u8, declared with the page tables below) n BGR u8 pages -> the stem's
+ *               canvas [n, Hn+6, Wn+8, 8], all of it written: pixel (h, w) at (h+3, w+3), channels 0..2 =
+ *               cv2.resize(INTER_AREA) / 255 with the mean / std applied by position to B, G, R, zero border and zero
+ *               channels 3..7.  Each page gets the rule OpenCV picks for its own scales: area decimation when no axis
+ *               grows, else bilinear resampling on both axes with INTER_AREA's "area-mode" coefficients.
+ *   stem       7x7 / stride 2 / pad 3 conv (w [64][3][7][7], bias [64]) + ReLU over that canvas -> out
  *               [n, Hn/2, Wn/2, 64]; Hn and Wn multiples of 32.
  *   maxpool     max_pool2d(3, 2, 1): in [n, H, W, C] -> out [n, (H+1)/2, (W+1)/2, C]; C a multiple of 8.
  *   upsample    bilinear, align_corners=False: src [n, Hs, Ws, C] -> channels [coff, coff+C) of dst [n, Hd, Wd, ldd],
@@ -298,10 +299,6 @@ int ytk_op_apply_rep_cut(const int* rep_cut, int B, int S, int C, int eos_id, in
  *               (device, or NULL): gvec [n, 64] = the channel gate, m [n, H, W] fp32 = the channel-mean map.
  *   head        ConvT(64->64, 2, 2) + ReLU, then ConvT(64->1, 2, 2) + sigmoid in one GEMM epilogue: x [n, H, W, 64]
  *               -> prob [n, 4H, 4W] fp32 (8-byte aligned); w1 [64][64][2][2], b1 [64], w2 [64][1][2][2], b2. */
-int ytk_op_dbnet_preprocess_u8(const uint8_t* src_dev, int n, int H0, int W0, int Hn, int Wn, void* canvas_dev,
-                               void* cuda_stream);
-int ytk_op_dbnet_preprocess_up_u8(const uint8_t* src_dev, int n, int H0, int W0, int Hn, int Wn, void* canvas_dev,
-                                  void* cuda_stream);
 int ytk_op_dbnet_stem_f16(const void* canvas_dev, int n, int Hn, int Wn, const float* w_host, const float* bias_host,
                           void* out_dev, void* cuda_stream);
 int ytk_op_maxpool3x3s2_f16(const void* in, int n, int H, int W, int C, void* out, void* cuda_stream);
@@ -324,7 +321,7 @@ typedef struct {
     double minv[9];    /* cv2.invert(cv2.getPerspectiveTransform(quad - (x0,y0), [[0,0],[w,0],[w,h],[0,h]])), row major */
     long long roi_off; /* byte offset of this crop's rectified ROI in scratch_dev: w*h*3 bytes */
     long long pix_off; /* byte offset of this crop's canvas in canvases_dev: canvas_h*canvas_w*3 bytes, RGB */
-    int page;          /* index into pages_dev */
+    int page;          /* index into the page table */
     int x0, y0, rw, rh; /* bounding-box slice of the (int64-truncated) quad inside the page */
     int w, h;          /* rectified size: (int |p0p1|, int |p1p2|) */
     int rot;           /* bit 0: rotate 90 degrees counter-clockwise after the warp (h > 2w); bit 1: then rotate by 180
@@ -332,23 +329,8 @@ typedef struct {
     int cw, ch;        /* content size after the down-scale-only fit (calc_resize_without_padding) */
     int canvas_w, canvas_h;
 } ytk_crop_geom;
-
-/* pages_dev: [n_pages, H0, W0, 3] uint8 BGR in device memory (e.g. the buffer handed to ytk_dbnet_forward_u8 with
- * pages_on_device = 1); geoms: host array (pageable: may be reused as soon as the call returns; page-locked: must stay
- * valid until the stream has passed the call); scratch_dev / canvases_dev: caller-owned device buffers.  scratch_dev
- * holds the rectified ROIs (at roi_off) and, 16-byte aligned after the last ROI, a copy of the n_crops records, so
- * scratch_bytes >= align16(max(roi_off + w*h*3)) + n_crops * sizeof(ytk_crop_geom): the call allocates nothing.
- * Asynchronous on cuda_stream: one H2D copy of the records + two kernel launches. */
-int ytk_extract_crops_u8(const uint8_t* pages_dev, int n_pages, int H0, int W0, const ytk_crop_geom* geoms, int n_crops,
-                         uint8_t* scratch_dev, long long scratch_bytes, uint8_t* canvases_dev, long long canvases_bytes,
-                         void* cuda_stream);
-
-/* One level of the recognizer's source_downscale pyramid (reference data/dataset.py:64-86):
- * cv2.resize(page, None, fx=0.5, fy=0.5, interpolation=cv2.INTER_AREA) for n_pages pages [n, H, W, 3] uint8 in device
- * memory, bit-exact with OpenCV 4.13 (2x2 cells round half up; the clipped last column / row of an odd size averages
- * the pixels that exist).  dH = cvRound(H / 2), dW = cvRound(W / 2) (round half to even) - anything else is rejected. */
-int ytk_halve_pages_u8(const uint8_t* src_dev, int n_pages, int H, int W, uint8_t* dst_dev, int dH, int dW,
-                       void* cuda_stream);
+/* The crop extraction and the source_downscale pyramid read their pages through a page table: see
+ * ytk_extract_crops_table_u8 and ytk_halve_pages_table_u8 below. */
 
 /* ---- RT-DETRv2 layout parser / table structure recognizer / table cell detector: replaces `self.model(img_tensor)` in
  * reference LayoutParser.__call__ (src/yomitoku/layout_parser.py:258-262 -> models/rtdetr.py:17-22),
@@ -388,26 +370,31 @@ typedef struct {
  * page or, where whole pages are read, not the whole page) are an error, not a launch.  At most 65535 pages a call. ---- */
 typedef ytk_rtdetr_src ytk_page;
 
-/* ytk_dbnet_forward_u8 for a page table: every page is resized to the network input of its own size, and all pages of
- * one call must map to the same input (Hn, Wn) (an error names both shapes otherwise); prob_out [n_pages, Hn, Wn].
- * pages: pages_bytes bytes on the device iff pages_on_device, else on the host. */
+/* The DBNet forward of u8 pages: every page is resized to the network input of its own size as ytk_dbnet_forward_u8
+ * describes, and all pages of one call must map to the same input (Hn, Wn) (an error names both shapes otherwise);
+ * prob_out [n_pages, Hn, Wn].  pages: pages_bytes bytes on the device iff pages_on_device, else on the host. */
 int ytk_dbnet_forward_table_u8(ytk_dbnet* h, const uint8_t* pages, int pages_on_device, long long pages_bytes,
                                const ytk_page* table, int n_pages, float* prob_out, int out_on_device,
                                void* cuda_stream);
-/* op level, for the parity tests: the pre-processing of ytk_dbnet_forward_table_u8 alone, each page resized to
- * (Hn, Wn) by the rule OpenCV picks for its own scales, into the canvas of ytk_op_dbnet_preprocess_u8.  The records are
- * uploaded to a buffer allocated and freed on the stream. */
+/* op level, for the parity tests: the pre-processing of ytk_dbnet_forward_table_u8 alone (the DBNet op "preprocess"
+ * above), each page resized to (Hn, Wn).  The records are uploaded to a buffer allocated and freed on the stream. */
 int ytk_op_dbnet_preprocess_table_u8(const uint8_t* pages_dev, long long pages_bytes, const ytk_page* table, int n,
                                      int Hn, int Wn, void* canvas_dev, void* cuda_stream);
-/* ytk_extract_crops_u8 for a page table: geoms[i].page indexes `table`, the ROI lies inside that page.  scratch_dev
- * also holds the page table after the records (one upload), so scratch_bytes >= align16(max(roi_off + w*h*3)) +
- * n_crops * sizeof(ytk_crop_geom) + n_pages * sizeof(ytk_page): the call allocates nothing. */
+/* The crop extraction: geoms[i].page indexes `table`, the ROI lies inside that page.  pages_dev: the pages in device
+ * memory (e.g. the buffer handed to ytk_dbnet_forward_table_u8 with pages_on_device = 1); geoms: host array (pageable:
+ * may be reused as soon as the call returns; page-locked: must stay valid until the stream has passed the call);
+ * scratch_dev / canvases_dev: caller-owned device buffers.  scratch_dev holds the rectified ROIs (at roi_off) and,
+ * 16-byte aligned after the last ROI, a copy of the n_crops records followed by the page table (one upload), so
+ * scratch_bytes >= align16(max(roi_off + w*h*3)) + n_crops * sizeof(ytk_crop_geom) + n_pages * sizeof(ytk_page): the
+ * call allocates nothing.  Asynchronous on cuda_stream: one H2D copy + two kernel launches. */
 int ytk_extract_crops_table_u8(const uint8_t* pages_dev, long long pages_bytes, const ytk_page* table, int n_pages,
                                const ytk_crop_geom* geoms, int n_crops, uint8_t* scratch_dev, long long scratch_bytes,
                                uint8_t* canvases_dev, long long canvases_bytes, void* cuda_stream);
-/* ytk_halve_pages_u8 for a page table: page i of src_table -> page i of dst_table, which must be
- * cvRound(H / 2) x cvRound(W / 2).  scratch_dev holds the two uploaded tables: scratch_bytes >= 2 * n_pages *
- * sizeof(ytk_page). */
+/* One level of the recognizer's source_downscale pyramid (reference data/dataset.py:64-86): page i of src_table ->
+ * page i of dst_table = cv2.resize(page, None, fx=0.5, fy=0.5, interpolation=cv2.INTER_AREA), bit-exact with OpenCV
+ * 4.13 (2x2 cells round half up; the clipped last column / row of an odd size averages the pixels that exist).  The
+ * destination page must be cvRound(H / 2) x cvRound(W / 2) (round half to even) - anything else is rejected.
+ * scratch_dev holds the two uploaded tables: scratch_bytes >= 2 * n_pages * sizeof(ytk_page). */
 int ytk_halve_pages_table_u8(const uint8_t* src_dev, long long src_bytes, const ytk_page* src_table, int n_pages,
                              uint8_t* dst_dev, long long dst_bytes, const ytk_page* dst_table, uint8_t* scratch_dev,
                              long long scratch_bytes, void* cuda_stream);

@@ -15,12 +15,14 @@ extern "C" {
 
 int crop_host_geom_size(void) { return (int)sizeof(ytk::CropGeom); }
 
-// Whole row R4 for n crops: warp (+ rotation) into scratch, then area resize + paste into the canvases.
+// Whole row R4 for n crops of same-size pages [n_pages][H0][W0][3]: warp (+ rotation) into scratch, then area resize +
+// paste into the canvases.
 void crop_host_extract(const uint8_t* pages, int H0, int W0, const ytk::CropGeom* g, int n, uint8_t* scratch,
                        uint8_t* canvases) {
     for (int i = 0; i < n; ++i) {
+        const uint8_t* page = pages + (long long)g[i].page * H0 * W0 * 3;
         for (int y = 0; y < g[i].h; ++y)
-            for (int x = 0; x < g[i].w; ++x) ytk::warp_store(g[i], pages, H0, W0, x, y, scratch);
+            for (int x = 0; x < g[i].w; ++x) ytk::warp_store_page(g[i], page, W0, x, y, scratch);
         for (int cy = 0; cy < g[i].canvas_h; ++cy)
             for (int cx = 0; cx < g[i].canvas_w; ++cx) ytk::canvas_store(g[i], scratch, cx, cy, canvases);
     }

@@ -34,7 +34,7 @@ def main():
     rec.model.run_packed_ptr = lambda ptr, on_device, total, descs, n, n_groups, stream=None: \
         fake_run_packed(None, total, descs, n, n_groups)
     ocr = BatchedOCR(det, rec, det_batch=8, workers=W)
-    det.model.detect_pages_u8 = lambda *a, **k: None      # no GPU here: the maps come from prob_override
+    det.model.detect_pages_table = lambda *a, **k: None      # no GPU here: the maps come from prob_override
     det.model.input_size = lambda h, w: (Hn, Wn)
     for _ in range(4):
         h = ocr.submit(pages, prob_override=probs)

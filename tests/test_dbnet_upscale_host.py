@@ -1,4 +1,5 @@
-"""CPU: the detector's resize for pages that grow to the detector input, and the refusals of its op-level entry.
+"""CPU: the detector's resize for pages that grow to the detector input, and the refusals of the op-level
+pre-processing entry on such pages.
 
 OpenCV's cv2.resize(INTER_AREA) uses its area tables only when no axis grows.  When some axis grows it resamples BOTH
 axes bilinearly with "area-mode" coefficients; per axis, for destination index d, source size s, destination size n:
@@ -20,6 +21,7 @@ import numpy as np
 import pytest
 import scipy.sparse as sp
 
+from test_op_entries_host import preprocess_table
 from yomitoku_b200 import _lib, build
 from yomitoku_b200.data import shortest_edge_size
 
@@ -109,33 +111,18 @@ def lib():
     return _lib.lib()
 
 
-def _up(lib, src=P, n=1, H0=900, W0=1200, Hn=1184, Wn=1600, canvas=P):
-    return lib.ytk_op_dbnet_preprocess_up_u8(src, n, H0, W0, Hn, Wn, canvas, None)
-
-
 @pytest.mark.parametrize("kwargs,fragment", [
-    (dict(src=None), b"ytk_op_dbnet_preprocess_up_u8: null argument"), (dict(canvas=None), b"null argument"),
-    (dict(n=0), b"non-positive size (n 0, page 900x1200, input 1184x1600)"), (dict(H0=0), b"non-positive size"),
-    (dict(W0=-1), b"non-positive size"), (dict(Hn=0), b"non-positive size"), (dict(Wn=-32), b"non-positive size"),
-    # pure decimation, and the same size on both axes: the area entry's shapes
-    (dict(H0=1200, W0=1600), b"1200x1600 -> 1184x1600 grows no axis; INTER_AREA decimation is "
-                             b"ytk_op_dbnet_preprocess_u8"),
-    (dict(H0=1184, W0=1600), b"1184x1600 -> 1184x1600 grows no axis"),
+    (dict(src=None), b"ytk_op_dbnet_preprocess_table_u8: null argument"), (dict(canvas=None), b"null argument"),
+    (dict(n=0), b"0 page records"), (dict(n=65536), b"65536 page records"), (dict(table=False), b"page records"),
+    (dict(H0=0), b"page 0 (at 0, 0x1200"), (dict(W0=-1), b"page 0 (at 0, 900x-1"),
+    (dict(Hn=0), b"non-positive input size 0x1600"), (dict(Wn=-32), b"non-positive input size 1184x-32"),
     (dict(canvas=P + 8), b"canvas_dev must be 16-byte aligned"),
 ])
-def test_preprocess_up_refusals(lib, kwargs, fragment):
+def test_preprocess_table_up_refusals(lib, kwargs, fragment):
+    """The pre-processing entry on pages that grow to the detector input (900x1200 -> 1184x1600)."""
     before = lib.ytk_launch_count()
-    status = _up(lib, **kwargs)
+    status = preprocess_table(lib, **dict(dict(H0=900, W0=1200), **kwargs))
     assert status != 0
     msg = lib.ytk_last_error()
     assert fragment in msg, msg
-    assert lib.ytk_launch_count() == before
-
-
-def test_area_entry_names_the_up_entry(lib):
-    """ytk_op_dbnet_preprocess_u8 keeps refusing an up-scale, and says which entry takes it."""
-    before = lib.ytk_launch_count()
-    assert lib.ytk_op_dbnet_preprocess_u8(P, 1, 900, 1200, 1184, 1600, P, None) != 0
-    msg = lib.ytk_last_error()
-    assert b"900x1200 -> 1184x1600 is an upscale" in msg and b"ytk_op_dbnet_preprocess_up_u8" in msg, msg
     assert lib.ytk_launch_count() == before

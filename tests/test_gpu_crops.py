@@ -1,4 +1,4 @@
-"""GPU: the device-side crop extraction (csrc/crop_ops.cu behind ytk_extract_crops_u8) - bit-exact against the crops the
+"""GPU: the device-side crop extraction (csrc/crop_ops.cu behind ytk_extract_crops_table_u8) - bit-exact against the crops the
 reference's own data/functions.py cut (tests/golden/crops_ref.npz), against OpenCV through the host mirror
 (yomitoku_b200.data.ParseqDataset), against the same arithmetic compiled for the host (oracle/crop_host.cpp), and end
 to end: BatchedOCR / TextRecognizer with device_crops must return exactly what the host-crop path returns."""

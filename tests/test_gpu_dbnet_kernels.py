@@ -2,7 +2,7 @@
 the kernel reads (fp16-rounded activations and packed weights, fp32 where the kernel reads fp32).  u = 2^-24 is the fp32
 unit roundoff; rounding a value y to fp16 costs at most 2^-11 |y| + 2^-25.
 
-  pre-processing  ytk_op_dbnet_preprocess_u8 (preprocess_kernel) vs OpenCV's INTER_AREA tables (computeResizeAreaTab
+  pre-processing  ytk_op_dbnet_preprocess_table_u8 (preprocess_kernel) vs OpenCV's INTER_AREA tables (computeResizeAreaTab
                   with its 1e-3 sliver rule) applied in float64 as two separable matrices, / 255, mean / std by position.
                   The device value must be fp16(r) for some r within e of the reference: equal to fp16(reference)
                   except where the reference lies within e of a rounding boundary of fp16.  e = 2 ((nx + ny + 4) u / 0.224
@@ -58,6 +58,7 @@ import torch.nn.functional as F
 from oracle import pipeline as opipe
 from oracle import weights
 from yomitoku_b200 import _lib
+from yomitoku_b200.data import page_table
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -163,18 +164,25 @@ PREP_CASES = [(hw, None, ("random",)) for hw in PREP_PAGES[:4]] + [
 ]
 
 
+def preprocess_pages(pages, Hn, Wn, canvas):
+    """ytk_op_dbnet_preprocess_table_u8 on same-size pages [n, H0, W0, 3] u8 (evenly spaced in the table) -> canvas"""
+    src = torch.from_numpy(np.ascontiguousarray(pages)).to(DEV)
+    table, total = page_table([pages.shape[1:3]] * len(pages))
+    _lib.check(_lib.lib().ytk_op_dbnet_preprocess_table_u8(_fp(src), total, table.ctypes.data, len(pages), Hn, Wn,
+                                                           _fp(canvas), None))
+    torch.cuda.synchronize()
+
+
 @pytest.mark.parametrize("hw,size,kinds", PREP_CASES, ids=["%dx%d-%s" % (h, w, "-".join(k)) for (h, w), _, k in
                                                          PREP_CASES])
-def test_preprocess_vs_float64(hw, size, kinds):
+def test_preprocess_table_vs_float64(hw, size, kinds):
     H0, W0 = hw
     Hn, Wn = size if size else opipe.detector_input_size(H0, W0)
     n = len(kinds)
     pages = np.stack([_page(k, H0, W0, seed=H0 * 7 + W0 + i) for i, k in enumerate(kinds)])
     # one canvas more than the call writes, everything NaN: the border ring and channels 3..7 must come back 0
     canvas = torch.full((n + 1, Hn + 6, Wn + 8, 8), float("nan"), dtype=torch.float16, device=DEV)
-    src = torch.from_numpy(pages).to(DEV)
-    _lib.check(_lib.lib().ytk_op_dbnet_preprocess_u8(_fp(src), n, H0, W0, Hn, Wn, _fp(canvas), None))
-    torch.cuda.synchronize()
+    preprocess_pages(pages, Hn, Wn, canvas)
     out = canvas.cpu().numpy()
     assert np.isnan(out[n]).all()                                 # nothing past the n canvases
     inner = np.zeros(out.shape[:3], dtype=bool)

@@ -1,6 +1,6 @@
 """GPU: pages that grow to the detector input, from the op up to the public API.
 
-  op level   ytk_op_dbnet_preprocess_up_u8 (preprocess_kernel<AreaUpSampler>) vs OpenCV's up-scaling tables of
+  op level   ytk_op_dbnet_preprocess_table_u8 (preprocess_kernel, AreaUpSampler) vs OpenCV's up-scaling tables of
              cv2.resize(INTER_AREA) (tests/test_dbnet_upscale_host.py: up_matrix, equal to cv2 within 1e-4 on the 0..255
              scale) applied in float64 as two separable matrices, / 255, mean / std by position.  The device value must
              be fp16(r) for some r within e of the reference.  Derivation of e (u = 2^-24): the kernel's weights (1 - f,
@@ -24,8 +24,6 @@
   API        BatchedOCR (__call__ with and without device crops, stream) and DocumentAnalyzer.analyze_pages accept
              900x1200 and 720x1280 pages and equal the one-page calls.
 """
-import ctypes
-
 import cv2
 import numpy as np
 import pytest
@@ -34,8 +32,8 @@ import torch
 from oracle import parseq as ops
 from oracle import weights
 from test_dbnet_upscale_host import SHAPE_IDS, SHAPES, TRAPS, same_tables, up_resize
-from test_gpu_dbnet_kernels import U, _fp16_match, _normalise, _page
-from yomitoku_b200 import OCR, DocumentAnalyzer, TextDetector, _lib
+from test_gpu_dbnet_kernels import U, _fp16_match, _normalise, _page, preprocess_pages
+from yomitoku_b200 import OCR, DocumentAnalyzer, TextDetector
 from yomitoku_b200.pipeline import BatchedOCR
 from yomitoku_b200.synth import synthetic_page, synthetic_prob_map
 
@@ -44,17 +42,10 @@ DEV = "cuda:0"
 SMALL = [(900, 1200), (720, 1280)]
 
 
-def _fp(t):
-    return ctypes.c_void_p(t.data_ptr())
-
-
 def _canvas_up(pages, Hn, Wn):
     """the op's canvases for pages [n, H0, W0, 3] u8, plus one NaN canvas past them -> numpy fp16 [n + 1, ...]"""
-    n, H0, W0, _ = pages.shape
-    canvas = torch.full((n + 1, Hn + 6, Wn + 8, 8), float("nan"), dtype=torch.float16, device=DEV)
-    src = torch.from_numpy(np.ascontiguousarray(pages)).to(DEV)
-    _lib.check(_lib.lib().ytk_op_dbnet_preprocess_up_u8(_fp(src), n, H0, W0, Hn, Wn, _fp(canvas), None))
-    torch.cuda.synchronize()
+    canvas = torch.full((len(pages) + 1, Hn + 6, Wn + 8, 8), float("nan"), dtype=torch.float16, device=DEV)
+    preprocess_pages(pages, Hn, Wn, canvas)
     return canvas.cpu().numpy()
 
 
@@ -65,7 +56,7 @@ def _e(ref):
 # ======================================================================================================== op level
 @pytest.mark.parametrize("n", [1, 3])
 @pytest.mark.parametrize("hw,size", SHAPES, ids=SHAPE_IDS)
-def test_preprocess_up_vs_float64(hw, size, n):
+def test_preprocess_table_up_vs_float64(hw, size, n):
     (H0, W0), (Hn, Wn) = hw, size
     kinds = ("random",) if n == 1 else ("random", "gradient", "bright")
     pages = np.stack([_page(k, H0, W0, seed=H0 * 7 + W0 + i) for i, k in enumerate(kinds)])
@@ -135,7 +126,7 @@ def _small_page(seed, hw):
 
 
 @pytest.mark.parametrize("hw", SMALL, ids=["%dx%d" % hw for hw in SMALL])
-def test_engine_u8_path_equals_host_seam(det, hw):
+def test_engine_u8_path_equals_host_seam_of_table_op(det, hw):
     """detect_pages_u8 (the engine runs the op's kernel on the same arguments) against the reference's way: the host
     resize + standardisation of TextDetector.preprocess through the model-level seam."""
     page = _small_page(70, hw)

@@ -1,11 +1,11 @@
 """GPU: batches of pages of different sizes, from the page-table kernels up to the public API.
 
-  op level      the page-table entries against the same-size entries page by page, bit for bit: detector
-                pre-processing (ytk_op_dbnet_preprocess_table_u8 vs ytk_op_dbnet_preprocess_u8 / _up_u8), crop extraction
-                (ytk_extract_crops_table_u8 vs ytk_extract_crops_u8, records from data.crop_records), pyramid halving
-                (ytk_halve_pages_table_u8 vs cv2.resize(fx=fy=0.5, INTER_AREA), odd sizes) and the DBNet forward
-                (ytk_dbnet_forward_table_u8 vs detect_pages_u8 of each page alone); invalid records are an error and
-                launch nothing.
+  op level      a mixed page table against one-page tables page by page, bit for bit: detector pre-processing
+                (ytk_op_dbnet_preprocess_table_u8), crop extraction (ytk_extract_crops_table_u8, records from
+                data.crop_records), pyramid halving (ytk_halve_pages_table_u8 vs cv2.resize(fx=fy=0.5, INTER_AREA), odd
+                sizes) and the DBNet forward (ytk_dbnet_forward_table_u8 vs detect_pages_u8 of each page alone; the
+                same-size entry ytk_dbnet_forward_u8 vs the table entry); invalid records are an error and launch
+                nothing.
   module level  BatchedOCR / TextDetector.detect_pages / DocumentAnalyzer.analyze_pages over a mixed batch equal the
                 one-page calls, with the trained detector head so that the detector's own maps carry the lines.
 """
@@ -55,7 +55,7 @@ def test_shapes_map_to_the_listed_detector_inputs():
         assert D.shortest_edge_size(h, w, 1280, 1600) == hnwn
 
 
-def test_preprocess_table_equals_same_size_op_per_page():
+def test_preprocess_table_equals_one_page_table_per_page():
     pages = _random_pages([s for s, _ in SHAPES], 0)
     flat, table = _flat(pages)
     L = _lib.lib()
@@ -66,11 +66,10 @@ def test_preprocess_table_equals_same_size_op_per_page():
         _lib.check(L.ytk_op_dbnet_preprocess_table_u8(_fp(flat), flat.numel(), table[idx].ctypes.data, n, Hn, Wn,
                                                       _fp(got), None))
         for j, i in enumerate(idx):
-            H0, W0 = pages[i].shape[:2]
             ref = torch.empty((1, Hn + 6, Wn + 8, 8), dtype=torch.float16, device=DEV)
-            src = torch.from_numpy(pages[i]).to(DEV)
-            op = L.ytk_op_dbnet_preprocess_u8 if (Hn <= H0 and Wn <= W0) else L.ytk_op_dbnet_preprocess_up_u8
-            _lib.check(op(_fp(src), 1, H0, W0, Hn, Wn, _fp(ref), None))
+            src, one = _flat([pages[i]])
+            _lib.check(L.ytk_op_dbnet_preprocess_table_u8(_fp(src), src.numel(), one.ctypes.data, 1, Hn, Wn, _fp(ref),
+                                                          None))
             torch.cuda.synchronize()
             assert torch.equal(got[j].view(torch.int16), ref[0].view(torch.int16)), (SHAPES[i], j)
         assert torch.isnan(got[n]).all()          # nothing written past the last page
@@ -90,7 +89,22 @@ def test_dbnet_table_forward_equals_per_page_forward():
     assert torch.equal(host.to(DEV), got)
 
 
-def test_extract_crops_table_equals_same_size_entry_per_page():
+def test_dbnet_same_size_entry_equals_table_forward():
+    """ytk_dbnet_forward_u8, the entry for a same-size [n, H0, W0, 3] batch, builds the evenly spaced table itself."""
+    det = TextDetector(from_pretrained=False, device="cuda")
+    load_trained_head(det.model)
+    pages = [synthetic_page(260 + i, height=1200, width=1600)[0] for i in range(3)]
+    flat, table = _flat(pages)
+    ref = det.model.detect_pages_table(flat, table)
+    h, L = det.model._ensure(), _lib.lib()
+    for src in (flat, flat.cpu().pin_memory()):
+        got = torch.full_like(ref, float("nan"))
+        _lib.check(L.ytk_dbnet_forward_u8(h, _fp(src), 1 if src.is_cuda else 0, 3, 1200, 1600, _fp(got), 1, None))
+        torch.cuda.synchronize()
+        assert torch.equal(got, ref), src.device
+
+
+def test_extract_crops_table_equals_one_page_table_per_page():
     pages, quads = [], []
     for k, (h, w) in enumerate(MIXED):
         p, q = synthetic_page(220 + k, height=h, width=w)

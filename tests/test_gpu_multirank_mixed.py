@@ -26,7 +26,6 @@ def _worker(rank, world, port, q):
         from yomitoku_b200 import TextRecognizer
         from yomitoku_b200 import parallel as par
         from yomitoku_b200.data import crop_geometry, page_table
-        from yomitoku_b200.models import device_pages
         from yomitoku_b200.pipeline import BatchedOCR
         from yomitoku_b200.synth import peaked_parseq_state_dict, synthetic_page
         from yomitoku_b200.text_recognizer import plan_mini_batches
@@ -49,8 +48,7 @@ def _worker(rank, world, port, q):
         geoms = np.concatenate(geoms)
         table, _ = page_table([p.shape[:2] for p in pages])
         flat = torch.from_numpy(np.concatenate([p.reshape(-1) for p in pages])).cuda()
-        pages_dev = device_pages(flat, table)
-        assert isinstance(pages_dev, tuple)
+        pages_dev = (flat, table)
         ref = ocr._run_groups_dev_local(groups, geoms, pages_dev, None)
         x0 = dict(par.STATS)
         got = ocr._run_groups_dev(groups, geoms, pages_dev, None)

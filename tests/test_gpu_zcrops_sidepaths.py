@@ -1,5 +1,5 @@
 """GPU: the side paths of the device-side crop extraction - the orientation fallback's 180-degree second look (record
-bit `rot & 2`) and the source_downscale pyramid (ytk_halve_pages_u8) - against OpenCV and against the host-crop path of
+bit `rot & 2`) and the source_downscale pyramid (ytk_halve_pages_table_u8) - against OpenCV and against the host-crop path of
 TextRecognizer / BatchedOCR.  (Sorted after the other GPU test files on purpose: these kernels' arithmetic is pinned on
 the CPU by tests/test_crop_math.py; this file adds the end-to-end equalities.)"""
 import os
@@ -34,8 +34,9 @@ def test_device_orientation_fallback_crops_match_opencv():
         assert np.array_equal(got, D.resize_with_padding(cv2.rotate(roi, cv2.ROTATE_180), CFG.data.img_size))
 
 
-def test_pyramid_levels_match_opencv():
-    """ytk_halve_pages_u8 == cv2.resize(page, None, fx=0.5, fy=0.5, INTER_AREA), level after level, odd sizes included."""
+def test_pyramid_levels_match_opencv_through_tables():
+    """ytk_halve_pages_table_u8 == cv2.resize(page, None, fx=0.5, fy=0.5, INTER_AREA), level after level, odd sizes
+    included; the first level from a same-size (2, H, W, 3) batch, the next ones from the returned page table."""
     from yomitoku_b200.models import halve_pages_device
     cv2.setNumThreads(1)
     rng = np.random.default_rng(31)
@@ -48,8 +49,12 @@ def test_pyramid_levels_match_opencv():
                 break
             dev = halve_pages_device(dev)
             host = [cv2.resize(h, None, fx=0.5, fy=0.5, interpolation=cv2.INTER_AREA) for h in host]
-            got = dev.cpu().numpy()
-            assert got.shape[1:] == host[0].shape and np.array_equal(got[0], host[0]) and np.array_equal(got[1], host[1])
+            flat, table = dev
+            got = flat.cpu().numpy()
+            assert [(int(t["H"]), int(t["W"])) for t in table] == [h.shape[:2] for h in host]
+            for t, h in zip(table, host):
+                o = int(t["page_off"])
+                assert np.array_equal(got[o:o + h.size].reshape(h.shape), h)
 
 
 def test_recognizer_side_paths_device_crops_equal_host_crops():

@@ -228,7 +228,7 @@ def test_recognizer_cpu_plumbing_config1():
     assert padded == [320] * 16 and group == [0] * 16
 
 
-def test_batched_pipeline_with_stub_models():
+def test_batched_pipeline_page_tables_with_stub_models():
     """CPU: the whole host side of BatchedOCR (shared staging ring, worker pool, crop arena, descriptor building,
     three-stage stream, result assembly) with the two device calls replaced by stand-ins that compute from the bytes
     they are handed.  Per page the recognizer stand-in must see exactly the crops the one-page ParseqDataset cuts."""
@@ -254,7 +254,7 @@ def test_batched_pipeline_with_stub_models():
         batches.append(pages)
         maps.append(pm)
     det.model.input_size = lambda h, w: (Hn, Wn)
-    det.model.detect_pages_u8 = lambda pages, out=None, stream=None: out      # maps come from prob_override
+    det.model.detect_pages_table = lambda flat, table, out=None, stream=None: out    # maps come from prob_override
     S = rec.model.max_label_length + 1
     seen = []
 
@@ -301,9 +301,31 @@ def unicodedata_nfkc(s):
     return unicodedata.normalize("NFKC", s)
 
 
-def test_batched_pipeline_device_crops_with_stub_models(monkeypatch):
+def _pages_of(pages_dev):
+    """The (H, W, 3) pages of a (flat buffer, page table) pair - what the device page ops are handed."""
+    flat, table = pages_dev
+    assert table.dtype == D.PAGE_DTYPE
+    f = flat.numpy()
+    return [np.ascontiguousarray(f[int(t["page_off"]):int(t["page_off"]) + int(t["H"]) * int(t["W"]) * 3]
+                                 .reshape(t["H"], t["W"], 3)) for t in table]
+
+
+def _host_halve(host, pages_dev):
+    """Stand-in for models.halve_pages_device: the product's halve_pixel compiled for the host, page by page."""
+    import ctypes
+    vp = ctypes.c_void_p
+    out = []
+    for p in _pages_of(pages_dev):
+        H, W = p.shape[:2]
+        d = np.zeros((int(np.rint(H * 0.5)), int(np.rint(W * 0.5)), 3), np.uint8)
+        host.crop_host_halve(p.ctypes.data_as(vp), W, H, d.shape[1], d.shape[0], d.ctypes.data_as(vp))
+        out.append(d)
+    return torch.from_numpy(np.concatenate([d.reshape(-1) for d in out])), D.page_table([d.shape[:2] for d in out])[0]
+
+
+def test_batched_pipeline_device_crops_page_tables_with_stub_models(monkeypatch):
     """CPU: the device_crops path of BatchedOCR (pages kept "on the device", workers return quads + crop records only,
-    canvases cut by ytk_extract_crops_u8 in group order) with the three device calls replaced by stand-ins; the crop
+    canvases cut by ytk_extract_crops_table_u8 in group order) with the three device calls replaced by stand-ins; the crop
     stand-in runs the product's own crop arithmetic compiled for the host (oracle/crop_host.cpp).  Every word must get
     the canvas the one-page OpenCV path (ParseqDataset) cuts for it, and stream() must equal per-batch calls."""
     import ctypes
@@ -328,7 +350,7 @@ def test_batched_pipeline_device_crops_with_stub_models(monkeypatch):
         batches.append(pages)
         maps.append(pm)
     det.model.input_size = lambda h, w: (Hn, Wn)
-    det.model.detect_pages_u8 = lambda pages, out=None, stream=None: out
+    det.model.detect_pages_table = lambda flat, table, out=None, stream=None: out
     S = rec.model.max_label_length + 1
 
     class FakeDev:      # stands for the flat uint8 cuda tensor of canvases
@@ -341,13 +363,13 @@ def test_batched_pipeline_device_crops_with_stub_models(monkeypatch):
     def fake_extract(pages_dev, geoms, stream=None):
         sb, cb = layout_crop_buffers(geoms)
         scratch, canv = np.zeros(max(sb, 1), np.uint8), np.full(max(cb, 1), 99, np.uint8)
-        pg = np.ascontiguousarray(pages_dev.numpy())
+        pg = _pages_of(pages_dev)
         vp = ctypes.c_void_p
         for i in sorted(set(geoms["page"].tolist())):       # the host harness takes one page at a time
             sel = np.ascontiguousarray(geoms[geoms["page"] == i])
             sel["page"] = 0
-            host.crop_host_extract(pg[i].ctypes.data_as(vp), pg.shape[1], pg.shape[2], sel.ctypes.data_as(vp), len(sel),
-                                   scratch.ctypes.data_as(vp), canv.ctypes.data_as(vp))
+            host.crop_host_extract(pg[i].ctypes.data_as(vp), pg[i].shape[0], pg[i].shape[1], sel.ctypes.data_as(vp),
+                                   len(sel), scratch.ctypes.data_as(vp), canv.ctypes.data_as(vp))
         return FakeDev(canv), cb
 
     def fake_ptr(ptr, on_device, total, descs, n, n_groups, stream=None):
@@ -487,7 +509,7 @@ def test_recognizer_call_device_crops_with_stub_models(monkeypatch):
                 assert 0 < sum(x != y for x, y in zip(b.contents, c.contents)) < len(b.contents)
 
 
-def test_batched_pipeline_device_crops_source_downscale_with_stub_models(monkeypatch):
+def test_batched_pipeline_device_crops_source_downscale_page_tables_with_stub_models(monkeypatch):
     """CPU: BatchedOCR with device_crops AND source_downscale: the workers return records + pyramid levels, the levels
     are built "on the device" (stand-in: the product's halve_pixel compiled for the host) for the whole batch, one
     extraction per level; every word must get the canvas ParseqDataset(source_downscale=True) cuts for it."""
@@ -503,7 +525,7 @@ def test_batched_pipeline_device_crops_source_downscale_with_stub_models(monkeyp
     rec = TextRecognizer(model_name="parseq-tiny-dynw-v4", from_pretrained=False, device="cpu", dynamic_width=True,
                          batch_bucketing=True, source_downscale=True)
     det.model.input_size = lambda h, w: (1184, 1600)
-    det.model.detect_pages_u8 = lambda pages, out=None, stream=None: out
+    det.model.detect_pages_table = lambda flat, table, out=None, stream=None: out
     S = rec.model.max_label_length + 1
     big = [[[100, 100], [900, 100], [900, 240], [100, 240]], [[50, 300], [700, 300], [700, 370], [50, 370]],
            [[1000, 100], [1100, 100], [1100, 900], [1000, 900]]]
@@ -525,23 +547,14 @@ def test_batched_pipeline_device_crops_source_downscale_with_stub_models(monkeyp
     def fake_extract(pages_dev, geoms, stream=None):
         sb, cb = layout_crop_buffers(geoms)
         scratch, canv = np.zeros(max(sb, 1), np.uint8), np.full(max(cb, 1), 99, np.uint8)
-        pg = np.ascontiguousarray(pages_dev.numpy())
+        pg = _pages_of(pages_dev)
         for i in sorted(set(geoms["page"].tolist())):
             m = geoms["page"] == i
             sel = np.ascontiguousarray(geoms[m])
             sel["page"] = 0
-            host.crop_host_extract(pg[i].ctypes.data_as(vp), pg.shape[1], pg.shape[2], sel.ctypes.data_as(vp), len(sel),
-                                   scratch.ctypes.data_as(vp), canv.ctypes.data_as(vp))
+            host.crop_host_extract(pg[i].ctypes.data_as(vp), pg[i].shape[0], pg[i].shape[1], sel.ctypes.data_as(vp),
+                                   len(sel), scratch.ctypes.data_as(vp), canv.ctypes.data_as(vp))
         return FakeDev(canv), cb
-
-    def fake_halve(pages_dev, stream=None):
-        src = np.ascontiguousarray(pages_dev.numpy())
-        n, H, W, _ = src.shape
-        dH, dW = int(np.rint(H * 0.5)), int(np.rint(W * 0.5))
-        dst = np.zeros((n, dH, dW, 3), np.uint8)
-        for i in range(n):
-            host.crop_host_halve(src[i].ctypes.data_as(vp), W, H, dW, dH, dst[i].ctypes.data_as(vp))
-        return torch.from_numpy(dst)
 
     def fake_ptr(ptr, on_device, total, descs, n, n_groups, stream=None):
         raw = np.ctypeslib.as_array(ctypes.cast(ptr, ctypes.POINTER(ctypes.c_uint8)), shape=(total,))
@@ -552,7 +565,7 @@ def test_batched_pipeline_device_crops_source_downscale_with_stub_models(monkeyp
         return ids, np.full((n, S), 0.5, np.float32), np.full((n_groups,), S, np.int32)
 
     monkeypatch.setattr(M, "extract_crops_device", fake_extract)
-    monkeypatch.setattr(M, "halve_pages_device", fake_halve)
+    monkeypatch.setattr(M, "halve_pages_device", lambda pages_dev, stream=None: _host_halve(host, pages_dev))
     monkeypatch.setattr(M, "concat_device_buffers",
                         lambda parts, stream=None: parts[0][0] if len(parts) == 1 else
                         FakeDev(np.concatenate([t.arr[:n] for t, n in parts])))
@@ -574,7 +587,7 @@ def test_batched_pipeline_device_crops_source_downscale_with_stub_models(monkeyp
         assert [w.content[0] for w in got[i].words] == [unicodedata_nfkc(e)[0] for e in expect]
 
 
-def test_batched_pipeline_orientation_fallback_with_stub_models(monkeypatch):
+def test_batched_pipeline_orientation_fallback_page_tables_with_stub_models(monkeypatch):
     """CPU: BatchedOCR honours rec_orientation_fallback (it switches the batch to the device-crops path, where the second
     look is the same record with `rot |= 2`): per page the words must equal what TextRecognizer.__call__ returns on the
     host path with the fallback on (stand-in model: ids / score depend on where the pixels are, so a 180-degree turn
@@ -610,18 +623,18 @@ def test_batched_pipeline_orientation_fallback_with_stub_models(monkeypatch):
     def fake_extract(pages_dev, geoms, stream=None):
         sb, cb = layout_crop_buffers(geoms)
         scratch, canv = np.zeros(max(sb, 1), np.uint8), np.full(max(cb, 1), 99, np.uint8)
-        pg = np.ascontiguousarray(pages_dev.numpy())
+        pg = _pages_of(pages_dev)
         for i in sorted(set(geoms["page"].tolist())):
             sel = np.ascontiguousarray(geoms[geoms["page"] == i])
             sel["page"] = 0
-            host.crop_host_extract(pg[i].ctypes.data_as(vp), pg.shape[1], pg.shape[2], sel.ctypes.data_as(vp), len(sel),
-                                   scratch.ctypes.data_as(vp), canv.ctypes.data_as(vp))
+            host.crop_host_extract(pg[i].ctypes.data_as(vp), pg[i].shape[0], pg[i].shape[1], sel.ctypes.data_as(vp),
+                                   len(sel), scratch.ctypes.data_as(vp), canv.ctypes.data_as(vp))
         return FakeDev(canv), cb
 
     monkeypatch.setattr(M, "extract_crops_device", fake_extract)
     det = TextDetector(from_pretrained=False, device="cpu")
     det.model.input_size = lambda h, w: (1184, 1600)
-    det.model.detect_pages_u8 = lambda pages, out=None, stream=None: out
+    det.model.detect_pages_table = lambda flat, table, out=None, stream=None: out
     rec = TextRecognizer(model_name="parseq-tiny-dynw-v4", from_pretrained=False, device="cpu", dynamic_width=True,
                          batch_bucketing=True, rec_orientation_fallback=True, rec_orientation_fallback_thresh=0.75)
 

@@ -126,14 +126,12 @@ def _stub_models(monkeypatch, source_downscale=False):
     host = ctypes.CDLL(build_crop_host.build())
     vp = ctypes.c_void_p
 
-    def pages_of(pages_dev):
-        if isinstance(pages_dev, tuple):        # (flat buffer, page table)
-            flat, table = pages_dev
-            assert table.dtype == D.PAGE_DTYPE
-            f = flat.numpy()
-            return [f[int(t["page_off"]):int(t["page_off"]) + int(t["H"]) * int(t["W"]) * 3].reshape(t["H"], t["W"], 3)
-                    for t in table]
-        return list(np.ascontiguousarray(pages_dev.numpy()))
+    def pages_of(pages_dev):                    # (flat buffer, page table)
+        flat, table = pages_dev
+        assert table.dtype == D.PAGE_DTYPE
+        f = flat.numpy()
+        return [f[int(t["page_off"]):int(t["page_off"]) + int(t["H"]) * int(t["W"]) * 3].reshape(t["H"], t["W"], 3)
+                for t in table]
 
     def fake_extract(pages_dev, geoms, stream=None):
         sb, cb = D.layout_crop_buffers(geoms)
@@ -156,8 +154,6 @@ def _stub_models(monkeypatch, source_downscale=False):
             d = np.zeros((dH, dW, 3), np.uint8)
             host.crop_host_halve(p.ctypes.data_as(vp), W, H, dW, dH, d.ctypes.data_as(vp))
             out.append(d)
-        if not isinstance(pages_dev, tuple):
-            return torch.from_numpy(np.stack(out))
         table, total = D.page_table([d.shape[:2] for d in out])
         return torch.from_numpy(np.concatenate([d.reshape(-1) for d in out])), table
 
@@ -169,20 +165,11 @@ def _stub_models(monkeypatch, source_downscale=False):
     det = TextDetector(from_pretrained=False, device="cpu")
     calls = []
 
-    def fake_u8(pages, out=None, stream=None):
-        calls.append(("u8", tuple(pages.shape)))
-        return out
-
     def fake_table(flat, table, out=None, stream=None):
-        from yomitoku_b200.models import uniform_pages
-        same = uniform_pages(flat, table)
-        if same is not None:
-            return fake_u8(same, out, stream)
-        calls.append(("table", len(table)))
+        calls.append([(int(t["H"]), int(t["W"])) for t in table])
         assert len({_input_size(int(t["H"]), int(t["W"])) for t in table}) == 1
         return out
 
-    det.model.detect_pages_u8 = fake_u8
     det.model.detect_pages_table = fake_table
     rec = TextRecognizer(model_name="parseq-tiny-dynw-v4", from_pretrained=False, device="cpu", dynamic_width=True,
                          batch_bucketing=True, source_downscale=source_downscale)
@@ -207,7 +194,7 @@ def _words(results):
 
 @pytest.mark.parametrize("device_crops,workers,source_downscale", [(True, 2, False), (False, 2, False),
                                                                    (True, 1, False), (True, 2, True)])
-def test_mixed_batch_equals_batches_of_one(monkeypatch, device_crops, workers, source_downscale):
+def test_mixed_batch_equals_batches_of_one_through_tables(monkeypatch, device_crops, workers, source_downscale):
     det, rec, calls = _stub_models(monkeypatch, source_downscale)
     mixed = _mixed_pages()
     pages, quads = [p for p, _ in mixed], [q for _, q in mixed]
@@ -226,17 +213,14 @@ def test_mixed_batch_equals_batches_of_one(monkeypatch, device_crops, workers, s
     assert _words(got) == _words(single)
     assert [_words(s) for s in streamed] == [_words([single[i] for i in ix]) for ix in ([0, 1, 2], [3, 4, 5],
                                                                                        [1, 2, 3, 4])]
-    # one detector call per chunk of pages that share an input size: the same-size entry where the chunk's pages have
-    # one size, the table entry where they do not
+    # one detector call per chunk of pages that share an input size, with the chunk's pages in the table
     plan = BatchPlan([p.shape[:2] for p in pages], _input_size, 2)
-    expect = []
-    for _, _, idx in plan.chunks:
-        shapes = {pages[i].shape for i in idx}
-        expect.append(("u8", (len(idx),) + pages[idx[0]].shape) if len(shapes) == 1 else ("table", len(idx)))
-    assert mixed_calls == expect and ("table", 2) in expect and len(plan.chunks) >= 4
+    expect = [[pages[i].shape[:2] for i in idx] for _, _, idx in plan.chunks]
+    assert mixed_calls == expect and len(plan.chunks) >= 4
+    assert any(len(set(c)) > 1 for c in expect)          # a chunk of pages of different sizes
 
 
-def test_same_size_batch_calls_the_same_size_entry(monkeypatch):
+def test_same_size_batch_calls_one_table_per_chunk(monkeypatch):
     det, rec, calls = _stub_models(monkeypatch)
     page, quads = synthetic_page(150)
     ocr = BatchedOCR(det, rec, workers=1, det_batch=2, device_crops=True)
@@ -245,4 +229,4 @@ def test_same_size_batch_calls_the_same_size_entry(monkeypatch):
         ocr([page] * 5, quads_override=[quads[:10]] * 5)
     finally:
         ocr.close()
-    assert calls == [("u8", (2, 1200, 1600, 3)), ("u8", (2, 1200, 1600, 3)), ("u8", (1, 1200, 1600, 3))]
+    assert calls == [[(1200, 1600)] * 2, [(1200, 1600)] * 2, [(1200, 1600)]]

@@ -114,21 +114,26 @@ def test_single_query_attn_refusals(lib, kwargs, fragment):
 W_HOST = (ctypes.c_float * (64 * 64 * 4))()      # host weights: large enough for every entry, never read on refusal
 
 
-def _prep(lib, src=P, n=1, H0=1200, W0=1600, Hn=1184, Wn=1600, canvas=P):
-    return lib.ytk_op_dbnet_preprocess_u8(src, n, H0, W0, Hn, Wn, canvas, None)
+def preprocess_table(lib, src=P, n=1, H0=1200, W0=1600, Hn=1184, Wn=1600, canvas=P, table=True):
+    """ytk_op_dbnet_preprocess_table_u8 on a table of n evenly spaced H0 x W0 whole pages (at most 4 records are
+    written) in a buffer of n 1200x1600 pages."""
+    t = (_lib.YtkRtdetrSrc * 4)()
+    for i in range(min(n, 4)):
+        t[i] = _lib.YtkRtdetrSrc(i * H0 * W0 * 3, H0, W0, 0, 0, W0, H0)
+    return lib.ytk_op_dbnet_preprocess_table_u8(src, n * 1200 * 1600 * 3, t if table else None, n, Hn, Wn, canvas,
+                                                None)
 
 
 @pytest.mark.parametrize("kwargs,fragment", [
     (dict(src=None), b"null argument"), (dict(canvas=None), b"null argument"),
-    (dict(n=0), b"non-positive size"), (dict(H0=0), b"non-positive size"), (dict(W0=-1), b"non-positive size"),
-    (dict(Hn=0), b"non-positive size"), (dict(Wn=0), b"non-positive size"),
-    # the upscale that ytk_dbnet_forward_u8 refuses too
-    (dict(Hn=1216), b"1200x1600 -> 1216x1600 is an upscale"), (dict(Wn=1632), b"1200x1600 -> 1184x1632 is an upscale"),
+    (dict(n=0), b"0 page records"), (dict(n=65536), b"65536 page records"), (dict(table=False), b"1 page records"),
+    (dict(H0=0), b"page 0 (at 0, 0x1600"), (dict(W0=-1), b"page 0 (at 0, 1200x-1"),
+    (dict(Hn=0), b"non-positive input size 0x1600"), (dict(Wn=0), b"non-positive input size 1184x0"),
     (dict(canvas=P + 8), b"16-byte aligned"),
 ])
-def test_dbnet_preprocess_refusals(lib, kwargs, fragment):
+def test_dbnet_preprocess_table_refusals(lib, kwargs, fragment):
     before = lib.ytk_launch_count()
-    _refused(lib, _prep(lib, **kwargs), fragment)
+    _refused(lib, preprocess_table(lib, **kwargs), fragment)
     assert lib.ytk_launch_count() == before
 
 

@@ -73,10 +73,6 @@ def _declare(lib):
                                         c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
     lib.ytk_op_apply_rep_cut.restype = c_int
     lib.ytk_op_apply_rep_cut.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]
-    lib.ytk_op_dbnet_preprocess_u8.restype = c_int
-    lib.ytk_op_dbnet_preprocess_u8.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
-    lib.ytk_op_dbnet_preprocess_up_u8.restype = c_int
-    lib.ytk_op_dbnet_preprocess_up_u8.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
     lib.ytk_op_dbnet_preprocess_table_u8.restype = c_int
     lib.ytk_op_dbnet_preprocess_table_u8.argtypes = [c_void_p, c_ll, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]
     lib.ytk_op_dbnet_stem_f16.restype = c_int
@@ -170,11 +166,6 @@ def _declare_crops(lib):
     lib.ytk_dbnet_post_front.restype = c_int
     lib.ytk_dbnet_post_front.argtypes = [c_void_p, c_int, c_int, c_int, ctypes.c_float, c_void_p, c_ll, c_void_p, c_int,
                                          c_void_p, c_void_p]
-    lib.ytk_extract_crops_u8.restype = c_int
-    lib.ytk_extract_crops_u8.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_ll, c_void_p, c_ll,
-                                         c_void_p]
-    lib.ytk_halve_pages_u8.restype = c_int
-    lib.ytk_halve_pages_u8.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p]
     lib.ytk_extract_crops_table_u8.restype = c_int
     lib.ytk_extract_crops_table_u8.argtypes = [c_void_p, c_ll, c_void_p, c_int, c_void_p, c_int, c_void_p, c_ll,
                                                c_void_p, c_ll, c_void_p]

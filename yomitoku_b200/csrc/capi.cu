@@ -556,48 +556,6 @@ static int check_page_table(const ytk_page* t, int n, long long pages_bytes, boo
 
 static_assert(sizeof(ytk_page) == sizeof(ytk::RtSrc), "ytk_page and ytk::RtSrc must have one layout");
 
-// The two pre-processing entries: `up` = 0 takes the shapes OpenCV decimates with its area tables (no axis grows),
-// `up` = 1 the shapes it up-scales bilinearly (some axis grows).  One launcher serves both and picks by the same rule.
-static int op_dbnet_preprocess(const char* who, int up, const uint8_t* src_dev, int n, int H0, int W0, int Hn, int Wn,
-                               void* canvas_dev, void* cuda_stream) {
-    if (!src_dev || !canvas_dev) {
-        ytk::set_error("%s: null argument", who);
-        return YTK_ERR;
-    }
-    if (n < 1 || H0 < 1 || W0 < 1 || Hn < 1 || Wn < 1) {
-        ytk::set_error("%s: non-positive size (n %d, page %dx%d, input %dx%d)", who, n, H0, W0, Hn, Wn);
-        return YTK_ERR;
-    }
-    const bool grows = Hn > H0 || Wn > W0;
-    if (grows && !up) {
-        ytk::set_error("%s: %dx%d -> %dx%d is an upscale; INTER_AREA decimation only (ytk_op_dbnet_preprocess_up_u8 "
-                       "takes it)", who, H0, W0, Hn, Wn);
-        return YTK_ERR;
-    }
-    if (!grows && up) {
-        ytk::set_error("%s: %dx%d -> %dx%d grows no axis; INTER_AREA decimation is ytk_op_dbnet_preprocess_u8", who, H0,
-                       W0, Hn, Wn);
-        return YTK_ERR;
-    }
-    if (misaligned(canvas_dev, 16)) {
-        ytk::set_error("%s: canvas_dev must be 16-byte aligned", who);
-        return YTK_ERR;
-    }
-    return ytk::launch_preprocess(src_dev, n, H0, W0, Hn, Wn, canvas_dev, static_cast<cudaStream_t>(cuda_stream))
-               ? YTK_ERR
-               : YTK_OK;
-}
-
-int ytk_op_dbnet_preprocess_u8(const uint8_t* src_dev, int n, int H0, int W0, int Hn, int Wn, void* canvas_dev,
-                               void* cuda_stream) {
-    return op_dbnet_preprocess("ytk_op_dbnet_preprocess_u8", 0, src_dev, n, H0, W0, Hn, Wn, canvas_dev, cuda_stream);
-}
-
-int ytk_op_dbnet_preprocess_up_u8(const uint8_t* src_dev, int n, int H0, int W0, int Hn, int Wn, void* canvas_dev,
-                                  void* cuda_stream) {
-    return op_dbnet_preprocess("ytk_op_dbnet_preprocess_up_u8", 1, src_dev, n, H0, W0, Hn, Wn, canvas_dev, cuda_stream);
-}
-
 int ytk_op_dbnet_preprocess_table_u8(const uint8_t* pages_dev, long long pages_bytes, const ytk_page* table, int n,
                                      int Hn, int Wn, void* canvas_dev, void* cuda_stream) {
     const char* who = "ytk_op_dbnet_preprocess_table_u8";
@@ -846,37 +804,10 @@ int ytk_dbnet_input_size(const ytk_dbnet* h, int H0, int W0, int* Hn, int* Wn) {
     return YTK_OK;
 }
 
-int ytk_dbnet_forward_u8(ytk_dbnet* h, const uint8_t* pages, int pages_on_device, int n_pages, int H0, int W0,
-                         float* prob_out, int out_on_device, void* cuda_stream) {
-    std::lock_guard<std::mutex> lk(h->mu);
-    DevGuard dev_guard(h->device);  // host threads start on device 0: the handle's device is the one that counts
-    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-    int Hn, Wn;
-    ytk::dbnet_input_size(H0, W0, h->shortest, h->limit, &Hn, &Wn);
-    ytk::DbnetEngine* e = get_engine(h, n_pages, Hn, Wn);
-    if (!e) return YTK_ERR;
-    order_after_previous(h, st);
-    const uint8_t* src = pages;
-    if (!pages_on_device) {
-        const size_t bytes = (size_t)n_pages * H0 * W0 * 3;
-        if (ensure_stage(h, bytes)) return YTK_ERR;
-        if (cudaMemcpyAsync(h->stage, pages, bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) {
-            ytk::set_error("H2D copy of pages failed");
-            return YTK_ERR;
-        }
-        src = reinterpret_cast<const uint8_t*>(h->stage);
-    }
-    if (ytk::launch_preprocess(src, n_pages, H0, W0, Hn, Wn, e->input, st)) {
-        ytk::set_error("preprocess launch failed");
-        return YTK_ERR;
-    }
-    return finish_forward(h, e, prob_out, out_on_device, st);
-}
-
-int ytk_dbnet_forward_table_u8(ytk_dbnet* h, const uint8_t* pages, int pages_on_device, long long pages_bytes,
-                               const ytk_page* table, int n_pages, float* prob_out, int out_on_device,
-                               void* cuda_stream) {
-    const char* who = "ytk_dbnet_forward_table_u8";
+// Both u8 entries: `who` names the entry the caller called in error messages.
+static int dbnet_forward_table(const char* who, ytk_dbnet* h, const uint8_t* pages, int pages_on_device,
+                               long long pages_bytes, const ytk_page* table, int n_pages, float* prob_out,
+                               int out_on_device, void* cuda_stream) {
     if (!h || !pages || !prob_out) {
         ytk::set_error("%s: null argument", who);
         return YTK_ERR;
@@ -924,6 +855,22 @@ int ytk_dbnet_forward_table_u8(ytk_dbnet* h, const uint8_t* pages, int pages_on_
         return YTK_ERR;
     }
     return finish_forward(h, e, prob_out, out_on_device, st);
+}
+
+int ytk_dbnet_forward_u8(ytk_dbnet* h, const uint8_t* pages, int pages_on_device, int n_pages, int H0, int W0,
+                         float* prob_out, int out_on_device, void* cuda_stream) {
+    const long long page_bytes = (long long)H0 * W0 * 3;
+    std::vector<ytk_page> table((size_t)std::max(n_pages, 0));
+    for (int i = 0; i < n_pages; ++i) table[i] = {i * page_bytes, H0, W0, 0, 0, W0, H0};
+    return dbnet_forward_table("ytk_dbnet_forward_u8", h, pages, pages_on_device, n_pages * page_bytes, table.data(),
+                               n_pages, prob_out, out_on_device, cuda_stream);
+}
+
+int ytk_dbnet_forward_table_u8(ytk_dbnet* h, const uint8_t* pages, int pages_on_device, long long pages_bytes,
+                               const ytk_page* table, int n_pages, float* prob_out, int out_on_device,
+                               void* cuda_stream) {
+    return dbnet_forward_table("ytk_dbnet_forward_table_u8", h, pages, pages_on_device, pages_bytes, table, n_pages,
+                               prob_out, out_on_device, cuda_stream);
 }
 
 int ytk_dbnet_forward_f32(ytk_dbnet* h, const float* x, int x_on_device, int n, int H, int W, float* prob_out,
@@ -992,61 +939,6 @@ int ytk_dbnet_debug_tensor(ytk_dbnet* h, int n_pages, int Hn, int Wn, const char
 
 static_assert(sizeof(ytk_crop_geom) == sizeof(ytk::CropGeom), "ytk_crop_geom and ytk::CropGeom must have one layout");
 
-int ytk_extract_crops_u8(const uint8_t* pages_dev, int n_pages, int H0, int W0, const ytk_crop_geom* geoms, int n_crops,
-                         uint8_t* scratch_dev, long long scratch_bytes, uint8_t* canvases_dev, long long canvases_bytes,
-                         void* cuda_stream) {
-    if (n_crops == 0) return YTK_OK;
-    if (!pages_dev || !geoms || !scratch_dev || !canvases_dev || n_pages <= 0 || H0 <= 0 || W0 <= 0 || n_crops < 0) {
-        ytk::set_error("ytk_extract_crops_u8: null or empty argument");
-        return YTK_ERR;
-    }
-    long long roi_end = 0;
-    for (int i = 0; i < n_crops; ++i) {
-        const ytk_crop_geom& g = geoms[i];
-        const long long sw = (g.rot & 1) ? g.h : g.w, sh = (g.rot & 1) ? g.w : g.h;
-        const bool ok = g.page >= 0 && g.page < n_pages && g.x0 >= 0 && g.y0 >= 0 && g.rw >= 1 && g.rh >= 1 &&
-                        (long long)g.x0 + g.rw <= W0 && (long long)g.y0 + g.rh <= H0 && g.w >= 1 && g.h >= 1 &&
-                        g.rot >= 0 && g.rot <= 3 && g.cw >= 1 && g.ch >= 1 && g.cw <= sw && g.ch <= sh &&
-                        g.cw <= g.canvas_w && g.ch <= g.canvas_h && g.roi_off >= 0 &&
-                        g.roi_off + (long long)g.w * g.h * 3 <= scratch_bytes && g.pix_off >= 0 &&
-                        g.pix_off + (long long)g.canvas_w * g.canvas_h * 3 <= canvases_bytes;
-        if (!ok) {
-            ytk::set_error("ytk_extract_crops_u8: inconsistent crop record %d (page %d, roi %d,%d %dx%d, out %dx%d rot %d, "
-                           "content %dx%d, canvas %dx%d)", i, g.page, g.x0, g.y0, g.rw, g.rh, g.w, g.h, g.rot, g.cw,
-                           g.ch, g.canvas_w, g.canvas_h);
-            return YTK_ERR;
-        }
-        roi_end = std::max(roi_end, g.roi_off + (long long)g.w * g.h * 3);
-    }
-    // the records are staged in the caller's scratch buffer, 16-byte aligned after the ROIs: no allocation here
-    const long long rec_off = (roi_end + 15) / 16 * 16;
-    const long long rec_bytes = (long long)n_crops * (long long)sizeof(ytk::CropGeom);
-    if (rec_off + rec_bytes > scratch_bytes) {
-        ytk::set_error("ytk_extract_crops_u8: scratch_dev holds %lld bytes, need %lld (ROIs) + %lld (records)", scratch_bytes,
-                       rec_off, rec_bytes);
-        return YTK_ERR;
-    }
-    cudaPointerAttributes attr;
-    if (cudaPointerGetAttributes(&attr, pages_dev) != cudaSuccess || attr.type != cudaMemoryTypeDevice) {
-        cudaGetLastError();
-        ytk::set_error("ytk_extract_crops_u8: pages_dev is not a device pointer");
-        return YTK_ERR;
-    }
-    DevGuard dev_guard(attr.device);  // host threads start on device 0: the device that owns the pages is the one that counts
-    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-    ytk::CropGeom* dev = reinterpret_cast<ytk::CropGeom*>(scratch_dev + rec_off);
-    cudaError_t err = cudaMemcpyAsync(dev, geoms, (size_t)rec_bytes, cudaMemcpyHostToDevice, st);
-    if (err != cudaSuccess) {
-        ytk::set_error("ytk_extract_crops_u8: record upload failed: %s", cudaGetErrorString(err));
-        return YTK_ERR;
-    }
-    if (ytk::launch_extract_crops(pages_dev, H0, W0, dev, n_crops, scratch_dev, canvases_dev, st)) {
-        ytk::set_error("ytk_extract_crops_u8: kernel launch failed");
-        return YTK_ERR;
-    }
-    return YTK_OK;
-}
-
 int ytk_extract_crops_table_u8(const uint8_t* pages_dev, long long pages_bytes, const ytk_page* table, int n_pages,
                                const ytk_crop_geom* geoms, int n_crops, uint8_t* scratch_dev, long long scratch_bytes,
                                uint8_t* canvases_dev, long long canvases_bytes, void* cuda_stream) {
@@ -1106,29 +998,6 @@ int ytk_extract_crops_table_u8(const uint8_t* pages_dev, long long pages_bytes, 
     const ytk::RtSrc* tab = reinterpret_cast<const ytk::RtSrc*>(scratch_dev + rec_off + rec_bytes);
     if (ytk::launch_extract_crops_table(pages_dev, tab, dev, n_crops, scratch_dev, canvases_dev, st)) {
         ytk::set_error("%s: kernel launch failed", who);
-        return YTK_ERR;
-    }
-    return YTK_OK;
-}
-
-int ytk_halve_pages_u8(const uint8_t* src_dev, int n_pages, int H, int W, uint8_t* dst_dev, int dH, int dW,
-                       void* cuda_stream) {
-    // cv2.resize(..., fx=0.5, fy=0.5): dsize = (cvRound(W * 0.5), cvRound(H * 0.5)), round half to even
-    const int eh = (int)nearbyint(H * 0.5), ew = (int)nearbyint(W * 0.5);
-    if (!src_dev || !dst_dev || n_pages <= 0 || H <= 0 || W <= 0 || dH != eh || dW != ew || dH < 1 || dW < 1) {
-        ytk::set_error("ytk_halve_pages_u8: bad arguments (%d pages %dx%d -> %dx%d, expected %dx%d)", n_pages, H, W, dH, dW,
-                       eh, ew);
-        return YTK_ERR;
-    }
-    cudaPointerAttributes attr;
-    if (cudaPointerGetAttributes(&attr, src_dev) != cudaSuccess || attr.type != cudaMemoryTypeDevice) {
-        cudaGetLastError();
-        ytk::set_error("ytk_halve_pages_u8: src_dev is not a device pointer");
-        return YTK_ERR;
-    }
-    DevGuard dev_guard(attr.device);
-    if (ytk::launch_halve_pages(src_dev, n_pages, H, W, dst_dev, dH, dW, static_cast<cudaStream_t>(cuda_stream))) {
-        ytk::set_error("ytk_halve_pages_u8: kernel launch failed");
         return YTK_ERR;
     }
     return YTK_OK;

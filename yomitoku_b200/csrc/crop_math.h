@@ -132,11 +132,6 @@ YTK_HD void warp_store_page(const CropGeom& g, const uint8_t* page, int W0, int 
     o[2] = (uint8_t)v[0];
 }
 
-// The same for same-size pages: [n][H0][W0][3] BGR, crop g on page g.page.
-YTK_HD void warp_store(const CropGeom& g, const uint8_t* pages, int H0, int W0, int x, int y, uint8_t* scratch) {
-    warp_store_page(g, pages + (long long)g.page * H0 * W0 * 3, W0, x, y, scratch);
-}
-
 // Taps of one destination index along one axis of cv2.resize(INTER_AREA) (computeResizeAreaTab): an optional partial
 // left cell, whole cells [s1, s2), an optional partial right cell.
 struct AreaTaps {

@@ -9,9 +9,8 @@
 //   crop_canvas_kernel  cv2.resize(INTER_AREA) of the ROI (shrinking only) pasted top-left on a black canvas
 //   halve_pages_kernel  one level of the source_downscale pyramid: cv2.resize(page, None, fx=0.5, fy=0.5, INTER_AREA)
 //
-// The pages are either same-size [n][H0][W0][3] or described by a page table (RtSrc records: byte offset and size of
-// each page in one flat buffer, so pages of different sizes share a launch); the kernels differ only in where a page's
-// base pointer and row pitch come from.
+// The pages are described by a page table (RtSrc records: byte offset and size of each page in one flat buffer, so
+// pages of different sizes share a launch).
 //
 // The arithmetic lives in crop_math.h and is compiled for the host as well (oracle/crop_host.cpp), where the CPU tests
 // pin it bit for bit against OpenCV.  This file MUST be compiled with --fmad=false (yomitoku_b200/build.py): OpenCV's
@@ -36,19 +35,15 @@ __device__ __forceinline__ void load_geom(CropGeom* sg, const CropGeom* g) {
     __syncthreads();
 }
 
-// pages: a page table (table != nullptr: crop g reads page table[g.page]) or same-size pages [n][H0][W0][3]
+// crop g reads page table[g.page] of `pages`
 __global__ void __launch_bounds__(kWarpThreads) crop_warp_kernel(const uint8_t* __restrict__ pages,
-                                                                  const RtSrc* __restrict__ table, int H0, int W0,
+                                                                  const RtSrc* __restrict__ table,
                                                                   const CropGeom* __restrict__ geoms,
                                                                   uint8_t* __restrict__ scratch) {
     __shared__ CropGeom g;
     load_geom(&g, geoms + blockIdx.x);
-    const uint8_t* page = pages + (long long)g.page * H0 * W0 * 3;
-    int W = W0;
-    if (table) {
-        page = pages + table[g.page].page_off;
-        W = table[g.page].W;
-    }
+    const uint8_t* page = pages + table[g.page].page_off;
+    const int W = table[g.page].W;
     const int npix = g.w * g.h;
     for (int p = blockIdx.y * blockDim.x + threadIdx.x; p < npix; p += gridDim.y * blockDim.x) {
         const int y = p / g.w;
@@ -68,50 +63,30 @@ __global__ void __launch_bounds__(kCanvasThreads) crop_canvas_kernel(const CropG
     }
 }
 
-// One page per blockIdx.y: from the page tables (src_table / dst_table != nullptr) or page img of same-size batches.
-__global__ void halve_pages_kernel(const uint8_t* __restrict__ src, const RtSrc* __restrict__ src_table, int sh, int sw,
-                                   uint8_t* __restrict__ dst, const RtSrc* __restrict__ dst_table, int dh, int dw) {
-    const long long img = blockIdx.y;
-    const uint8_t* s = src + img * sh * sw * 3;
-    uint8_t* d = dst + img * dh * dw * 3;
-    if (src_table) {
-        const RtSrc a = src_table[img], b = dst_table[img];
-        s = src + a.page_off;
-        sh = a.H;
-        sw = a.W;
-        d = dst + b.page_off;
-        dh = b.H;
-        dw = b.W;
-    }
+// One page per blockIdx.y: page img of src_table -> page img of dst_table.
+__global__ void halve_pages_kernel(const uint8_t* __restrict__ src, const RtSrc* __restrict__ src_table,
+                                   uint8_t* __restrict__ dst, const RtSrc* __restrict__ dst_table) {
+    const RtSrc a = src_table[blockIdx.y], b = dst_table[blockIdx.y];
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= dh * dw) return;
-    const int y = idx / dw;
-    halve_pixel(s, sw, sh, idx - y * dw, y, d + (long long)idx * 3);
-}
-
-static int halve(const uint8_t* src, const RtSrc* src_table, int n, int sh, int sw, uint8_t* dst,
-                 const RtSrc* dst_table, int dh, int dw, long long max_pixels, cudaStream_t st) {
-    if (n <= 0 || max_pixels <= 0) return 0;
-    if (n > 65535 || max_pixels > INT_MAX) return 1;
-    halve_pages_kernel<<<dim3((unsigned)((max_pixels + 255) / 256), (unsigned)n), 256, 0, st>>>(
-        src, src_table, sh, sw, dst, dst_table, dh, dw);
-    count_launch();
-    return cudaGetLastError() != cudaSuccess;
-}
-
-int launch_halve_pages(const uint8_t* src, int n, int sh, int sw, uint8_t* dst, int dh, int dw, cudaStream_t st) {
-    return halve(src, nullptr, n, sh, sw, dst, nullptr, dh, dw, (long long)dh * dw, st);
+    if (idx >= b.H * b.W) return;
+    const int y = idx / b.W;
+    halve_pixel(src + a.page_off, a.W, a.H, idx - y * b.W, y, dst + b.page_off + (long long)idx * 3);
 }
 
 int launch_halve_pages_table(const uint8_t* src, const RtSrc* src_table_dev, int n, uint8_t* dst,
                              const RtSrc* dst_table_dev, long long max_dst_pixels, cudaStream_t st) {
-    return halve(src, src_table_dev, n, 0, 0, dst, dst_table_dev, 0, 0, max_dst_pixels, st);
+    if (n <= 0 || max_dst_pixels <= 0) return 0;
+    if (n > 65535 || max_dst_pixels > INT_MAX) return 1;
+    halve_pages_kernel<<<dim3((unsigned)((max_dst_pixels + 255) / 256), (unsigned)n), 256, 0, st>>>(
+        src, src_table_dev, dst, dst_table_dev);
+    count_launch();
+    return cudaGetLastError() != cudaSuccess;
 }
 
-static int extract(const uint8_t* pages, const RtSrc* table, int H0, int W0, const CropGeom* geoms_dev, int n_crops,
-                   uint8_t* scratch, uint8_t* canvases, cudaStream_t st) {
+int launch_extract_crops_table(const uint8_t* pages, const RtSrc* table_dev, const CropGeom* geoms_dev, int n_crops,
+                               uint8_t* scratch, uint8_t* canvases, cudaStream_t st) {
     if (n_crops <= 0) return 0;
-    crop_warp_kernel<<<dim3((unsigned)n_crops, kWarpSlices), kWarpThreads, 0, st>>>(pages, table, H0, W0, geoms_dev,
+    crop_warp_kernel<<<dim3((unsigned)n_crops, kWarpSlices), kWarpThreads, 0, st>>>(pages, table_dev, geoms_dev,
                                                                                     scratch);
     count_launch();
     if (cudaGetLastError() != cudaSuccess) return 1;
@@ -119,16 +94,6 @@ static int extract(const uint8_t* pages, const RtSrc* table, int H0, int W0, con
                                                                                           canvases);
     count_launch();
     return cudaGetLastError() != cudaSuccess;
-}
-
-int launch_extract_crops(const uint8_t* pages, int H0, int W0, const CropGeom* geoms_dev, int n_crops,
-                         uint8_t* scratch, uint8_t* canvases, cudaStream_t st) {
-    return extract(pages, nullptr, H0, W0, geoms_dev, n_crops, scratch, canvases, st);
-}
-
-int launch_extract_crops_table(const uint8_t* pages, const RtSrc* table_dev, const CropGeom* geoms_dev, int n_crops,
-                               uint8_t* scratch, uint8_t* canvases, cudaStream_t st) {
-    return extract(pages, table_dev, 0, 0, geoms_dev, n_crops, scratch, canvases, st);
 }
 
 }  // namespace ytk

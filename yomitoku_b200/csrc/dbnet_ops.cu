@@ -119,21 +119,16 @@ struct AreaUpSampler {
     }
 };
 
-// Page img of the launch: from the page table when there is one, else page img of a same-size [n][H0][W0][3] batch.
-__global__ void preprocess_kernel(const uint8_t* __restrict__ src, const RtSrc* __restrict__ table, int H0, int W0,
-                                  int Hn, int Wn, op_t* __restrict__ dst) {
+// Page img of the launch is table[img] of `src`.
+__global__ void preprocess_kernel(const uint8_t* __restrict__ src, const RtSrc* __restrict__ table, int Hn, int Wn,
+                                  op_t* __restrict__ dst) {
     const int Hp = Hn + 6, Wp = Wn + 8;
     const int img = blockIdx.y;
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= Hp * Wp) return;
-    const uint8_t* page = src + (size_t)img * H0 * W0 * 3;
-    int H = H0, W = W0;
-    if (table) {
-        const RtSrc p = table[img];
-        page = src + p.page_off;
-        H = p.H;
-        W = p.W;
-    }
+    const RtSrc p = table[img];
+    const uint8_t* page = src + p.page_off;
+    const int H = p.H, W = p.W;
     const int wp = idx % Wp;
     const int hp = idx / Wp;
     float o[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -153,23 +148,14 @@ __global__ void preprocess_kernel(const uint8_t* __restrict__ src, const RtSrc* 
     reinterpret_cast<uint4*>(dst)[(size_t)img * Hp * Wp + idx] = pack8(o);
 }
 
-static int preprocess(const uint8_t* src, const RtSrc* table, int n_img, int H0, int W0, int Hn, int Wn, void* dst,
-                      cudaStream_t st) {
+int launch_preprocess_table(const uint8_t* pages, const RtSrc* table_dev, int n_img, int Hn, int Wn, void* dst,
+                            cudaStream_t st) {
     if (n_img < 1 || n_img > 65535) return 1;  // one page per blockIdx.y
     const int threads = 256;
     const dim3 grid((unsigned)(((long long)(Hn + 6) * (Wn + 8) + threads - 1) / threads), (unsigned)n_img);
-    preprocess_kernel<<<grid, threads, 0, st>>>(src, table, H0, W0, Hn, Wn, reinterpret_cast<op_t*>(dst));
+    preprocess_kernel<<<grid, threads, 0, st>>>(pages, table_dev, Hn, Wn, reinterpret_cast<op_t*>(dst));
     count_launch();
     return cudaGetLastError() != cudaSuccess;
-}
-
-int launch_preprocess(const uint8_t* src, int n_img, int H0, int W0, int Hn, int Wn, void* dst, cudaStream_t st) {
-    return preprocess(src, nullptr, n_img, H0, W0, Hn, Wn, dst, st);
-}
-
-int launch_preprocess_table(const uint8_t* pages, const RtSrc* table_dev, int n_img, int Hn, int Wn, void* dst,
-                            cudaStream_t st) {
-    return preprocess(pages, table_dev, n_img, 0, 0, Hn, Wn, dst, st);
 }
 
 // Model-level seam: the reference hands DBNet a normalised (N,3,H,W) fp32 tensor (text_detector.py:127-129).  Repack

@@ -17,7 +17,7 @@ from concurrent.futures import ProcessPoolExecutor
 import numpy as np
 
 from .data import CROP_GEOM_DTYPE, ParseqDataset, crop_records, page_table
-from .models import dbnet_post_front, device_pages
+from .models import dbnet_post_front
 from .postprocessor import DBnetPostProcessor
 from .schemas import OCRSchema
 from .text_recognizer import plan_mini_batches
@@ -697,7 +697,7 @@ class BatchedOCR:
 
     def _run_groups_dev_local(self, groups, geoms, pages_dev, stream=None, levels=None, plan=None):
         """This rank's share of `_run_groups_dev`: the canvases of a <= max_tokens chunk are cut on the device
-        (ytk_extract_crops_u8, one call per source_downscale pyramid level) in group order and go to PARSeq without
+        (ytk_extract_crops_table_u8, one call per source_downscale pyramid level) in group order and go to PARSeq without
         leaving HBM.  `plan` = `_plan_groups_dev(groups, geoms, levels)` when it was prepared ahead of time."""
         from .models import extract_crops_pyramid
         pages = pages_dev if isinstance(pages_dev, dict) else {0: pages_dev}
@@ -959,8 +959,7 @@ class BatchedOCR:
                            arena.desc(i * cap, (cap,), np.uint8))
                 futs[i] = _Done(_host_stage(job)) if pool is None else pool.submit(_host_stage, job)
         if pages_dev is not None:
-            # what the crop kernels read: the (n, H, W, 3) view of a same-size batch, else (flat buffer, page table)
-            pages_dev = device_pages(pages_dev, plan.table)
+            pages_dev = (pages_dev, plan.table)     # what the crop kernels read
         if pool is None:
             return _Handle(futs, None, 0, pages_dev)
         handle = _Handle(futs, arena, cap, pages_dev)

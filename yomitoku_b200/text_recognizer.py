@@ -203,7 +203,7 @@ class TextRecognizer(BaseModule):
 
     def _run_records(self, pages, sel, levels, padded, group, n_groups):
         """Cuts the crops of the records `sel` (already in packing order) on the GPU and runs them as one packed call.
-        pages[k] = the page at pyramid level k (cuda tensor), levels[r] = level of record r; padded[r] / group[r] =
+        pages[k] = the page at pyramid level k (models.extract_crops_pyramid), levels[r] = level of record r; padded[r] / group[r] =
         padded width and mini-batch index of record r.  Returns (ids, probs) with the positions a `refine_iters == 0`
         model never produced filled like the host path does."""
         from . import _lib, models
