@@ -399,6 +399,25 @@ int ytk_halve_pages_table_u8(const uint8_t* src_dev, long long src_bytes, const 
                              uint8_t* dst_dev, long long dst_bytes, const ytk_page* dst_table, uint8_t* scratch_dev,
                              long long scratch_bytes, void* cuda_stream);
 
+/* ---- Pages that are already on the device (a GPU JPEG decode, video frames, an earlier model's output): each source
+ * page is an H x W x 3 uint8 array with arbitrary non-negative byte strides, so a contiguous HWC page, a crop or a step
+ * of one and the permute(1, 2, 0) of a CHW tensor all go in without a copy. ---- */
+typedef struct {
+    const uint8_t* data;   /* device pointer of pixel (0, 0), channel 0 */
+    long long sh, sw, sc;  /* byte strides of a row, a column and a channel (>= 0) */
+    int H, W;              /* page size (>= 1) */
+    int rgb;               /* channel order of the source: 0 = B, G, R (the pages of this API); 1 = R, G, B */
+    int pad_;
+} ytk_page_src;            /* 48 bytes */
+
+/* Packs n source pages into the page-table buffer dst_dev: page i is written as H x W x 3 BGR bytes at
+ * table[i].page_off (table[i] must be the whole page, of the source's size).  The copy is exact.  srcs / table: host
+ * arrays (pageable: reusable as soon as the call returns); every source and dst_dev on the same device; scratch_dev
+ * holds the uploaded records: scratch_bytes >= n * (sizeof(ytk_page_src) + sizeof(ytk_page)).  Asynchronous on
+ * cuda_stream: one H2D copy + one kernel launch, nothing allocated; invalid records are an error, not a launch. */
+int ytk_pack_pages_u8(const ytk_page_src* srcs, int n, uint8_t* dst_dev, long long dst_bytes, const ytk_page* table,
+                      uint8_t* scratch_dev, long long scratch_bytes, void* cuda_stream);
+
 /* The reference's whole input path on the device: per record, the rectangle as RGB,
  * Image.fromarray(rgb_crop).resize((img, img), Image.BILINEAR) bit for bit (Pillow's fixed-point separable resample,
  * horizontal pass first) and ToTensor, then the forward of ytk_rtdetr_forward_f32 with the same outputs, ordering and

@@ -6,8 +6,10 @@
 The constructors, the `configs` dict and the call contracts mirror kotaro-kinoshita/yomitoku
 (src/yomitoku/{text_detector,text_recognizer,ocr,document_analyzer,layout_parser,table_structure_recognizer,
 layout_analyzer,table_cell_detector}.py); the models (DBNet++, PARSeq, RT-DETRv2) run as hand-written sm_90a CUDA kernels behind the C ABI
-in include/yomitoku_b200.h (libytk_b200.so).
+in include/yomitoku_b200.h (libytk_b200.so).  Pages may be BGR numpy arrays or already on the GPU: uint8 CUDA tensors or
+a `DevicePages` made by `device_pages` (device_pages.py).
 """
+from .device_pages import DevicePages, device_pages
 from .document_analyzer import DocumentAnalyzer
 from .layout_analyzer import LayoutAnalyzer
 from .layout_parser import LayoutParser
@@ -18,4 +20,4 @@ from .text_detector import TextDetector
 from .text_recognizer import TextRecognizer
 
 __all__ = ["OCR", "TextDetector", "TextRecognizer", "DocumentAnalyzer", "LayoutAnalyzer", "LayoutParser",
-           "TableStructureRecognizer", "CellDetector"]
+           "TableStructureRecognizer", "CellDetector", "DevicePages", "device_pages"]

@@ -172,6 +172,8 @@ def _declare_crops(lib):
     lib.ytk_halve_pages_table_u8.restype = c_int
     lib.ytk_halve_pages_table_u8.argtypes = [c_void_p, c_ll, c_void_p, c_int, c_void_p, c_ll, c_void_p, c_void_p, c_ll,
                                              c_void_p]
+    lib.ytk_pack_pages_u8.restype = c_int
+    lib.ytk_pack_pages_u8.argtypes = [c_void_p, c_int, c_void_p, c_ll, c_void_p, c_void_p, c_ll, c_void_p]
 
 
 class YtkRtdetrSrc(ctypes.Structure):

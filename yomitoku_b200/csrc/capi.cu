@@ -18,6 +18,7 @@
 #include "dbnet_ops.h"
 #include "dbpost_ops.h"
 #include "gemm_tc.h"
+#include "page_ops.h"
 #include "parseq_engine.h"
 #include "resample_ops.h"
 #include "rtdetr_engine.h"
@@ -1047,6 +1048,73 @@ int ytk_halve_pages_table_u8(const uint8_t* src_dev, long long src_bytes, const 
     }
     const ytk::RtSrc* tabs = reinterpret_cast<const ytk::RtSrc*>(scratch_dev);
     if (ytk::launch_halve_pages_table(src_dev, tabs, n_pages, dst_dev, tabs + n_pages, max_pixels, st)) {
+        ytk::set_error("%s: kernel launch failed", who);
+        return YTK_ERR;
+    }
+    return YTK_OK;
+}
+
+static_assert(sizeof(ytk_page_src) == 48 && sizeof(ytk_page_src) == sizeof(ytk::PageSrc) &&
+                  offsetof(ytk_page_src, H) == offsetof(ytk::PageSrc, H) &&
+                  offsetof(ytk_page_src, rgb) == offsetof(ytk::PageSrc, rgb),
+              "ytk_page_src and ytk::PageSrc must have one layout");
+
+int ytk_pack_pages_u8(const ytk_page_src* srcs, int n, uint8_t* dst_dev, long long dst_bytes, const ytk_page* table,
+                      uint8_t* scratch_dev, long long scratch_bytes, void* cuda_stream) {
+    const char* who = "ytk_pack_pages_u8";
+    if (!srcs || !dst_dev || !scratch_dev) {
+        ytk::set_error("%s: null argument", who);
+        return YTK_ERR;
+    }
+    if (check_page_table(table, n, dst_bytes, true, who)) return YTK_ERR;
+    cudaPointerAttributes attr;
+    if (cudaPointerGetAttributes(&attr, dst_dev) != cudaSuccess || attr.type != cudaMemoryTypeDevice) {
+        cudaGetLastError();
+        ytk::set_error("%s: dst_dev is not a device pointer", who);
+        return YTK_ERR;
+    }
+    const int device = attr.device;
+    long long max_pixels = 0;
+    for (int i = 0; i < n; ++i) {
+        const ytk_page_src& s = srcs[i];
+        if (!s.data || s.H < 1 || s.W < 1 || s.sh < 0 || s.sw < 0 || s.sc < 0 || (s.rgb != 0 && s.rgb != 1)) {
+            ytk::set_error("%s: source %d (%dx%d, strides %lld/%lld/%lld, rgb %d) is empty, has a negative stride or "
+                           "an unknown channel order", who, i, s.H, s.W, s.sh, s.sw, s.sc, s.rgb);
+            return YTK_ERR;
+        }
+        if (table[i].H != s.H || table[i].W != s.W) {
+            ytk::set_error("%s: source %d is %dx%d, its page record %dx%d", who, i, s.H, s.W, table[i].H, table[i].W);
+            return YTK_ERR;
+        }
+        cudaPointerAttributes a;
+        if (cudaPointerGetAttributes(&a, s.data) != cudaSuccess || a.type != cudaMemoryTypeDevice ||
+            a.device != device) {
+            cudaGetLastError();
+            ytk::set_error("%s: source %d is not in device memory of device %d (the device of dst_dev)", who, i, device);
+            return YTK_ERR;
+        }
+        max_pixels = std::max(max_pixels, (long long)s.H * s.W);
+    }
+    const long long src_bytes = (long long)n * (long long)sizeof(ytk_page_src);
+    const long long tab_bytes = (long long)n * (long long)sizeof(ytk_page);
+    if (scratch_bytes < src_bytes + tab_bytes) {
+        ytk::set_error("%s: scratch_dev holds %lld bytes, need %lld (source records) + %lld (page table)", who,
+                       scratch_bytes, src_bytes, tab_bytes);
+        return YTK_ERR;
+    }
+    DevGuard dev_guard(device);
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    std::vector<uint8_t> blob((size_t)(src_bytes + tab_bytes));
+    memcpy(blob.data(), srcs, (size_t)src_bytes);
+    memcpy(blob.data() + src_bytes, table, (size_t)tab_bytes);
+    cudaError_t err = cudaMemcpyAsync(scratch_dev, blob.data(), blob.size(), cudaMemcpyHostToDevice, st);
+    if (err != cudaSuccess) {
+        ytk::set_error("%s: record upload failed: %s", who, cudaGetErrorString(err));
+        return YTK_ERR;
+    }
+    const ytk::PageSrc* dev_srcs = reinterpret_cast<const ytk::PageSrc*>(scratch_dev);
+    const ytk::RtSrc* dev_tab = reinterpret_cast<const ytk::RtSrc*>(scratch_dev + src_bytes);
+    if (ytk::launch_pack_pages(dev_srcs, dev_tab, n, max_pixels, dst_dev, st)) {
         ytk::set_error("%s: kernel launch failed", who);
         return YTK_ERR;
     }

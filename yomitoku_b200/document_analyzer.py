@@ -21,6 +21,7 @@ from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
+from .device_pages import DevicePages, as_device_pages, single_page
 from .ocr import ocr_aggregate
 from .reading_order import prediction_reading_order
 from .schemas import (DocumentAnalyzerSchema, FigureSchema, LayoutAnalyzerSchema, OCRSchema, ParagraphSchema,
@@ -421,12 +422,22 @@ class DocumentAnalyzer:
     def _layout(self, img):
         if self.layout is None:
             return _empty_layout(), None
+        if isinstance(img, DevicePages) and not self._layout_takes_device_pages():
+            img = img.numpy(0)          # a layout analyzer of the reference's protocol: numpy pages
         return self.layout(img)
+
+    def _layout_takes_device_pages(self):
+        from .layout_analyzer import LayoutAnalyzer
+        return isinstance(self.layout, LayoutAnalyzer)
 
     def __call__(self, img):
         """(DocumentAnalyzerSchema, ocr_vis, layout_vis) like the reference (:603-678): detection -> recognition in one
         worker thread, the layout analyzer in another; with split_text_across_cells the recognizer waits for the layout
-        because its crops are the detected lines cut at the cell borders."""
+        because its crops are the detected lines cut at the cell borders.  img: BGR page (numpy, or on the GPU: a CUDA
+        (H, W, 3) uint8 tensor or a one-page DevicePages, packed once and read by both halves)."""
+        dp = as_device_pages(img)
+        if dp is not None:
+            img = single_page(dp, "DocumentAnalyzer")
         with ThreadPoolExecutor(max_workers=2) as ex:
             if self.split_text_across_cells:
                 f_det = ex.submit(self.text_detector, img)
@@ -439,7 +450,7 @@ class DocumentAnalyzer:
                 f_lay = ex.submit(self._layout, img)
                 (det, rec, ocr_vis), (layout, layout_vis) = f_ocr.result(), f_lay.result()
         ocr = OCRSchema(words=ocr_aggregate(det, rec))
-        return DocumentAnalyzerSchema(**self.aggregate(ocr, layout, img)), ocr_vis, layout_vis
+        return DocumentAnalyzerSchema(**self.aggregate(ocr, layout, None if dp is not None else img)), ocr_vis, layout_vis
 
     # -------------------------------------------------------------------------------------- many pages
     def analyze_pages(self, pages, layouts=None):
@@ -448,13 +459,21 @@ class DocumentAnalyzer:
         host post-processing in the process pool) while the layout analyzer works through the pages in a thread pool;
         then `aggregate` per page.  `layouts` (optional list of LayoutAnalyzerSchema) replaces the layout analyzer.
         With split_text_across_cells the detected lines are cut at the cell borders between the two device stages.
+        Pages already on the GPU (a list of CUDA (H, W, 3) uint8 tensors, an (n, H, W, 3) CUDA tensor or a DevicePages)
+        are packed once: the OCR half and the layout half read the same buffer.
         Returns a list of DocumentAnalyzerSchema."""
         from .pipeline import BatchedOCR
         if self._batched is None:
             self._batched = BatchedOCR(self.text_detector, self.text_recognizer)
         ocr = self._batched
-        with ThreadPoolExecutor(max_workers=max(1, min(4, len(pages)))) as ex:
-            if layouts is None and hasattr(self.layout, "analyze_pages"):
+        dp = as_device_pages(pages)
+        if dp is not None:
+            pages = dp
+        n = len(pages)
+        with ThreadPoolExecutor(max_workers=max(1, min(4, n))) as ex:
+            if layouts is None and dp is not None and not self._layout_takes_device_pages():
+                f_lay = [ex.submit(self._layout, dp.select(i)) for i in range(n)]
+            elif layouts is None and hasattr(self.layout, "analyze_pages"):
                 # the built-in LayoutAnalyzer: all pages' layouts in one device batch (its own thread: the OCR stages
                 # below run meanwhile)
                 f_all = ex.submit(self.layout.analyze_pages, pages)
@@ -465,7 +484,7 @@ class DocumentAnalyzer:
 
                     def result(self):
                         return f_all.result()[self.i], None
-                f_lay = [_One(i) for i in range(len(pages))]
+                f_lay = [_One(i) for i in range(n)]
             elif layouts is None:
                 f_lay = [ex.submit(self._layout, p) for p in pages]
             if self.split_text_across_cells:
@@ -479,4 +498,5 @@ class DocumentAnalyzer:
             else:
                 results = ocr(pages)
                 lay = layouts if layouts is not None else [f.result()[0] for f in f_lay]
-        return [DocumentAnalyzerSchema(**self.aggregate(r, l, p)) for r, l, p in zip(results, lay, pages)]
+        imgs = [None] * n if dp is not None else pages        # aggregate reads boxes only, never the pixels
+        return [DocumentAnalyzerSchema(**self.aggregate(r, l, p)) for r, l, p in zip(results, lay, imgs)]

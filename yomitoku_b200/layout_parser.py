@@ -15,6 +15,7 @@ from PIL import Image
 from . import _lib
 from .base import BaseModelCatalog, BaseModule, logger
 from .config import LayoutParserRTDETRv2Config, LayoutParserRTDETRv2V2Config
+from .device_pages import DevicePages, as_device_pages, host_page, require_device, single_page
 from .document_analyzer import is_contained
 from .models import RTDETRv2
 from .postprocessor import RTDETRPostProcessor
@@ -114,9 +115,17 @@ def rtdetr_device_forward(model, pages, boxes, pages_dev=None):
     index, box) of the BGR u8 `pages`, resized on the device, and the crop sizes.  pages_dev: those pages as
     upload_pages made them (shared with another model), else they are uploaded here.  None when the device path does
     not apply (upload_pages, rtdetr_sources): the caller then runs `model(torch.cat(preprocess(...)))`, which gives the
-    same bits."""
+    same bits.  `pages` may be a DevicePages: its buffer is read, nothing is uploaded (pages on another device than the
+    model raise ValueError); on None the caller downloads the pages for the host path (device_pages.host_page)."""
     if model._device.type != "cuda" or not torch.cuda.is_available():
         return None
+    if isinstance(pages, DevicePages):
+        require_device(pages, model.cuda_device(), type(model).__name__)
+        src = rtdetr_sources(pages.shapes, boxes)
+        if src is None:
+            return None
+        preds = model.forward_u8(pages.ready().buf, src[0])
+        return {k: v.cpu() for k, v in preds.items()}, src[1]
     src = rtdetr_sources([p.shape for p in pages], boxes)
     if src is None:
         return None
@@ -174,19 +183,32 @@ class LayoutParser(BaseModule):
         return filter_contained_rectangles_across_categories(by_category, "tables", "paragraphs")
 
     def __call__(self, img, pages_dev=None):
-        """pages_dev (optional): `img` already on the device as upload_pages([img], ...) made it."""
-        results = self.parse_pages([img], pages_dev)[0]
-        vis = layout_visualizer(results, img) if self.visualize else None
+        """img: BGR page (numpy, or on the GPU: a CUDA (H, W, 3) uint8 tensor or a one-page DevicePages).  pages_dev
+        (optional, numpy pages): `img` already on the device as upload_pages([img], ...) made it."""
+        dp = as_device_pages(img)
+        if dp is not None:
+            img = single_page(dp, "LayoutParser")
+        results = self.parse_pages(img if dp is not None else [img], pages_dev)[0]
+        vis = layout_visualizer(results, host_page(img)) if self.visualize else None
         return results, vis
 
     def parse_pages(self, pages, pages_dev=None):
         """Batched entry (new surface): list of BGR pages (any sizes) -> list of LayoutParserSchema; one device call.
         On a CUDA device the pages go up once as u8 (or are read from pages_dev, upload_pages(pages, ...)) and are
-        resized there; otherwise they are preprocessed on the host."""
-        whole = [(i, (0, 0, p.shape[1], p.shape[0])) for i, p in enumerate(pages)]
+        resized there; otherwise they are preprocessed on the host.  Pages already on the GPU (CUDA tensors or a
+        DevicePages) are read where they are."""
+        dp = as_device_pages(pages)
+        if dp is not None:
+            pages = dp
+        shapes = dp.shapes if dp is not None else [p.shape[:2] for p in pages]
+        whole = [(i, (0, 0, w, h)) for i, (h, w) in enumerate(shapes)]
         dev = rtdetr_device_forward(self.model, pages, whole, pages_dev)
-        preds = dev[0] if dev is not None else self.model(torch.cat([self.preprocess(p) for p in pages]))
-        return [self.postprocess({k: v[i:i + 1] for k, v in preds.items()}, p.shape[:2]) for i, p in enumerate(pages)]
+        if dev is None:
+            host = [host_page(pages, i) for i in range(len(shapes))] if dp is not None else pages
+            preds = self.model(torch.cat([self.preprocess(p) for p in host]))
+        else:
+            preds = dev[0]
+        return [self.postprocess({k: v[i:i + 1] for k, v in preds.items()}, s) for i, s in enumerate(shapes)]
 
 
 _PALETTE = {"paragraphs": (0, 200, 0), "tables": (200, 0, 0), "figures": (0, 0, 200)}

@@ -3,6 +3,7 @@
 `"text_detector"` and a `"text_recognizer"` dict of constructor overrides (anything but a dict raises ValueError), and
 `ocr(img) -> (OCRSchema, vis)`.  `ocr_aggregate` pairs detections with recognitions positionally - with a quad dropped
 by the recognizer the lists mis-align exactly as in the reference (SURVEY.md section 8b, error conventions)."""
+from .device_pages import as_device_pages
 from .schemas import OCRSchema
 from .text_detector import TextDetector
 from .text_recognizer import TextRecognizer
@@ -25,7 +26,11 @@ class OCR:
         self.recognizer = TextRecognizer(**{**common, **configs.get("text_recognizer", {})})
 
     def __call__(self, img):
-        """img: BGR page (numpy).  Returns (OCRSchema, visualisation or None)."""
+        """img: BGR page (numpy, or on the GPU: a CUDA (H, W, 3) uint8 tensor or a one-page DevicePages, packed once and
+        read by both modules).  Returns (OCRSchema, visualisation or None)."""
+        dp = as_device_pages(img)
+        if dp is not None:
+            img = dp
         detected, vis = self.detector(img)
         recognized, vis = self.recognizer(img, detected.points, vis=vis)
         return OCRSchema(words=ocr_aggregate(detected, recognized)), vis

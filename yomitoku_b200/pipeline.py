@@ -17,6 +17,7 @@ from concurrent.futures import ProcessPoolExecutor
 import numpy as np
 
 from .data import CROP_GEOM_DTYPE, ParseqDataset, crop_records, page_table
+from .device_pages import as_device_pages, require_device
 from .models import dbnet_post_front
 from .postprocessor import DBnetPostProcessor
 from .schemas import OCRSchema
@@ -353,20 +354,28 @@ class BatchedOCR:
         without a copy; `self._last_shared` then holds the two buffers."""
         import torch
         plan = BatchPlan([p.shape[:2] for p in pages], self.detector.model.input_size, self.det_batch)
-        self._last_shared = None
+        out, ob = self._prob_out(plan, shared)
         if shared:
             pb = self._shared("pages", plan.page_bytes)
-            ob = self._shared("prob", plan.prob_len * 4)
             with _span("detect.stage_pages"):
                 for (h, w), off, p in zip(plan.shapes, plan.table["page_off"], pages):
                     np.copyto(pb.view(int(off), (h, w, 3), np.uint8), p)
             stage = pb.torch[:plan.page_bytes]
-            out = ob.torch[:plan.prob_len * 4].view(torch.float32)
             self._last_shared = (pb, ob)
         else:
             stage = torch.from_numpy(np.concatenate([np.ascontiguousarray(p).reshape(-1) for p in pages]))
-            out = torch.empty(plan.prob_len, dtype=torch.float32)
         return stage, out, plan
+
+    def _prob_out(self, plan, shared):
+        """The host buffer of a batch's probability maps (flat f32 tensor) and, with `shared`, the ring buffer holding it
+        (`self._last_shared` is then (pages buffer or None, that buffer))."""
+        import torch
+        self._last_shared = None
+        if shared:
+            ob = self._shared("prob", plan.prob_len * 4)
+            self._last_shared = (None, ob)
+            return ob.torch[:plan.prob_len * 4].view(torch.float32), ob
+        return torch.empty(plan.prob_len, dtype=torch.float32), None
 
     def _detect_chunk(self, stage, plan, chunk, maps, stream=None):
         """One detector call: the chunk's pages of the flat stage (host or device) -> maps (n, Hn, Wn)."""
@@ -886,13 +895,23 @@ class BatchedOCR:
                         self._slot_busy[self._slot] = prev
                         self._slot = self._ring
                         self._ring += 1
-        n = len(pages)
-        stage, out, plan = self._stage(pages, shared=pool is not None)
+        dp = as_device_pages(pages)
+        if dp is not None:
+            # pages already in HBM: no staging copy and no upload; the packed buffer is what the detector and the crop
+            # kernels read, so the host stage sees page shapes only (the device-crops jobs)
+            require_device(dp, self.detector.model.cuda_device(), "BatchedOCR")
+            dp.ready(stream)
+            plan = BatchPlan(dp.shapes, self.detector.model.input_size, self.det_batch)
+            stage, pages_dev = None, dp.buf
+            out, _ = self._prob_out(plan, shared=pool is not None)
+        else:
+            stage, out, plan = self._stage(pages, shared=pool is not None)
+            pages_dev = None
+        n = len(plan.shapes)
         prob = out.numpy()
         sh = self._last_shared if pool is not None else None
         arena, cap = None, self.crop_cap
-        pages_dev = None
-        if self.device_crops or getattr(self.recognizer, "rec_orientation_fallback", False):
+        if pages_dev is None and (self.device_crops or getattr(self.recognizer, "rec_orientation_fallback", False)):
             # (the orientation fallback's second look is implemented on the device-crops path only: its crops are the
             # same records with one bit set, no rectified images have to come back from the workers)
             # the pages stay in HBM for the crop kernels of this batch; the tensor belongs to the handle (no ring slot
@@ -943,9 +962,8 @@ class BatchedOCR:
                 if runs[j] is not None:
                     job = (("shape", h0, w0), _Runs(runs[j], hn, wn), qo, None, "geom")
                 elif sh is None:
-                    job = (pages[i], pm if (prob_override is None or dev_post) else prob_override[i], qo)
-                    if pages_dev is not None:
-                        job = (("shape", h0, w0), job[1], qo, None, "geom")
+                    pm_in = pm if (prob_override is None or dev_post) else prob_override[i]
+                    job = (pages[i], pm_in, qo) if pages_dev is None else (("shape", h0, w0), pm_in, qo, None, "geom")
                 elif pages_dev is not None:
                     if prob_override is not None and not dev_post:
                         np.copyto(pm, prob_override[i])
@@ -1147,7 +1165,9 @@ class BatchedOCR:
         return _stream_impl(self, batches, lookahead, prob_override, quads_override)
 
     def __call__(self, pages, prob_override=None, quads_override=None):
-        """pages: list of BGR uint8 arrays, of one size or of many.  prob_override / quads_override (benchmarks with random
+        """pages: list of BGR uint8 arrays, of one size or of many, or pages already on the GPU (a list of CUDA (H, W, 3)
+        uint8 tensors, an (n, H, W, 3) CUDA tensor or a DevicePages: no host staging and no upload, the detector and the
+        crop kernels read the packed buffer).  prob_override / quads_override (benchmarks with random
         detector weights): the detector still runs, but post-processing sees the given probability maps / the
         recognizer the given quads."""
         return self.collect(self.submit(pages, prob_override, quads_override))
@@ -1168,6 +1188,9 @@ def _stream_impl(ocr, batches, lookahead, prob_override, quads_override):
     q = queue.Queue(maxsize=max(1, lookahead))
     err = []
     dev = torch.cuda.current_device() if torch.cuda.is_available() else None
+    # CUDA tensor pages are packed on the caller's current stream (device_pages), which the producer thread does not
+    # inherit
+    caller_stream = torch.cuda.current_stream() if torch.cuda.is_available() else None
 
     def producer():
         try:
@@ -1177,6 +1200,10 @@ def _stream_impl(ocr, batches, lookahead, prob_override, quads_override):
             for k, pages in enumerate(batches):
                 with _span("producer.next_batch"):
                     pass
+                if caller_stream is not None:
+                    with torch.cuda.stream(caller_stream):
+                        dp = as_device_pages(pages)
+                    pages = pages if dp is None else dp
                 po = None if prob_override is None else prob_override[k]
                 qo = None if quads_override is None else quads_override[k]
                 q.put(ocr.submit(pages, po, qo, stream=det_stream, wait_recognized=True))

@@ -14,6 +14,7 @@ import torch
 
 from .base import BaseModelCatalog, BaseModule, logger
 from .config import TableCellParserRTDETRv2Config, load_config
+from .device_pages import as_device_pages, single_page
 from .document_analyzer import calc_iou, is_bottom_adjacent, is_contained, is_right_adjacent
 from .layout_parser import _area, filter_contained_rectangles_across_categories, rtdetr_device_forward, rtdetr_input_tensor
 from .models import RTDETRv2
@@ -220,17 +221,20 @@ class CellDetector(BaseModule):
         return cells
 
     def __call__(self, img, tables):
-        """BGR page + the layout parser's tables -> List[TableDetectorSchema], tables without cells left out."""
+        """BGR page (numpy, or on the GPU: a CUDA (H, W, 3) uint8 tensor or a one-page DevicePages) + the layout
+        parser's tables -> List[TableDetectorSchema], tables without cells left out."""
         outputs = []
         if not tables:
             return outputs
+        dp = as_device_pages(img)
         # every table of the page in one batch, resized on the device when rtdetr_device_forward applies
         boxes = [[int(v) for v in table.box] for table in tables]
-        dev = rtdetr_device_forward(self.model, [img], [(0, b) for b in boxes])
+        pages = [img] if dp is None else single_page(dp, "CellDetector")
+        dev = rtdetr_device_forward(self.model, pages, [(0, b) for b in boxes])
         if dev is not None:
             preds, data = dev[0], [{"size": s, "offset": (b[0], b[1])} for s, b in zip(dev[1], boxes)]
         else:
-            data = self.preprocess(img, tables)
+            data = self.preprocess(img if dp is None else dp.numpy(0), tables)
             preds = self.model(torch.cat([d["tensor"] for d in data]))
         for i, (d, table) in enumerate(zip(data, tables)):
             cells, kv_regions, grid_regions = self.postprocess({k: v[i:i + 1] for k, v in preds.items()}, d, table.box)

@@ -11,6 +11,7 @@ import torch
 
 from .base import BaseModelCatalog, BaseModule, logger
 from .config import TableStructureRecognizerRTDETRv2Config
+from .device_pages import DevicePages, as_device_pages, host_page, single_page
 from .document_analyzer import _intersection, is_contained
 from .layout_parser import filter_contained_rectangles_within_category, rtdetr_device_forward, rtdetr_input_tensor
 from .models import RTDETRv2
@@ -105,14 +106,19 @@ class TableStructureRecognizer(BaseModule):
         """(outputs on the host, per table {"size", "offset"}) for every table of the page in one batch: resized on the
         device when rtdetr_device_forward applies, else `preprocess` on the host."""
         boxes = [[int(v) for v in box] for box in table_boxes]
-        dev = rtdetr_device_forward(self.model, [img], [(0, b) for b in boxes], pages_dev)
+        pages = img if isinstance(img, DevicePages) else [img]
+        dev = rtdetr_device_forward(self.model, pages, [(0, b) for b in boxes], pages_dev)
         if dev is not None:
             return dev[0], [{"size": s, "offset": (b[0], b[1])} for s, b in zip(dev[1], boxes)]
-        data = self.preprocess(img, table_boxes)
+        data = self.preprocess(host_page(img), table_boxes)
         return self.model(torch.cat([d["tensor"] for d in data])), data
 
     def __call__(self, img, table_boxes, vis=None, pages_dev=None):
-        """pages_dev (optional): `img` already on the device as upload_pages([img], ...) made it."""
+        """img: BGR page (numpy, or on the GPU: a CUDA (H, W, 3) uint8 tensor or a one-page DevicePages).  pages_dev
+        (optional, numpy pages): `img` already on the device as upload_pages([img], ...) made it."""
+        dp = as_device_pages(img)
+        if dp is not None:
+            img = single_page(dp, "TableStructureRecognizer")
         outputs = []
         if len(table_boxes):
             preds, data = self._infer(img, table_boxes, pages_dev)
@@ -121,7 +127,7 @@ class TableStructureRecognizer(BaseModule):
                 if table.n_row > 0 and table.n_col > 0:
                     outputs.append(table)
         if self.visualize:
-            vis = img.copy() if vis is None else vis
+            vis = host_page(img).copy() if vis is None else vis
             for table in outputs:
                 vis = table_visualizer(vis, table)
         return outputs, vis

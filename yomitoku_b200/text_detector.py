@@ -14,6 +14,7 @@ import torch
 from .base import BaseModelCatalog, BaseModule, logger
 from .config import TextDetectorDBNetConfig, TextDetectorDBNetV2_1Config, TextDetectorDBNetV2Config
 from .data import array_to_tensor, resize_shortest_edge, standardization_image
+from .device_pages import as_device_pages, host_page, require_device, single_page
 from .models import DBNet
 from .postprocessor import DBnetPostProcessor
 from .schemas import TextDetectorSchema
@@ -96,31 +97,62 @@ class TextDetector(BaseModule):
         prob = self.model.detect_pages_u8(np.ascontiguousarray(img))
         return prob.cpu().numpy()[:, None] if prob.is_cuda else prob.numpy()[:, None]
 
+    def _device_input(self, pages, who):
+        """DevicePages for device input (None for host pages), checked against the model's device and made ready for
+        the calls on the default stream."""
+        dp = as_device_pages(pages)
+        if dp is not None:
+            if not self.on_cuda:
+                raise ValueError("%s: pages on %s, the detector is on %s" % (who, dp.device, self.device))
+            require_device(dp, self.model.cuda_device(), who)
+            dp.ready()
+        return dp
+
     def __call__(self, img):
-        """Apply the detection model to a BGR page (np.ndarray HxWx3 u8); returns (TextDetectorSchema, vis)."""
-        ori_h, ori_w = img.shape[:2]
-        if self.device_post:
+        """Apply the detection model to a BGR page (np.ndarray HxWx3 u8, or on the GPU: a CUDA (H, W, 3) uint8 tensor or
+        a one-page DevicePages); returns (TextDetectorSchema, vis)."""
+        dp = self._device_input(img, "TextDetector")
+        if dp is not None:
+            single_page(dp, "TextDetector")
+            quads, scores = self._detect_pages_dev(dp)[0]
+        elif self.device_post:
             quads, scores = self._detect_device(np.ascontiguousarray(img)[None])[0]
         else:
+            ori_h, ori_w = img.shape[:2]
             preds = {"binary": self._probability_map(img)}
             quads, scores = self.postprocess(preds, (ori_h, ori_w))
         results = TextDetectorSchema(points=quads, scores=scores)
         vis = None
         if self.visualize:
-            vis = det_visualizer(img, quads, line_color=tuple(self._cfg.visualize.color[::-1]))
+            vis = det_visualizer(host_page(img if dp is None else dp), quads,
+                                 line_color=tuple(self._cfg.visualize.color[::-1]))
         return results, vis
 
+    def _detect_pages_dev(self, dp):
+        """Pages in HBM -> per page (quads, scores): `detect_pages` with the packed buffer as its input."""
+        return self._detect_flat(dp.buf, dp.shapes)
+
     def detect_pages(self, pages):
-        """Batched entry (new surface, SURVEY.md section 0): list of BGR pages, of one size or of many -> list of
-        TextDetectorSchema.  The pages go to the device back to back with a page table (data.page_table); one device
-        launch sequence per group of pages that share a detector input size (a same-size batch is one group), host
-        post-processing per page."""
+        """Batched entry (new surface, SURVEY.md section 0): list of BGR pages, of one size or of many (or pages on the
+        GPU: CUDA tensors or a DevicePages) -> list of TextDetectorSchema.  The pages go to the device back to back with a
+        page table (data.page_table); one device launch sequence per group of pages that share a detector input size (a
+        same-size batch is one group), host post-processing per page."""
+        dp = self._device_input(pages, "TextDetector.detect_pages")
+        if dp is not None:
+            res = self._detect_pages_dev(dp)
+        else:
+            flat = torch.from_numpy(np.concatenate([np.ascontiguousarray(p).reshape(-1) for p in pages]))
+            if self.device_post:
+                flat = flat.to(self.model.cuda_device(), non_blocking=False)
+            res = self._detect_flat(flat, [p.shape[:2] for p in pages])
+        return [TextDetectorSchema(points=quads, scores=scores) for quads, scores in res]
+
+    def _detect_flat(self, flat, shapes):
+        """Pages of the given shapes back to back in `flat` (host, or the detector's device) -> per page (quads,
+        scores)."""
         from .pipeline import BatchPlan
-        plan = BatchPlan([p.shape[:2] for p in pages], self.model.input_size, max(1, len(pages)))
-        flat = torch.from_numpy(np.concatenate([np.ascontiguousarray(p).reshape(-1) for p in pages]))
-        if self.device_post:
-            flat = flat.to(self.model.cuda_device(), non_blocking=False)
-        out = [None] * len(pages)
+        plan = BatchPlan(shapes, self.model.input_size, max(1, len(shapes)))
+        out = [None] * len(shapes)
         for ch in plan.chunks:
             idx = ch[2]
             prob = self.model.detect_pages_table(flat, plan.table[idx])
@@ -129,8 +161,8 @@ class TextDetector(BaseModule):
             else:
                 prob = prob.cpu().numpy() if prob.is_cuda else prob.numpy()
                 res = [self.postprocess({"binary": prob[j:j + 1, None]}, plan.shapes[i]) for j, i in enumerate(idx)]
-            for i, (quads, scores) in zip(idx, res):
-                out[i] = TextDetectorSchema(points=quads, scores=scores)
+            for i, r in zip(idx, res):
+                out[i] = r
         return out
 
 

@@ -23,6 +23,7 @@ from .config import (TextRecognizerPARSeqConfig, TextRecognizerPARSeqLargeV41Con
                      TextRecognizerPARSeqTinyConfig, TextRecognizerPARSeqTinyDynwV4Config,
                      TextRecognizerPARSeqV2Config)
 from .data import ParseqDataset, crop_records, resize_with_padding
+from .device_pages import as_device_pages, require_device, single_page
 from .models import PARSeq
 from .postprocessor import ParseqTokenizer as Tokenizer
 from .schemas import TextRecognizerSchema
@@ -225,20 +226,24 @@ class TextRecognizer(BaseModule):
                 probs[k, L:] = 1.0
         return ids, probs
 
-    def _device_records(self, img, points):
+    def _device_records(self, img, points, dp=None):
         """Page on the device + one crop record per valid quad, in quad order (data.crop_records); the pyramid levels
-        of source_downscale are built on the device when a record needs them."""
-        geoms, levels, _ = crop_records(img.shape, points, self._cfg.data.img_size, self.dynamic_width,
+        of source_downscale are built on the device when a record needs them.  dp: the page already in HBM (a one-page
+        DevicePages, `img` is then unused), else `img` is uploaded."""
+        shape = img.shape if dp is None else dp.shapes[0] + (3,)
+        geoms, levels, _ = crop_records(shape, points, self._cfg.data.img_size, self.dynamic_width,
                                         self.source_downscale)
-        return {0: self._upload_page(img)}, geoms, levels
+        return {0: self._upload_page(img) if dp is None else dp.pair()}, geoms, levels
 
-    def _call_device_crops(self, img, points):
+    def _call_device_crops(self, img, points, dp=None):
         """`__call__` with the crops cut on the GPU: same order / plan / pairing decisions as the host path, taken
-        from the crop records (canvas and content widths follow from the quads alone)."""
+        from the crop records (canvas and content widths follow from the quads alone).  dp: the page already in HBM
+        (a one-page DevicePages), else `img` is uploaded."""
+        shape = dp.shapes[0] + (3,) if dp is not None else img.shape
         if points is None:
-            h, w = img.shape[:2]
+            h, w = shape[:2]
             points = [[[0, 0], [w, 0], [w, h], [0, h]]]
-        pages, geoms, levels = self._device_records(img, points)
+        pages, geoms, levels = self._device_records(img, points, dp)
         n = len(geoms)
         if n == 0:
             return TextRecognizerSchema(contents=[], scores=[], points=points, directions=[])
@@ -284,7 +289,19 @@ class TextRecognizer(BaseModule):
                 preds[idx], scores[idx], directions[idx] = r_preds[j], r_scores[j], r_dirs[j]
 
     def __call__(self, img, points=None, vis=None):
-        """img: BGR page; points: list of quads (4 clockwise points).  Returns (TextRecognizerSchema, vis)."""
+        """img: BGR page (numpy, or on the GPU: a CUDA (H, W, 3) uint8 tensor or a one-page DevicePages); points: list of
+        quads (4 clockwise points).  Returns (TextRecognizerSchema, vis)."""
+        dp = as_device_pages(img)
+        if dp is not None:
+            if not self.device_crops:
+                raise ValueError("TextRecognizer: pages on the GPU need the device crop extraction, which is off "
+                                 "(YTK_DEVICE_CROPS=0 or a recognizer not on a CUDA device)")
+            single_page(dp, "TextRecognizer")
+            require_device(dp, self.model.cuda_device(), "TextRecognizer")
+            results = self._call_device_crops(None, points, dp.ready())
+            if self.visualize and vis is None:
+                vis = dp.numpy(0)
+            return results, vis
         if self.device_crops:
             results = self._call_device_crops(img, points)
             if self.visualize and vis is None:
