@@ -438,6 +438,29 @@ int ytk_op_resize_bilinear_u8(const uint8_t* pages_dev, long long pages_bytes, c
  * is invalid */
 long long ytk_op_resize_bilinear_scratch_bytes(const ytk_rtdetr_src* srcs, int n, int size);
 double ytk_rtdetr_flops(ytk_rtdetr* h, int n);
+
+/* ---- Table semantic parser: the word-to-element assignment of reference TableSemanticParser.aggregate
+ * (src/yomitoku/table_semantic_parser.py:683-701), every table and the paragraphs of every page in one launch. ---- */
+typedef struct {
+    int w0, w1;   /* the group's words: word_boxes rows [w0, w1) */
+    int e0, e1;   /* its elements (one table's cells, or one page's paragraphs): elem_boxes rows [e0, e1) */
+} ytk_overlap_group;
+
+/* For every word of every group, the element of the group that covers the largest share of the word: both boxes
+ * truncated toward zero to integers and intersected, ratio = integer intersection area / the word's raw fp64 area,
+ * the first element with the largest ratio wins and elements with elem_skip != 0 never do; -1 when no element overlaps
+ * the word or the best ratio is below overlap_th.  Bit-exact with the reference's Python (IEEE fp64, no contraction).
+ * word_boxes [n_words][4] / elem_boxes [n_elems][4]: fp64 x1, y1, x2, y2 on the device, 16-byte aligned, every
+ * coordinate finite with |v| < 2^30 (the caller checks the values; the call cannot); elem_skip [n_elems] bytes on the
+ * device.  groups: host array.  Group g's results are best_dev / ratio_dev [off_g, off_g + w1 - w0) with off_g the
+ * word count of the groups before it, so out_capacity >= the sum of all w1 - w0.  ratio is the best ratio found (0
+ * without overlap) even where best is -1.  Asynchronous on cuda_stream: one H2D copy of the group records and one
+ * launch; invalid groups are an error, not a launch. */
+int ytk_op_assign_best_overlap_f64(const double* word_boxes_dev, int n_words, const double* elem_boxes_dev,
+                                   const uint8_t* elem_skip_dev, int n_elems, const ytk_overlap_group* groups,
+                                   int n_groups, double overlap_th, int* best_dev, double* ratio_dev,
+                                   long long out_capacity, void* cuda_stream);
+
 /* test hook: copies an intermediate activation (by name, see rtdetr_engine.cu) of the LAST forward of batch size n to
  * the host as fp32; shape4 = {n, h, w, c} (token matrices: {1, 1, rows, c}) */
 int ytk_rtdetr_debug_tensor(ytk_rtdetr* h, int n, const char* name, float* host_out, long long capacity, int* shape4);

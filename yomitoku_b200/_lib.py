@@ -88,6 +88,9 @@ def _declare(lib):
     lib.ytk_op_dbnet_head_f32.restype = c_int
     lib.ytk_op_dbnet_head_f32.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, ctypes.c_float,
                                           c_void_p, c_void_p]
+    lib.ytk_op_assign_best_overlap_f64.restype = c_int
+    lib.ytk_op_assign_best_overlap_f64.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int,
+                                                   ctypes.c_double, c_void_p, c_void_p, c_ll, c_void_p]
 
 
 class YtkAttnSeq(ctypes.Structure):

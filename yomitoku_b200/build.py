@@ -24,9 +24,11 @@ NVCC_FLAGS = [
 
 # OpenCV's float / double expressions are not contracted into FMAs: the bit-exact restatement in crop_math.h needs the
 # same (csrc/crop_ops.cu header).  Pillow's resample coefficients are double arithmetic computed on the host
-# (csrc/resample_ops.cu header): neither the device nor the host compiler may contract them.
+# (csrc/resample_ops.cu header): neither the device nor the host compiler may contract them.  The table parser's overlap
+# ratios are fp64 restatements of Python arithmetic (csrc/table_ops.cu header).
 EXTRA_FLAGS = {"crop_ops.cu": ["--fmad=false"],
-               "resample_ops.cu": ["--fmad=false", "-Xcompiler", "-ffp-contract=off"]}
+               "resample_ops.cu": ["--fmad=false", "-Xcompiler", "-ffp-contract=off"],
+               "table_ops.cu": ["--fmad=false"]}
 
 
 def _sources():

@@ -22,6 +22,7 @@
 #include "parseq_engine.h"
 #include "resample_ops.h"
 #include "rtdetr_engine.h"
+#include "table_ops.h"
 
 // Binds the calling host thread to a device for the duration of an API call and puts the previous device back (host
 // threads start on device 0, and a handle on cuda:1 must not leave "the current device" changed for the caller - PyTorch
@@ -1219,6 +1220,72 @@ double ytk_parseq_last_flops(ytk_parseq* h) { return h->engine.flops; }
 int ytk_parseq_last_steps(ytk_parseq* h) { return h->engine.last_steps; }
 void ytk_parseq_last_phase_ms(ytk_parseq* h, float* ms4) {
     for (int i = 0; i < 4; ++i) ms4[i] = h->engine.phase_ms[i];
+}
+
+int ytk_op_assign_best_overlap_f64(const double* word_boxes_dev, int n_words, const double* elem_boxes_dev,
+                                   const uint8_t* elem_skip_dev, int n_elems, const ytk_overlap_group* groups,
+                                   int n_groups, double overlap_th, int* best_dev, double* ratio_dev,
+                                   long long out_capacity, void* cuda_stream) {
+    const char* who = "ytk_op_assign_best_overlap_f64";
+    if (n_words < 0 || n_elems < 0 || n_groups < 0 || (n_groups > 0 && !groups)) {
+        ytk::set_error("%s: %d words, %d elements, %d groups (non-negative, groups given)", who, n_words, n_elems,
+                       n_groups);
+        return YTK_ERR;
+    }
+    if (std::isnan(overlap_th)) {
+        ytk::set_error("%s: overlap_th is NaN", who);
+        return YTK_ERR;
+    }
+    // group records, their result offsets and one CTA per (group, kOverlapThreads words), checked and built on the host
+    std::vector<ytk::OverlapGroup> dg((size_t)n_groups);
+    std::vector<ytk::OverlapItem> items;
+    long long total = 0;
+    for (int g = 0; g < n_groups; ++g) {
+        const ytk_overlap_group& r = groups[g];
+        if (r.w0 < 0 || r.w1 < r.w0 || r.w1 > n_words || r.e0 < 0 || r.e1 < r.e0 || r.e1 > n_elems) {
+            ytk::set_error("%s: group %d has words [%d, %d) of %d and elements [%d, %d) of %d", who, g, r.w0, r.w1,
+                           n_words, r.e0, r.e1, n_elems);
+            return YTK_ERR;
+        }
+        dg[g] = ytk::OverlapGroup{r.w0, r.w1, r.e0, r.e1, total, 0};
+        for (int w = r.w0; w < r.w1; w += ytk::kOverlapThreads) items.push_back(ytk::OverlapItem{g, w});
+        total += r.w1 - r.w0;
+    }
+    if (total > out_capacity || items.size() > (size_t)INT_MAX) {
+        ytk::set_error("%s: %lld results for an output capacity of %lld (%zu blocks)", who, total, out_capacity,
+                       items.size());
+        return YTK_ERR;
+    }
+    if (items.empty()) return YTK_OK;
+    if (!word_boxes_dev || !elem_boxes_dev || !elem_skip_dev || !best_dev || !ratio_dev) {
+        ytk::set_error("%s: null argument", who);
+        return YTK_ERR;
+    }
+    if (misaligned(word_boxes_dev, 16) || misaligned(elem_boxes_dev, 16)) {
+        ytk::set_error("%s: word_boxes_dev and elem_boxes_dev must be 16-byte aligned", who);
+        return YTK_ERR;
+    }
+    cudaPointerAttributes attr{};
+    if (cudaPointerGetAttributes(&attr, word_boxes_dev) != cudaSuccess || attr.type != cudaMemoryTypeDevice) {
+        cudaGetLastError();
+        ytk::set_error("%s: word_boxes_dev is not a device pointer", who);
+        return YTK_ERR;
+    }
+    DevGuard dev_guard(attr.device);
+    cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    const size_t gbytes = dg.size() * sizeof(ytk::OverlapGroup), ibytes = items.size() * sizeof(ytk::OverlapItem);
+    std::vector<uint8_t> blob(gbytes + ibytes);
+    std::memcpy(blob.data(), dg.data(), gbytes);
+    std::memcpy(blob.data() + gbytes, items.data(), ibytes);
+    uint8_t* d = static_cast<uint8_t*>(stream_buffer(blob.data(), blob.size(), st, who));
+    if (!d) return YTK_ERR;
+    const int rc = ytk::launch_assign_best_overlap(word_boxes_dev, elem_boxes_dev, elem_skip_dev,
+                                                   reinterpret_cast<const ytk::OverlapGroup*>(d),
+                                                   reinterpret_cast<const ytk::OverlapItem*>(d + gbytes),
+                                                   (int)items.size(), overlap_th, best_dev, ratio_dev, st);
+    cudaFreeAsync(d, st);
+    if (rc) ytk::set_error("%s: kernel launch failed", who);
+    return rc ? YTK_ERR : YTK_OK;
 }
 
 }  // extern "C"

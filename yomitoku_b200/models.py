@@ -274,6 +274,51 @@ def concat_device_buffers(parts, stream=None):
     return torch.cat([t[:n] for t, n in parts])
 
 
+OVERLAP_GROUP_DTYPE = np.dtype([("w0", "<i4"), ("w1", "<i4"), ("e0", "<i4"), ("e1", "<i4")])   # = ytk_overlap_group
+_COORD_LIMIT = float(1 << 30)
+
+
+def assign_best_overlap(word_boxes, elem_boxes, elem_skip, groups, overlap_th=0.2, device="cuda"):
+    """The word-to-element assignment of the table semantic parser on the GPU, every group in one launch (C ABI
+    ytk_op_assign_best_overlap_f64, csrc/table_ops.cu).
+
+    word_boxes (n_words, 4) / elem_boxes (n_elems, 4): x1, y1, x2, y2, converted to float64; elem_skip (n_elems,):
+    true for elements that never take a word (role "group"); groups: OVERLAP_GROUP_DTYPE records (or an (n, 4) int
+    array) of word / element ranges.  Returns (best, ratio): for every group in order and every word of its range, the
+    index into elem_boxes of the element that covers the largest share of the word (the first on ties), or -1 when none
+    does or its share is below overlap_th, and that share (0 without overlap).  Synchronises the device."""
+    words = np.ascontiguousarray(np.asarray(word_boxes, np.float64).reshape(-1, 4))
+    elems = np.ascontiguousarray(np.asarray(elem_boxes, np.float64).reshape(-1, 4))
+    skip = np.ascontiguousarray(np.asarray(elem_skip, np.uint8).reshape(-1))
+    if len(skip) != len(elems):
+        raise ValueError("assign_best_overlap: %d skip flags for %d elements" % (len(skip), len(elems)))
+    if not isinstance(groups, np.ndarray) or groups.dtype != OVERLAP_GROUP_DTYPE:
+        groups = np.asarray(groups, np.int32).reshape(-1, 4).copy().view(OVERLAP_GROUP_DTYPE).reshape(-1)
+    groups = np.ascontiguousarray(groups)
+    for name, a in (("word", words), ("element", elems)):
+        if len(a) and not (np.isfinite(a).all() and np.abs(a).max() < _COORD_LIMIT):
+            raise ValueError("assign_best_overlap: %s coordinates must be finite with |v| < 2^30" % name)
+    if (groups["w1"] < groups["w0"]).any():
+        raise ValueError("assign_best_overlap: a group has w1 < w0")
+    total = int((groups["w1"].astype(np.int64) - groups["w0"]).sum())
+    if total == 0:
+        return np.zeros(0, np.int32), np.zeros(0, np.float64)
+    dev = torch.device(device)
+    if dev.type == "cuda" and dev.index is None:
+        dev = torch.device("cuda", torch.cuda.current_device())
+    with torch.cuda.device(dev):
+        boxes = torch.from_numpy(np.concatenate([words, elems, np.zeros((1, 4))])).to(dev)   # never an empty tensor
+        skip_d = torch.from_numpy(np.concatenate([skip, np.zeros(1, np.uint8)])).to(dev)
+        best = torch.empty(total, dtype=torch.int32, device=dev)
+        ratio = torch.empty(total, dtype=torch.float64, device=dev)
+        stream = torch.cuda.current_stream(dev)
+        _lib.check(_lib.lib().ytk_op_assign_best_overlap_f64(
+            boxes.data_ptr(), len(words), boxes[len(words):].data_ptr(), skip_d.data_ptr(), len(elems),
+            groups.ctypes.data, len(groups), float(overlap_th), best.data_ptr(), ratio.data_ptr(), total,
+            ctypes.c_void_p(stream.cuda_stream)))
+        return best.cpu().numpy(), ratio.cpu().numpy()
+
+
 # ======================================================================================================== DBNet
 def _dbnet_random_state_dict(seed=0):
     """Random init with the reference's key set (DBNet(cfg) with from_pretrained=False, base.py:84-86)."""

@@ -243,3 +243,27 @@ class CellDetector(BaseModule):
             outputs.append(TableDetectorSchema(id=None, box=table.box, role=table.role, cells=cells,
                                                kv_regions=kv_regions, grid_regions=grid_regions))
         return outputs
+
+    def detect_pages(self, pages, tables_per_page):
+        """Batched entry (new surface): `__call__` for many pages with ONE model forward over the table crops of all of
+        them.  pages: a DevicePages or a list of BGR numpy pages; tables_per_page: the layout parser's tables of each
+        page.  Returns a list (per page) of List[TableDetectorSchema], equal to `__call__(page, tables)` per page."""
+        recs = [(i, [int(v) for v in t.box]) for i, tables in enumerate(tables_per_page) for t in tables]
+        out = [[] for _ in tables_per_page]
+        if not recs:
+            return out
+        dp = as_device_pages(pages)
+        dev = rtdetr_device_forward(self.model, dp if dp is not None else pages, recs)
+        if dev is not None:
+            preds, data = dev[0], [{"size": s, "offset": (b[0], b[1])} for s, (_, b) in zip(dev[1], recs)]
+        else:
+            data = [d for i, tables in enumerate(tables_per_page) if tables
+                    for d in self.preprocess(dp.numpy(i) if dp is not None else pages[i], tables)]
+            preds = self.model(torch.cat([d["tensor"] for d in data]))
+        tables = [t for ts in tables_per_page for t in ts]
+        for k, ((i, _), d, table) in enumerate(zip(recs, data, tables)):
+            cells, kv_regions, grid_regions = self.postprocess({n: v[k:k + 1] for n, v in preds.items()}, d, table.box)
+            if cells:
+                out[i].append(TableDetectorSchema(id=None, box=table.box, role=table.role, cells=cells,
+                                                  kv_regions=kv_regions, grid_regions=grid_regions))
+        return out
