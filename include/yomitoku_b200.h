@@ -41,14 +41,18 @@ int ytk_gemm_profile_end(double* flops, double* ms, long long* launches);
  * [Cout][kh][kw][Cin], bias fp32 [Cout] or NULL, resid: [N,Ho,Wo,ldr] fp16/fp32 or NULL, out: [N,Ho,Wo,ldc]
  * fp16/fp32.  Replaces torch.nn.Conv2d + BatchNorm2d(eval, folded) + ReLU (+ residual add) of
  * torchvision ResNet-50 bottlenecks (reference models/dbnet_plus.py:30-38) and the decoder convs (:56-116).
- * mode 1 = ConvTranspose2d(kernel 2, stride 2) written as a GEMM with a pixel-shuffle epilogue (:111,:114). */
+ * mode 1 = ConvTranspose2d(kernel 2, stride 2) written as a GEMM with a pixel-shuffle epilogue (:111,:114).
+ * Refused before any launch: in_ld < Cin, a mode other than 0 / 1, and the epilogue conditions below. */
 int ytk_op_conv2d_f16(const void* in, int N, int H, int W, int Cin, long long in_ld, const void* w, const float* bias,
                        int kh, int kw, int stride, int pad, int dil, int Cout, const void* resid, int resid_f32,
                        long long ldr, void* out, int out_f32, long long ldc, int act, int mode, void* cuda_stream);
 
-/* Linear layer y = act(A W^T + b (+ resid)); A [M,lda] fp16, W [N,K] fp16 (torch nn.Linear layout), K % 64 == 0.
- * Replaces nn.Linear / timm Mlp / attention projections (reference models/layers/parseq_transformer.py:43-52,
- * models/parseq.py:72). */
+/* Linear layer y = act(A W^T + b (+ resid)); A [M,lda] fp16, W [N,K] fp16 (torch nn.Linear layout), K % 64 == 0,
+ * lda >= K and a multiple of 8.  Replaces nn.Linear / timm Mlp / attention projections (reference
+ * models/layers/parseq_transformer.py:43-52, models/parseq.py:72).
+ * Epilogue conditions of both entries, refused before any launch: N (Cout) >= 1; act in 0..4; out, resid and bias
+ * 16-byte aligned; ldc >= N (conv mode 1: ldc >= Cout / 4) and ldr >= N, both keeping rows 16-byte aligned (a multiple
+ * of 8 fp16 or 4 fp32 elements).  The output may start at a column offset inside a wider buffer (a concat half). */
 int ytk_op_linear_f16(const void* A, long long lda, int M, int K, const void* W, int N, const float* bias,
                        const void* resid, int resid_f32, long long ldr, void* out, int out_f32, long long ldc, int act,
                        void* cuda_stream);

@@ -1,5 +1,5 @@
-"""CPU: the op-level entries of the deformable attention, LayerNorm and single-query attention kernels and of the DBNet
-detector's kernels refuse invalid arguments on the host - a nonzero status, a message that names the problem, and no
+"""CPU: the op-level entries of the deformable attention, LayerNorm and single-query attention kernels, of the DBNet
+detector's kernels and of the GEMM (linear / convolution) refuse invalid arguments on the host - a nonzero status, a message that names the problem, and no
 kernel launch.  The pointers are never dereferenced on these paths, so plain addresses stand in for device buffers."""
 import ctypes
 
@@ -345,4 +345,55 @@ def test_apply_rep_cut_refusals(lib, kwargs, fragment):
     before = lib.ytk_launch_count()
     _refused(lib, lib.ytk_op_apply_rep_cut(a["rep_cut"], a["B"], a["S"], a["C"], a["eos"], a["ids"], a["probs"], None),
              fragment)
+    assert lib.ytk_launch_count() == before
+
+
+# ======================================================================================================== GEMM entries
+def _linear(lib, A=P, lda=256, M=300, K=256, W=P, N=200, bias=P, resid=None, resid_f32=0, ldr=0, out=P, out_f32=0,
+            ldc=200, act=0):
+    return lib.ytk_op_linear_f16(A, lda, M, K, W, N, bias, resid, resid_f32, ldr, out, out_f32, ldc, act, None)
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(out=None), b"null output"),
+    # a misaligned output would take the staged epilogue, whose 16-byte stores fault: refused on the host
+    (dict(out=P + 8), b"16-byte aligned"), (dict(out=P + 4, out_f32=1), b"16-byte aligned"),
+    (dict(resid=P + 8, ldr=200), b"16-byte aligned"), (dict(bias=P + 4), b"16-byte aligned"),
+    (dict(ldc=192), b"ldc=192 is less than the 200 columns"), (dict(ldc=196), b"ldc=196 must keep rows 16-byte"),
+    (dict(out_f32=1, ldc=196), b"ldc=196 is less than the 200 columns"),
+    (dict(resid=P, ldr=192), b"ldr=192 is less than Cout=200"),
+    (dict(resid=P, resid_f32=1, ldr=196), b"ldr=196 is less than Cout=200"),
+    (dict(N=0), b"Cout=0"), (dict(N=-8), b"Cout=-8"),
+    (dict(act=5), b"act 5 unknown"), (dict(act=-1), b"act -1 unknown"),
+    (dict(lda=192), b"lda=192 must be >= K=256"), (dict(lda=260), b"lda=260 must be >= K=256 and a multiple of 8"),
+    (dict(K=100, lda=104), b"K=100"), (dict(M=0), b"M=0"),
+])
+def test_linear_refusals(lib, kwargs, fragment):
+    before = lib.ytk_launch_count()
+    _refused(lib, _linear(lib, **kwargs), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+def _conv(lib, x=P, N=1, H=37, W=50, Cin=128, in_ld=128, w=P, bias=P, k=3, s=1, p=1, d=1, Cout=256, resid=None,
+          resid_f32=0, ldr=0, out=P, out_f32=0, ldc=256, act=1, mode=0):
+    return lib.ytk_op_conv2d_f16(x, N, H, W, Cin, in_ld, w, bias, k, k, s, p, d, Cout, resid, resid_f32, ldr, out,
+                                 out_f32, ldc, act, mode, None)
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(in_ld=120), b"in_ld 120 < Cin 128"),
+    # the fused DBNet head (2) and the row statistics (3) need arguments this entry does not take
+    (dict(mode=2), b"mode 2 unsupported"), (dict(mode=3), b"mode 3 unsupported"), (dict(mode=-1), b"mode -1"),
+    (dict(out=None), b"null output"),
+    (dict(out=P + 8), b"16-byte aligned"), (dict(out=P + 8, out_f32=1), b"16-byte aligned"),
+    (dict(resid=P + 8, ldr=256), b"16-byte aligned"), (dict(bias=P + 4), b"16-byte aligned"),
+    (dict(ldc=248), b"ldc=248 is less than the 256 columns"),
+    # 2x2 pixel shuffle: each of the four column blocks of width Cout / 4 is one output pixel's row
+    (dict(mode=1, k=1, p=0, ldc=56), b"ldc=56 is less than the 64 columns"),
+    (dict(resid=P, ldr=248), b"ldr=248 is less than Cout=256"),
+    (dict(Cout=0), b"Cout=0"), (dict(act=7), b"act 7 unknown"),
+])
+def test_conv2d_refusals(lib, kwargs, fragment):
+    before = lib.ytk_launch_count()
+    _refused(lib, _conv(lib, **kwargs), fragment)
     assert lib.ytk_launch_count() == before

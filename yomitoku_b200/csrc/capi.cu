@@ -135,6 +135,15 @@ int ytk_gemm_profile_end(double* flops, double* ms, long long* launches) {
 int ytk_op_conv2d_f16(const void* in, int N, int H, int W, int Cin, long long in_ld, const void* w, const float* bias,
                        int kh, int kw, int stride, int pad, int dil, int Cout, const void* resid, int resid_f32,
                        long long ldr, void* out, int out_f32, long long ldc, int act, int mode, void* cuda_stream) {
+    if (in_ld < Cin) {
+        ytk::set_error("ytk_op_conv2d_f16: in_ld %lld < Cin %d", in_ld, Cin);
+        return YTK_ERR;
+    }
+    // the fused DBNet head and the row statistics have their own entries, with the arguments those epilogues need
+    if (mode != ytk::EPI_NORMAL && mode != ytk::EPI_SHUFFLE2X) {
+        ytk::set_error("ytk_op_conv2d_f16: mode %d unsupported (0 = plain, 1 = 2x2 pixel shuffle)", mode);
+        return YTK_ERR;
+    }
     ytk::ConvGeom g{N, H, W, Cin, in_ld, kh, kw, stride, pad, dil, Cout};
     ytk::Epilogue e;
     e.bias = bias;

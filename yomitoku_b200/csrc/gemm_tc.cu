@@ -1022,6 +1022,67 @@ static int pick_bw_log2(int Ho, int Wo) {
     return best;
 }
 
+// Refuses an epilogue the kernel cannot store safely, before any CUDA call.  The staged epilogue moves 16-byte pieces
+// (uint4 / float4) at base + (pixel * pitch + column) * element size and reads the bias as float4, so bases and pitches
+// must keep those pieces 16-byte aligned; the TMA epilogue encodes a tensor of width Cout with row pitch ldc.
+static int check_epilogue(int Cout, const Epilogue& e) {
+    auto misaligned = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; };
+    if (e.out == nullptr) {
+        set_error("gemm plan: null output");
+        return 1;
+    }
+    if (Cout < 1) {
+        set_error("gemm plan: Cout=%d", Cout);
+        return 1;
+    }
+    if (e.act < ACT_NONE || e.act > ACT_SILU) {
+        set_error("gemm plan: act %d unknown (0..4)", e.act);
+        return 1;
+    }
+    // the fused final conv stores float2 pairs: its probability map needs 8-byte alignment only
+    if ((e.mode != EPI_CONVT_FINAL && misaligned(e.out)) || misaligned(e.resid) || misaligned(e.bias)) {
+        set_error("gemm plan: output, residual and bias must be 16-byte aligned");
+        return 1;
+    }
+    if (e.mode == EPI_ROWMAX) {
+        if (e.resid != nullptr) {
+            set_error("gemm plan: ROWMAX takes no residual");
+            return 1;
+        }
+    } else if (e.mode == EPI_CONVT_FINAL) {
+        if (Cout != 256 || e.fin_w == nullptr || !e.out_f32) {
+            set_error("gemm plan: CONVT_FINAL needs Cout=256, fp32 output and the final conv weights");
+            return 1;
+        }
+    } else {
+        if ((e.out_f32 ? (e.ldc % 4) : (e.ldc % 8)) != 0) {
+            set_error("gemm plan: ldc=%lld must keep rows 16-byte aligned", e.ldc);
+            return 1;
+        }
+        // SHUFFLE2X: column block (i, j) of width Cout / 4 goes to its own output pixel
+        const long long width = e.mode == EPI_SHUFFLE2X ? Cout / 4 : Cout;
+        if (e.ldc < width) {
+            set_error("gemm plan: ldc=%lld is less than the %lld columns of an output row", e.ldc, width);
+            return 1;
+        }
+    }
+    if (e.resid) {
+        if ((e.resid_f32 ? (e.ldr % 4) : (e.ldr % 8)) != 0) {
+            set_error("gemm plan: ldr=%lld must keep rows 16-byte aligned", e.ldr);
+            return 1;
+        }
+        if (e.ldr < Cout) {
+            set_error("gemm plan: ldr=%lld is less than Cout=%d", e.ldr, Cout);
+            return 1;
+        }
+    }
+    if (e.mode == EPI_SHUFFLE2X && ((Cout % 4) != 0 || ((Cout / 4) % 32) != 0)) {
+        set_error("gemm plan: SHUFFLE2X needs Cout/4 to be a multiple of 32 (Cout=%d)", Cout);
+        return 1;
+    }
+    return 0;
+}
+
 static int finish_plan(GemmPlan* plan, const void* w_packed, int Ktot, int Cout, const Epilogue& e) {
     GemmArgs& a = plan->args;
     plan->block_n = pick_block_n(Cout);
@@ -1066,44 +1127,19 @@ static int finish_plan(GemmPlan* plan, const void* w_packed, int Ktot, int Cout,
     a.mode = e.mode;
     a.fin_w = e.fin_w;
     a.fin_b = e.fin_b;
-    if (e.out == nullptr) {
-        set_error("gemm plan: null output");
-        return 1;
-    }
     if (e.mode == EPI_ROWMAX) {
-        if (e.resid != nullptr) {
-            set_error("gemm plan: ROWMAX takes no residual");
-            return 1;
-        }
         a.out_f32 = 1;
         a.ldc = 2LL * a.tiles_n;   // float4 partials per row
-    } else if (e.mode == EPI_CONVT_FINAL) {
-        if (Cout != 256 || e.fin_w == nullptr || !e.out_f32) {
-            set_error("gemm plan: CONVT_FINAL needs Cout=256, fp32 output and the final conv weights");
-            return 1;
-        }
-    } else if ((e.out_f32 ? (e.ldc % 4) : (e.ldc % 8)) != 0) {
-        set_error("gemm plan: ldc=%lld must keep rows 16-byte aligned", e.ldc);
-        return 1;
-    }
-    if (e.resid && ((e.resid_f32 ? (e.ldr % 4) : (e.ldr % 8)) != 0)) {
-        set_error("gemm plan: ldr=%lld must keep rows 16-byte aligned", e.ldr);
-        return 1;
-    }
-    if (e.mode == EPI_SHUFFLE2X && ((Cout % 4) != 0 || ((Cout / 4) % 32) != 0)) {
-        set_error("gemm plan: SHUFFLE2X needs Cout/4 to be a multiple of 32 (Cout=%d)", Cout);
-        return 1;
     }
     const int tiles = a.n_img * a.tiles_h * a.tiles_w * a.tiles_n;
-    // TMA epilogue: plain stores whose residual (if any) has the output's element size; 16-byte aligned bases
-    // and rows whose extent is a multiple of 16 bytes: a TMA store clips the box at the tensor's inner
-    // extent in 16-byte units (Cout = 7119 fp32 columns: column 7119 of a 7120-wide buffer was written)
+    // TMA epilogue: plain stores whose residual (if any) has the output's element size and rows whose extent is a
+    // multiple of 16 bytes: a TMA store clips the box at the tensor's inner extent in 16-byte units (Cout = 7119 fp32
+    // columns: column 7119 of a 7120-wide buffer was written).  Bases and pitches are 16-byte aligned (check_epilogue).
     a.epi_tma = 0;
     a.epi_swz = 0;
     a.epi_pf = 0;
     if (epi_mode_env() == 2 && e.mode == EPI_NORMAL && (e.resid == nullptr || (e.resid_f32 != 0) == (e.out_f32 != 0)) &&
-        ((long long)Cout * (e.out_f32 ? 4 : 2)) % 16 == 0 &&
-        (reinterpret_cast<uintptr_t>(e.out) & 15) == 0 && (reinterpret_cast<uintptr_t>(e.resid) & 15) == 0) {
+        ((long long)Cout * (e.out_f32 ? 4 : 2)) % 16 == 0) {
         static const bool no_swz = getenv("YTK_EPI_SWZ") != nullptr && getenv("YTK_EPI_SWZ")[0] == '0';
         // whole-tile L2 prefetch of the residual one tile ahead: opt-in (YTK_EPI_PF=1).
         static const bool no_pf = !(getenv("YTK_EPI_PF") != nullptr && getenv("YTK_EPI_PF")[0] == '1');
@@ -1144,6 +1180,7 @@ int conv_plan_create(GemmPlan* plan, const void* in, const ConvGeom& g, const vo
         set_error("conv plan: %dx%d filter exceeds %d taps", g.kh, g.kw, kMaxTaps);
         return 1;
     }
+    if (check_epilogue(g.Cout, e)) return 1;
     const int Ho = (g.H + 2 * g.pad - g.dil * (g.kh - 1) - 1) / g.stride + 1;
     const int Wo = (g.W + 2 * g.pad - g.dil * (g.kw - 1) - 1) / g.stride + 1;
     a.Ho = Ho;
@@ -1218,6 +1255,11 @@ int gemm_plan_create(GemmPlan* plan, const void* A, long long lda, int M, int K,
         set_error("gemm plan: M=%d", M);
         return 1;
     }
+    if (lda < K || lda % 8 != 0) {
+        set_error("gemm plan: lda=%lld must be >= K=%d and a multiple of 8", lda, K);
+        return 1;
+    }
+    if (check_epilogue(N, e)) return 1;
     a.Ho = 1;
     a.Wo = M;
     a.n_img = 1;
@@ -1241,6 +1283,7 @@ int gemm_plan_create(GemmPlan* plan, const void* A, long long lda, int M, int K,
 int stem_plan_create(GemmPlan* plan, const void* in_padded, int N, int Hn, int Wn, const void* w_packed,
                      const Epilogue& e) {
     memset(plan, 0, sizeof(*plan));
+    if (check_epilogue(64, e)) return 1;
     GemmArgs& a = plan->args;
     const int Ho = Hn / 2, Wo = Wn / 2, Hp = Hn + 6, Wp = Wn + 8;
     a.Ho = Ho;
@@ -1274,25 +1317,13 @@ int stem_plan_create(GemmPlan* plan, const void* in_padded, int N, int Hn, int W
 
 int gemm_plan_set_out(GemmPlan* plan, void* out) {
     GemmArgs& a = plan->args;
-    a.out = out;
-    if (!a.epi_tma) return 0;
     if ((reinterpret_cast<uintptr_t>(out) & 15) != 0) {
-        set_error("gemm_plan_set_out: output must be 16-byte aligned for the TMA epilogue");
+        set_error("gemm_plan_set_out: output must be 16-byte aligned");
         return 1;
     }
+    a.out = out;
+    if (!a.epi_tma) return 0;
     return make_tmap_epi(&plan->maps.out, out, a.out_f32, a, a.Cout, a.ldc, a.epi_swz);
-}
-
-void gemm_plan_set_m(GemmPlan* plan, int M) {
-    GemmArgs& a = plan->args;
-    a.epi_tma = 0;   // the epilogue tensor maps were encoded for the original extent
-    const double per_row = a.Wo > 0 ? plan->flops / a.Wo : 0.0;
-    a.Wo = M;
-    a.tiles_w = (M + 127) / 128;
-    plan->flops = per_row * M;
-    const int tiles = a.tiles_w * a.tiles_n;
-    plan->grid = tiles < num_sms() ? tiles : num_sms();
-    if (plan->grid < 1) plan->grid = 1;
 }
 
 template <int BLOCK_N, int OUT_F32, int RESID, int MODE, int DIRECT>
@@ -1366,6 +1397,7 @@ struct ProfRec {
     cudaEvent_t a, b;
     double flops;
     int pixels, cout, k, block_n, mode, act, resid, out_f32, ntaps;   // shape of the launch (YTK_GEMM_DUMP)
+    int epi, bw_log2;   // epilogue path (1 = TMA, 0 = staged) and tile patch (BW = 1 << bw_log2)
 };
 std::mutex g_prof_mu;
 bool g_prof_on = false;
@@ -1412,12 +1444,12 @@ int gemm_profile_end(double* flops, double* ms, long long* launches) {
     if (launches) *launches = (long long)g_prof.size();
     if (const char* path = getenv("YTK_GEMM_DUMP")) {      // per-launch table of the window for shape-level analysis
         if (FILE* fp = fopen(path, "a")) {
-            fprintf(fp, "pixels,cout,k,ntaps,block_n,mode,act,resid,out_f32,flops,ms\n");
+            fprintf(fp, "pixels,cout,k,ntaps,block_n,mode,act,resid,out_f32,flops,ms,epi,bw_log2\n");
             for (ProfRec& r : g_prof) {
                 float e = 0.f;
                 cudaEventElapsedTime(&e, r.a, r.b);
-                fprintf(fp, "%d,%d,%d,%d,%d,%d,%d,%d,%d,%.0f,%.6f\n", r.pixels, r.cout, r.k, r.ntaps, r.block_n,
-                        r.mode, r.act, r.resid, r.out_f32, r.flops, e);
+                fprintf(fp, "%d,%d,%d,%d,%d,%d,%d,%d,%d,%.0f,%.6f,%d,%d\n", r.pixels, r.cout, r.k, r.ntaps, r.block_n,
+                        r.mode, r.act, r.resid, r.out_f32, r.flops, e, r.epi, r.bw_log2);
             }
             fclose(fp);
         }
@@ -1444,6 +1476,8 @@ int gemm_plan_launch(const GemmPlan* plan, cudaStream_t stream) {
             rec.act = g.act;
             rec.resid = g.resid ? (g.resid_f32 ? 2 : 1) : 0;
             rec.out_f32 = g.out_f32;
+            rec.epi = g.epi_tma;
+            rec.bw_log2 = g.bw_log2;
             prof = true;
         }
     }

@@ -105,9 +105,13 @@ struct GemmPlan {
     double flops;  // 2*M*N*K of the true problem (for roofline accounting)
 };
 
-// All return 0 on success, nonzero on failure (message via ytk::last_error()).
+// All return 0 on success, nonzero on failure (message via ytk::last_error()).  Every plan refuses, before any CUDA
+// call: a null output, Cout < 1, an act outside ACT_NONE..ACT_SILU, an output (except EPI_CONVT_FINAL's), residual or
+// bias base that is not 16-byte aligned, pitches ldc / ldr that do not keep rows 16-byte aligned, ldc < Cout
+// (EPI_NORMAL; Cout / 4 for EPI_SHUFFLE2X) and ldr < Cout.
 int conv_plan_create(GemmPlan* plan, const void* in, const ConvGeom& g, const void* w_packed, const Epilogue& e);
-// A: [M, lda] bf16 row-major (K multiple of 64, first K columns used); Wt: [N, K] bf16 row-major.
+// A: [M, lda] 16-bit row-major (K multiple of 64, lda >= K and a multiple of 8, first K columns used); Wt: [N, K] 16-bit
+// row-major.
 int gemm_plan_create(GemmPlan* plan, const void* A, long long lda, int M, int K, const void* Wt, int N,
                      const Epilogue& e);
 // ResNet stem: 7x7 stride-2 pad-3 conv over a zero-padded 8-channel NHWC canvas [N, Hn+6, Wn+8, 8] (pixel (h,w) at
@@ -115,10 +119,8 @@ int gemm_plan_create(GemmPlan* plan, const void* A, long long lda, int M, int K,
 // rows overlap in memory (W stride = 2 pixels).  w_packed: [Cout][7][64] bf16.
 int stem_plan_create(GemmPlan* plan, const void* in_padded, int N, int Hn, int Wn, const void* w_packed,
                      const Epilogue& e);
-// Same but the M extent can be changed per launch (rows beyond M are never stored).
-void gemm_plan_set_m(GemmPlan* plan, int M);
 // Points a prepared plan at another output buffer of the same shape and pitch (the AR loop's K/V cache slot of the
-// step); re-encodes the output tensor map when the plan stores through TMA.  Returns 0 on success.
+// step; 16-byte aligned); re-encodes the output tensor map when the plan stores through TMA.  Returns 0 on success.
 int gemm_plan_set_out(GemmPlan* plan, void* out);
 int gemm_plan_launch(const GemmPlan* plan, cudaStream_t stream);
 
