@@ -107,6 +107,42 @@ int ytk_op_layernorm_f32(float* x, int M, int D, int d_real, const float* gamma,
                          void* out_f16, float* out_f32, const float* addvec, int period, const int* add_row0_dev,
                          int add_row0, int writeback, void* cuda_stream);
 
+/* op level, for the parity tests: the RT-DETRv2 engine's small kernels, each called as the engine calls it.  Device
+ * pointers; activations NHWC / token rows fp16, decoder state fp32; asynchronous on the stream; invalid arguments are an
+ * error, not a launch.  Level arrays (level_h / level_w: host arrays of n_levels, 1..4) describe the level-major row
+ * order of ytk_op_deform_attn_f16: level l of image i is rows [off[l] * n_img + i * h[l] * w[l], ...), and an anchor is
+ * off[l] + y * w[l] + x.  Anchor ids read from device arrays (invalid_dev, idx_dev) must lie in [0, sum of h * w): the
+ * call cannot check them.
+ *   avgpool2        AvgPool2d(2, 2) of the variant-d shortcut: in [n, H, W, C] -> out [n, H/2, W/2, C]; H, W even, C a
+ *                   multiple of 8, 16-byte aligned.
+ *   upsample        nearest x2: src [n, Hs, Ws] rows of pitch lds (first C channels read) -> channels [coff, coff + C)
+ *                   of dst [n, 2Hs, 2Ws] rows of pitch ldd, nothing else written; C, lds, ldd, coff multiples of 8.
+ *   add             out = a + b (fp16 [rows, C]), or with b_f32 (fp32 table [period, C]) out = a + b_f32[row % period];
+ *                   exactly one of b / b_f32; C a multiple of 8; a, b, out 16-byte aligned.
+ *   mask_invalid    rows of the n_invalid anchors of invalid_dev, in every image, of x fp32 [rows, D] become bias [D].
+ *   enc_scores      scores [n_img, anchors] = max over the first C columns of logits fp32 [rows, ldl] (level-major).
+ *   gather_queries  per (image i, query j), a = idx_dev[i * K + j]: tgt / tgt16 [n_img * K, D] = om [rows, D] at a's row
+ *                   (fp32 / fp16), anchor_sel [n_img * K, 4] = anchors [anchors, 4][a].
+ *   ref_update      ref [n, 4] = sigmoid(delta [n, ldd] (first 4 columns) + base), base = anchor_sel [n, 4] if given,
+ *                   else inverse_sigmoid(ref) = log(max(x, 1e-5) / max(1 - x, 1e-5)), x = ref clipped to [0, 1].
+ *   qpos_l0         out [rows, H1] fp16 = relu(W [H1, 4] ref [rows, 4] + b [H1]); ref and W 16-byte aligned. */
+int ytk_op_rt_avgpool2_f16(const void* in, int n, int H, int W, int C, void* out, void* cuda_stream);
+int ytk_op_rt_upsample_nearest2_f16(const void* src, long long lds, int n, int Hs, int Ws, int C, void* dst,
+                                    long long ldd, int coff, void* cuda_stream);
+int ytk_op_rt_add_f16(const void* a, const void* b, const float* b_f32, int C, int period, void* out, long long rows,
+                      void* cuda_stream);
+int ytk_op_rt_mask_invalid_f32(float* x, int D, const float* bias, const int* invalid_dev, int n_invalid,
+                               const int* level_h, const int* level_w, int n_levels, int n_img, void* cuda_stream);
+int ytk_op_rt_enc_scores_f32(const float* logits, long long ldl, int C, const int* level_h, const int* level_w,
+                             int n_levels, int n_img, float* scores, void* cuda_stream);
+int ytk_op_rt_gather_queries_f32(const float* om, int D, const int* idx_dev, int K, const int* level_h,
+                                 const int* level_w, int n_levels, int n_img, float* tgt, void* tgt16,
+                                 const float* anchors, float* anchor_sel, void* cuda_stream);
+int ytk_op_rt_ref_update_f32(const float* delta, long long ldd, const float* anchor_sel, float* ref, int n,
+                             void* cuda_stream);
+int ytk_op_rt_qpos_l0_f32(const float* ref, const float* W, const float* b, int H1, void* out, int rows,
+                          void* cuda_stream);
+
 /* ---- Device-side front half of the DBNet post-processing (reference postprocessor/dbnet_postporcessor.py:39-82:
  * binarize, findContours, and the pixel work of minAreaRect / box_score_fast).  One record per horizontal run of an
  * 8-connected component of (prob > thresh). ---- */
@@ -283,6 +319,22 @@ int ytk_op_refine_embed(const int* raw, const int* row_group, const int* group_l
                         const float* b_c, void* cin, int* klen, int* kpad, void* cuda_stream);
 int ytk_op_apply_rep_cut(const int* rep_cut, int B, int S, int C, int eos_id, int* ids, float* probs,
                          void* cuda_stream);
+
+/* op level, for the parity tests: the recognizer's input path (timm PatchEmbed's im2col, reference
+ * parseq_transformer.py:220-227).  Writes A [tokens, Kpad] fp16, token row t of a crop = its patch (gy, gx), columns
+ * c * ph * pw + py * pw + px = the normalised pixel (u / 255 - 0.5) / 0.5 (-1 right of the stored canvas width w),
+ * columns 3 * ph * pw .. Kpad = 0; and x [tokens, D] fp32 = pos_embed [*, D] row gy * full_gw + gx.  32 % ph == 0,
+ * Kpad >= 3 * ph * pw, 1..65535 crops.  Device pointers; asynchronous on the stream; invalid arguments are an error, not
+ * a launch.
+ *   u8   crops: packed RGB canvases [32][w][3]; descs_dev: ncrops records on the device (pix_off, w, wp, tok_off and ntok
+ *        are read: wp a multiple of pw with wp / pw <= full_gw, w <= wp, ntok = (32 / ph) * (wp / pw)); rows outside
+ *        every crop's [tok_off, tok_off + ntok) are not written.
+ *   f32  images (B, 3, 32, W) fp32, already normalised, as fed to PARSeq.forward: A holds their fp16 values; W a multiple
+ *        of pw with W / pw <= full_gw; crop b's tokens are rows b * ntok ... */
+int ytk_op_patchify_u8(const uint8_t* crops, const ytk_crop* descs_dev, int ncrops, int ph, int pw, int Kpad,
+                       const float* pos_embed, int full_gw, int D, void* A, float* x, void* cuda_stream);
+int ytk_op_patchify_f32(const float* images, int B, int W, int ph, int pw, int Kpad, const float* pos_embed, int full_gw,
+                        int D, void* A, float* x, void* cuda_stream);
 
 /* op level, for the parity tests: the DBNet detector's own kernels, each called as the engine calls it.  Activations
  * are NHWC fp16 on the device, 16-byte aligned; weights are the reference's fp32 layouts on the host, packed by the

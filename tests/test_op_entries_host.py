@@ -397,3 +397,193 @@ def test_conv2d_refusals(lib, kwargs, fragment):
     before = lib.ytk_launch_count()
     _refused(lib, _conv(lib, **kwargs), fragment)
     assert lib.ytk_launch_count() == before
+
+
+# ======================================================================================================== RT-DETRv2 glue
+def _avgpool(lib, src=P, n=1, H=160, W=160, C=256, out=P):
+    return lib.ytk_op_rt_avgpool2_f16(src, n, H, W, C, out, None)
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(src=None), b"null argument"), (dict(out=None), b"null argument"),
+    (dict(n=0), b"n 0, 160x160, C 256 unsupported"), (dict(H=7), b"7x160"), (dict(W=161), b"160x161"),
+    (dict(H=0, W=0), b"0x0"), (dict(C=12), b"C 12 unsupported"), (dict(C=0), b"C 0 unsupported"),
+    (dict(src=P + 8), b"16-byte aligned"), (dict(out=P + 2), b"16-byte aligned"),
+])
+def test_rt_avgpool2_refusals(lib, kwargs, fragment):
+    before = lib.ytk_launch_count()
+    _refused(lib, _avgpool(lib, **kwargs), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+def _nearest(lib, src=P, lds=512, n=1, Hs=20, Ws=20, C=256, dst=P, ldd=512, coff=0):
+    return lib.ytk_op_rt_upsample_nearest2_f16(src, lds, n, Hs, Ws, C, dst, ldd, coff, None)
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(src=None), b"null argument"), (dict(dst=None), b"null argument"),
+    (dict(n=0), b"n 0, 20x20, C 256"), (dict(Hs=0), b"0x20"), (dict(Ws=-1), b"20x-1"),
+    (dict(C=252), b"C 252 unsupported"), (dict(C=0), b"C 0 unsupported"),
+    # 16-byte vectors: pitches and the column offset in whole groups of 8 fp16
+    (dict(lds=516), b"lds 516, ldd 512, coff 0 must be non-negative multiples of 8"),
+    (dict(ldd=516), b"lds 512, ldd 516, coff 0 must be"), (dict(coff=4), b"coff 4 must be"),
+    (dict(coff=-8), b"coff -8 must be"),
+    (dict(lds=248), b"pitches too small (lds 248 for C 256"),
+    (dict(coff=264), b"ldd 512 for channels [264, 520))"), (dict(ldd=248), b"ldd 248 for channels [0, 256))"),
+    (dict(src=P + 8), b"16-byte aligned"), (dict(dst=P + 2), b"16-byte aligned"),
+])
+def test_rt_upsample_nearest2_refusals(lib, kwargs, fragment):
+    before = lib.ytk_launch_count()
+    _refused(lib, _nearest(lib, **kwargs), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+def _add(lib, a=P, b=P, b_f32=None, C=256, period=1, out=P, rows=400):
+    return lib.ytk_op_rt_add_f16(a, b, b_f32, C, period, out, rows, None)
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(a=None), b"exactly one of b / b_f32"), (dict(out=None), b"exactly one of b / b_f32"),
+    (dict(b=None), b"exactly one of b / b_f32"), (dict(b_f32=P), b"exactly one of b / b_f32"),
+    (dict(C=252), b"C 252, period 1 unsupported"), (dict(C=0), b"C 0, period"), (dict(rows=0), b"0 rows"),
+    (dict(b=None, b_f32=P, period=0), b"period 0 unsupported"),
+    (dict(a=P + 8), b"16-byte aligned"), (dict(b=P + 4), b"16-byte aligned"), (dict(out=P + 2), b"16-byte aligned"),
+])
+def test_rt_add_refusals(lib, kwargs, fragment):
+    before = lib.ytk_launch_count()
+    _refused(lib, _add(lib, **kwargs), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+def _lv(hw=((80, 80), (40, 40), (20, 20))):
+    return _levels(hw, [1] * len(hw))[:2]
+
+
+def _level_cases(n_levels_key="n_levels"):
+    """refusals of the shared level-table check (the deformable attention entry's, without points)"""
+    return [
+        (dict(level_arrays=(None, None)), b"null argument"), (dict(**{n_levels_key: 0}), b"0 levels unsupported"),
+        (dict(**{n_levels_key: 5}), b"5 levels unsupported"),
+        (dict(hw=((80, 80), (40, 0), (20, 20))), b"level 1 is 40x0"), (dict(hw=((-1, 80),)), b"level 0 is -1x80"),
+        (dict(hw=((65536, 32768),)), b"levels 0..0 hold more than"),
+    ]
+
+
+def _mask(lib, x=P, D=256, bias=P, invalid=P, n_invalid=100, hw=((80, 80), (40, 40), (20, 20)), level_arrays=None,
+          n_levels=None, n_img=2):
+    h, w = level_arrays if level_arrays is not None else _lv(hw)
+    return lib.ytk_op_rt_mask_invalid_f32(x, D, bias, invalid, n_invalid, h, w, len(hw) if n_levels is None else n_levels,
+                                          n_img, None)
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(x=None), b"null argument"), (dict(bias=None), b"null argument"), (dict(invalid=None), b"null argument"),
+    (dict(D=0), b"D 0, 100 invalid anchors, n_img 2"), (dict(n_invalid=-1), b"-1 invalid anchors"),
+    (dict(n_img=0), b"n_img 0 unsupported"),
+] + _level_cases())
+def test_rt_mask_invalid_refusals(lib, kwargs, fragment):
+    before = lib.ytk_launch_count()
+    _refused(lib, _mask(lib, **kwargs), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+def test_rt_mask_invalid_without_anchors_launches_nothing(lib):
+    before = lib.ytk_launch_count()
+    assert _mask(lib, invalid=None, n_invalid=0) == 0
+    assert lib.ytk_launch_count() == before
+
+
+def _scores(lib, logits=P, ldl=8, C=6, hw=((80, 80), (40, 40), (20, 20)), level_arrays=None, n_levels=None, n_img=2,
+            scores=P):
+    h, w = level_arrays if level_arrays is not None else _lv(hw)
+    return lib.ytk_op_rt_enc_scores_f32(logits, ldl, C, h, w, len(hw) if n_levels is None else n_levels, n_img, scores,
+                                        None)
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(logits=None), b"null argument"), (dict(scores=None), b"null argument"),
+    (dict(C=0), b"C 0, ldl 8, n_img 2 unsupported"), (dict(C=9), b"C 9, ldl 8"), (dict(n_img=0), b"n_img 0"),
+] + _level_cases())
+def test_rt_enc_scores_refusals(lib, kwargs, fragment):
+    before = lib.ytk_launch_count()
+    _refused(lib, _scores(lib, **kwargs), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+def _gather(lib, om=P, D=256, idx=P, K=300, hw=((80, 80), (40, 40), (20, 20)), level_arrays=None, n_levels=None,
+            n_img=2, tgt=P, tgt16=P, anchors=P, asel=P):
+    h, w = level_arrays if level_arrays is not None else _lv(hw)
+    return lib.ytk_op_rt_gather_queries_f32(om, D, idx, K, h, w, len(hw) if n_levels is None else n_levels, n_img, tgt,
+                                            tgt16, anchors, asel, None)
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(om=None), b"null argument"), (dict(idx=None), b"null argument"), (dict(tgt=None), b"null argument"),
+    (dict(tgt16=None), b"null argument"), (dict(anchors=None), b"null argument"), (dict(asel=None), b"null argument"),
+    (dict(D=0), b"D 0, K 300, n_img 2 unsupported"), (dict(K=0), b"K 0"), (dict(n_img=0), b"n_img 0"),
+    (dict(K=1 << 30, n_img=4), b"K 1073741824, n_img 4"),
+] + _level_cases())
+def test_rt_gather_queries_refusals(lib, kwargs, fragment):
+    before = lib.ytk_launch_count()
+    _refused(lib, _gather(lib, **kwargs), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(delta=None), b"null argument"), (dict(ref=None), b"null argument"),
+    (dict(n=0), b"0 boxes"), (dict(n=1 << 29), b"536870912 boxes"), (dict(ldd=3), b"ldd 3 unsupported"),
+])
+def test_rt_ref_update_refusals(lib, kwargs, fragment):
+    a = dict(delta=P, ldd=4, asel=None, ref=P, n=600)
+    a.update(kwargs)
+    before = lib.ytk_launch_count()
+    _refused(lib, lib.ytk_op_rt_ref_update_f32(a["delta"], a["ldd"], a["asel"], a["ref"], a["n"], None), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+@pytest.mark.parametrize("kwargs,fragment", [
+    (dict(ref=None), b"null argument"), (dict(W=None), b"null argument"), (dict(b=None), b"null argument"),
+    (dict(out=None), b"null argument"), (dict(H1=0), b"H1 0, 600 rows"), (dict(rows=0), b"0 rows"),
+    (dict(ref=P + 8), b"16-byte aligned"), (dict(W=P + 4), b"16-byte aligned"),
+])
+def test_rt_qpos_l0_refusals(lib, kwargs, fragment):
+    a = dict(ref=P, W=P, b=P, H1=512, out=P, rows=600)
+    a.update(kwargs)
+    before = lib.ytk_launch_count()
+    _refused(lib, lib.ytk_op_rt_qpos_l0_f32(a["ref"], a["W"], a["b"], a["H1"], a["out"], a["rows"], None), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+# ======================================================================================================== PARSeq patchify
+_PATCH_CASES = [
+    (dict(pos=None), b"null argument"), (dict(A=None), b"null argument"), (dict(x=None), b"null argument"),
+    (dict(n=0), b"0 images"), (dict(n=65536), b"65536 images"),
+    (dict(ph=3), b"patch 3x8"), (dict(ph=0), b"patch 0x8"), (dict(pw=0), b"patch 4x0"), (dict(ph=64), b"patch 64x8"),
+    (dict(full_gw=0), b"full_gw 0"), (dict(D=0), b"D 0 unsupported"),
+    (dict(Kpad=95), b"Kpad 95 < 3 * 4 * 8"), (dict(ph=8, pw=8, Kpad=128), b"Kpad 128 < 3 * 8 * 8"),
+]
+
+
+@pytest.mark.parametrize("kwargs,fragment", _PATCH_CASES + [(dict(src=None), b"null argument"),
+                                                             (dict(descs=None), b"null argument")])
+def test_patchify_u8_refusals(lib, kwargs, fragment):
+    a = dict(src=P, descs=P, n=4, ph=4, pw=8, Kpad=128, pos=P, full_gw=100, D=192, A=P, x=P)
+    a.update(kwargs)
+    before = lib.ytk_launch_count()
+    _refused(lib, lib.ytk_op_patchify_u8(a["src"], a["descs"], a["n"], a["ph"], a["pw"], a["Kpad"], a["pos"],
+                                         a["full_gw"], a["D"], a["A"], a["x"], None), fragment)
+    assert lib.ytk_launch_count() == before
+
+
+@pytest.mark.parametrize("kwargs,fragment", _PATCH_CASES + [
+    (dict(src=None), b"null argument"),
+    (dict(W=100), b"W 100 unsupported"), (dict(W=0), b"W 0 unsupported"), (dict(W=-8), b"W -8 unsupported"),
+    (dict(W=808), b"W 808 unsupported (a positive multiple of pw 8, at most full_gw 100"),
+])
+def test_patchify_f32_refusals(lib, kwargs, fragment):
+    a = dict(src=P, n=4, W=128, ph=4, pw=8, Kpad=128, pos=P, full_gw=100, D=192, A=P, x=P)
+    a.update(kwargs)
+    before = lib.ytk_launch_count()
+    _refused(lib, lib.ytk_op_patchify_f32(a["src"], a["n"], a["W"], a["ph"], a["pw"], a["Kpad"], a["pos"],
+                                          a["full_gw"], a["D"], a["A"], a["x"], None), fragment)
+    assert lib.ytk_launch_count() == before

@@ -88,6 +88,31 @@ def _declare(lib):
     lib.ytk_op_dbnet_head_f32.restype = c_int
     lib.ytk_op_dbnet_head_f32.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, ctypes.c_float,
                                           c_void_p, c_void_p]
+    lib.ytk_op_rt_avgpool2_f16.restype = c_int
+    lib.ytk_op_rt_avgpool2_f16.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
+    lib.ytk_op_rt_upsample_nearest2_f16.restype = c_int
+    lib.ytk_op_rt_upsample_nearest2_f16.argtypes = [c_void_p, c_ll, c_int, c_int, c_int, c_int, c_void_p, c_ll, c_int,
+                                                    c_void_p]
+    lib.ytk_op_rt_add_f16.restype = c_int
+    lib.ytk_op_rt_add_f16.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_ll, c_void_p]
+    lib.ytk_op_rt_mask_invalid_f32.restype = c_int
+    lib.ytk_op_rt_mask_invalid_f32.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int,
+                                               c_int, c_void_p]
+    lib.ytk_op_rt_enc_scores_f32.restype = c_int
+    lib.ytk_op_rt_enc_scores_f32.argtypes = [c_void_p, c_ll, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p]
+    lib.ytk_op_rt_gather_queries_f32.restype = c_int
+    lib.ytk_op_rt_gather_queries_f32.argtypes = [c_void_p, c_int, c_void_p, c_int, c_void_p, c_void_p, c_int, c_int,
+                                                 c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
+    lib.ytk_op_rt_ref_update_f32.restype = c_int
+    lib.ytk_op_rt_ref_update_f32.argtypes = [c_void_p, c_ll, c_void_p, c_void_p, c_int, c_void_p]
+    lib.ytk_op_rt_qpos_l0_f32.restype = c_int
+    lib.ytk_op_rt_qpos_l0_f32.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_void_p]
+    lib.ytk_op_patchify_u8.restype = c_int
+    lib.ytk_op_patchify_u8.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p,
+                                       c_void_p, c_void_p]
+    lib.ytk_op_patchify_f32.restype = c_int
+    lib.ytk_op_patchify_f32.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p,
+                                        c_void_p, c_void_p]
     lib.ytk_op_assign_best_overlap_f64.restype = c_int
     lib.ytk_op_assign_best_overlap_f64.argtypes = [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_int,
                                                    ctypes.c_double, c_void_p, c_void_p, c_ll, c_void_p]

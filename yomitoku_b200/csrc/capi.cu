@@ -200,15 +200,47 @@ int ytk_op_topk_f32(const float* scores_dev, int n, int L, int K, int* out_idx_d
 
 static bool misaligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; }
 
+// The decoder's level table from host arrays of n_levels sizes (and sampling points, where the kernel reads them: pass
+// NULL otherwise, and the points stay 0).  Returns false after set_error on a bad table.
+static bool rt_levels(const char* who, const int* level_h, const int* level_w, const int* level_points, int n_levels,
+                      ytk::RtLevels* lv) {
+    if (!level_h || !level_w) {
+        ytk::set_error("%s: null argument", who);
+        return false;
+    }
+    if (n_levels < 1 || n_levels > ytk::RtLevels::kMax) {
+        ytk::set_error("%s: %d levels unsupported (1..%d)", who, n_levels, ytk::RtLevels::kMax);
+        return false;
+    }
+    lv->n = n_levels;
+    lv->off[0] = 0;
+    for (int l = 0; l < n_levels; ++l) {
+        const int p = level_points ? level_points[l] : 0;
+        if (level_h[l] < 1 || level_w[l] < 1 || (level_points && p < 1)) {
+            if (level_points)
+                ytk::set_error("%s: level %d is %dx%d with %d points", who, l, level_h[l], level_w[l], p);
+            else
+                ytk::set_error("%s: level %d is %dx%d", who, l, level_h[l], level_w[l]);
+            return false;
+        }
+        if ((long long)lv->off[l] + (long long)level_h[l] * level_w[l] > INT_MAX) {
+            ytk::set_error("%s: levels 0..%d hold more than %d anchors", who, l, INT_MAX);
+            return false;
+        }
+        lv->h[l] = level_h[l];
+        lv->w[l] = level_w[l];
+        lv->points[l] = p;
+        lv->off[l + 1] = lv->off[l] + level_h[l] * level_w[l];
+    }
+    lv->total = lv->off[n_levels];
+    return true;
+}
+
 int ytk_op_deform_attn_f16(const float* ow, long long ldo, const float* ref, const void* value, long long ldv, int voff,
                            const int* level_h, const int* level_w, const int* level_points, int n_levels, int n_img, int K,
                            int heads, int head_dim, float offset_scale, void* out, long long ldout, void* cuda_stream) {
     if (!ow || !ref || !value || !out || !level_h || !level_w || !level_points) {
         ytk::set_error("ytk_op_deform_attn_f16: null argument");
-        return YTK_ERR;
-    }
-    if (n_levels < 1 || n_levels > ytk::RtLevels::kMax) {
-        ytk::set_error("ytk_op_deform_attn_f16: %d levels unsupported (1..%d)", n_levels, ytk::RtLevels::kMax);
         return YTK_ERR;
     }
     if (n_img < 1 || K < 1 || heads < 1 || head_dim < 1 || voff < 0) {
@@ -217,22 +249,9 @@ int ytk_op_deform_attn_f16(const float* ow, long long ldo, const float* ref, con
         return YTK_ERR;
     }
     ytk::RtLevels lv;
-    lv.n = n_levels;
-    lv.off[0] = 0;
+    if (!rt_levels("ytk_op_deform_attn_f16", level_h, level_w, level_points, n_levels, &lv)) return YTK_ERR;
     int P = 0;
-    for (int l = 0; l < n_levels; ++l) {
-        if (level_h[l] < 1 || level_w[l] < 1 || level_points[l] < 1) {
-            ytk::set_error("ytk_op_deform_attn_f16: level %d is %dx%d with %d points", l, level_h[l], level_w[l],
-                           level_points[l]);
-            return YTK_ERR;
-        }
-        lv.h[l] = level_h[l];
-        lv.w[l] = level_w[l];
-        lv.points[l] = level_points[l];
-        lv.off[l + 1] = lv.off[l] + level_h[l] * level_w[l];
-        P += level_points[l];
-    }
-    lv.total = lv.off[n_levels];
+    for (int l = 0; l < n_levels; ++l) P += lv.points[l];
     if (ldo < 3LL * heads * P || ldv < (long long)voff + (long long)heads * head_dim || ldout < (long long)heads * head_dim ||
         misaligned(ref, 16)) {
         ytk::set_error("ytk_op_deform_attn_f16: pitches too small (ldo %lld, ldv %lld with voff %d, ldout %lld) or ref not "
@@ -241,6 +260,211 @@ int ytk_op_deform_attn_f16(const float* ow, long long ldo, const float* ref, con
     }
     return ytk::launch_rt_deform_attn(ow, ldo, ref, value, ldv, voff, lv, n_img, K, heads, head_dim, offset_scale, out,
                                       ldout, static_cast<cudaStream_t>(cuda_stream))
+               ? YTK_ERR
+               : YTK_OK;
+}
+
+int ytk_op_rt_avgpool2_f16(const void* in, int n, int H, int W, int C, void* out, void* cuda_stream) {
+    if (!in || !out) {
+        ytk::set_error("ytk_op_rt_avgpool2_f16: null argument");
+        return YTK_ERR;
+    }
+    if (n < 1 || H < 2 || W < 2 || (H | W) & 1 || C < 8 || C % 8) {
+        ytk::set_error("ytk_op_rt_avgpool2_f16: n %d, %dx%d, C %d unsupported (H, W even, C a positive multiple of 8)", n,
+                       H, W, C);
+        return YTK_ERR;
+    }
+    if (misaligned(in, 16) || misaligned(out, 16)) {
+        ytk::set_error("ytk_op_rt_avgpool2_f16: in and out must be 16-byte aligned");
+        return YTK_ERR;
+    }
+    return ytk::launch_rt_avgpool2(in, out, n, H, W, C, static_cast<cudaStream_t>(cuda_stream)) ? YTK_ERR : YTK_OK;
+}
+
+int ytk_op_rt_upsample_nearest2_f16(const void* src, long long lds, int n, int Hs, int Ws, int C, void* dst,
+                                    long long ldd, int coff, void* cuda_stream) {
+    if (!src || !dst) {
+        ytk::set_error("ytk_op_rt_upsample_nearest2_f16: null argument");
+        return YTK_ERR;
+    }
+    if (n < 1 || Hs < 1 || Ws < 1 || C < 8 || C % 8) {
+        ytk::set_error("ytk_op_rt_upsample_nearest2_f16: n %d, %dx%d, C %d unsupported (C a positive multiple of 8)", n,
+                       Hs, Ws, C);
+        return YTK_ERR;
+    }
+    // the kernel moves 16-byte vectors: every row start and the column offset must be a multiple of 8 elements
+    if (lds % 8 || ldd % 8 || coff < 0 || coff % 8) {
+        ytk::set_error("ytk_op_rt_upsample_nearest2_f16: lds %lld, ldd %lld, coff %d must be non-negative multiples of 8",
+                       lds, ldd, coff);
+        return YTK_ERR;
+    }
+    if (lds < C || ldd < (long long)coff + C) {
+        ytk::set_error("ytk_op_rt_upsample_nearest2_f16: pitches too small (lds %lld for C %d, ldd %lld for channels "
+                       "[%d, %d))", lds, C, ldd, coff, coff + C);
+        return YTK_ERR;
+    }
+    if (misaligned(src, 16) || misaligned(dst, 16)) {
+        ytk::set_error("ytk_op_rt_upsample_nearest2_f16: src and dst must be 16-byte aligned");
+        return YTK_ERR;
+    }
+    return ytk::launch_rt_upsample_nearest2(src, lds, n, Hs, Ws, C, dst, ldd, coff,
+                                            static_cast<cudaStream_t>(cuda_stream))
+               ? YTK_ERR
+               : YTK_OK;
+}
+
+int ytk_op_rt_add_f16(const void* a, const void* b, const float* b_f32, int C, int period, void* out, long long rows,
+                      void* cuda_stream) {
+    if (!a || !out || (!b == !b_f32)) {
+        ytk::set_error("ytk_op_rt_add_f16: a and out, and exactly one of b / b_f32, must be given");
+        return YTK_ERR;
+    }
+    if (rows < 1 || C < 8 || C % 8 || (b_f32 && period < 1)) {
+        ytk::set_error("ytk_op_rt_add_f16: %lld rows, C %d, period %d unsupported (C a positive multiple of 8, period "
+                       ">= 1 with b_f32)", rows, C, period);
+        return YTK_ERR;
+    }
+    if (misaligned(a, 16) || misaligned(b, 16) || misaligned(out, 16)) {
+        ytk::set_error("ytk_op_rt_add_f16: a, b and out must be 16-byte aligned");
+        return YTK_ERR;
+    }
+    return ytk::launch_rt_add(a, b, b_f32, C, period, out, rows, static_cast<cudaStream_t>(cuda_stream)) ? YTK_ERR
+                                                                                                         : YTK_OK;
+}
+
+int ytk_op_rt_mask_invalid_f32(float* x, int D, const float* bias, const int* invalid_dev, int n_invalid,
+                               const int* level_h, const int* level_w, int n_levels, int n_img, void* cuda_stream) {
+    const char* who = "ytk_op_rt_mask_invalid_f32";
+    if (!x || !bias || (n_invalid > 0 && !invalid_dev)) {
+        ytk::set_error("%s: null argument", who);
+        return YTK_ERR;
+    }
+    if (D < 1 || n_invalid < 0 || n_img < 1 || (long long)n_invalid * n_img > INT_MAX) {
+        ytk::set_error("%s: D %d, %d invalid anchors, n_img %d unsupported", who, D, n_invalid, n_img);
+        return YTK_ERR;
+    }
+    ytk::RtLevels lv;
+    if (!rt_levels(who, level_h, level_w, nullptr, n_levels, &lv)) return YTK_ERR;
+    return ytk::launch_rt_mask_invalid(x, D, bias, invalid_dev, n_invalid, lv, n_img,
+                                       static_cast<cudaStream_t>(cuda_stream))
+               ? YTK_ERR
+               : YTK_OK;
+}
+
+int ytk_op_rt_enc_scores_f32(const float* logits, long long ldl, int C, const int* level_h, const int* level_w,
+                             int n_levels, int n_img, float* scores, void* cuda_stream) {
+    const char* who = "ytk_op_rt_enc_scores_f32";
+    if (!logits || !scores) {
+        ytk::set_error("%s: null argument", who);
+        return YTK_ERR;
+    }
+    if (C < 1 || ldl < C || n_img < 1) {
+        ytk::set_error("%s: C %d, ldl %lld, n_img %d unsupported (1 <= C <= ldl)", who, C, ldl, n_img);
+        return YTK_ERR;
+    }
+    ytk::RtLevels lv;
+    if (!rt_levels(who, level_h, level_w, nullptr, n_levels, &lv)) return YTK_ERR;
+    return ytk::launch_rt_enc_scores(logits, ldl, C, lv, n_img, scores, static_cast<cudaStream_t>(cuda_stream))
+               ? YTK_ERR
+               : YTK_OK;
+}
+
+int ytk_op_rt_gather_queries_f32(const float* om, int D, const int* idx_dev, int K, const int* level_h,
+                                 const int* level_w, int n_levels, int n_img, float* tgt, void* tgt16,
+                                 const float* anchors, float* anchor_sel, void* cuda_stream) {
+    const char* who = "ytk_op_rt_gather_queries_f32";
+    if (!om || !idx_dev || !tgt || !tgt16 || !anchors || !anchor_sel) {
+        ytk::set_error("%s: null argument", who);
+        return YTK_ERR;
+    }
+    if (D < 1 || K < 1 || n_img < 1 || (long long)n_img * K > INT_MAX) {
+        ytk::set_error("%s: D %d, K %d, n_img %d unsupported", who, D, K, n_img);
+        return YTK_ERR;
+    }
+    ytk::RtLevels lv;
+    if (!rt_levels(who, level_h, level_w, nullptr, n_levels, &lv)) return YTK_ERR;
+    return ytk::launch_rt_gather_queries(om, D, idx_dev, K, lv, n_img, tgt, tgt16, anchors, anchor_sel,
+                                         static_cast<cudaStream_t>(cuda_stream))
+               ? YTK_ERR
+               : YTK_OK;
+}
+
+int ytk_op_rt_ref_update_f32(const float* delta, long long ldd, const float* anchor_sel, float* ref, int n,
+                             void* cuda_stream) {
+    if (!delta || !ref) {
+        ytk::set_error("ytk_op_rt_ref_update_f32: null argument");
+        return YTK_ERR;
+    }
+    if (n < 1 || n > INT_MAX / 4 || ldd < 4) {
+        ytk::set_error("ytk_op_rt_ref_update_f32: %d boxes, ldd %lld unsupported (ldd >= 4)", n, ldd);
+        return YTK_ERR;
+    }
+    return ytk::launch_rt_ref_update(delta, ldd, anchor_sel, ref, n, static_cast<cudaStream_t>(cuda_stream)) ? YTK_ERR
+                                                                                                            : YTK_OK;
+}
+
+int ytk_op_rt_qpos_l0_f32(const float* ref, const float* W, const float* b, int H1, void* out, int rows,
+                          void* cuda_stream) {
+    if (!ref || !W || !b || !out) {
+        ytk::set_error("ytk_op_rt_qpos_l0_f32: null argument");
+        return YTK_ERR;
+    }
+    if (H1 < 1 || rows < 1) {
+        ytk::set_error("ytk_op_rt_qpos_l0_f32: H1 %d, %d rows unsupported", H1, rows);
+        return YTK_ERR;
+    }
+    if (misaligned(ref, 16) || misaligned(W, 16)) {
+        ytk::set_error("ytk_op_rt_qpos_l0_f32: ref and W must be 16-byte aligned (the kernel reads float4)");
+        return YTK_ERR;
+    }
+    return ytk::launch_rt_qpos_l0(ref, W, b, H1, out, rows, static_cast<cudaStream_t>(cuda_stream)) ? YTK_ERR : YTK_OK;
+}
+
+// The shape conditions both patchify entries share.
+static bool bad_patch(const char* who, int nimg, int ph, int pw, int Kpad, int full_gw, int D) {
+    if (nimg < 1 || nimg > 65535 || ph < 1 || pw < 1 || 32 % ph || full_gw < 1 || D < 1) {
+        ytk::set_error("%s: %d images, patch %dx%d, full_gw %d, D %d unsupported (1..65535 images, 32 %% ph == 0)", who,
+                       nimg, ph, pw, full_gw, D);
+        return true;
+    }
+    if (Kpad < 3 * ph * pw) {
+        ytk::set_error("%s: Kpad %d < 3 * %d * %d", who, Kpad, ph, pw);
+        return true;
+    }
+    return false;
+}
+
+static_assert(sizeof(ytk_crop) == sizeof(ytk::CropDesc), "ytk_crop and ytk::CropDesc must have one layout");
+
+int ytk_op_patchify_u8(const uint8_t* crops, const ytk_crop* descs_dev, int ncrops, int ph, int pw, int Kpad,
+                       const float* pos_embed, int full_gw, int D, void* A, float* x, void* cuda_stream) {
+    const char* who = "ytk_op_patchify_u8";
+    if (!crops || !descs_dev || !pos_embed || !A || !x) {
+        ytk::set_error("%s: null argument", who);
+        return YTK_ERR;
+    }
+    if (bad_patch(who, ncrops, ph, pw, Kpad, full_gw, D)) return YTK_ERR;
+    return ytk::launch_patchify_u8(crops, reinterpret_cast<const ytk::CropDesc*>(descs_dev), ncrops, ph, pw, Kpad,
+                                   pos_embed, full_gw, D, A, x, 0, static_cast<cudaStream_t>(cuda_stream))
+               ? YTK_ERR
+               : YTK_OK;
+}
+
+int ytk_op_patchify_f32(const float* images, int B, int W, int ph, int pw, int Kpad, const float* pos_embed, int full_gw,
+                        int D, void* A, float* x, void* cuda_stream) {
+    const char* who = "ytk_op_patchify_f32";
+    if (!images || !pos_embed || !A || !x) {
+        ytk::set_error("%s: null argument", who);
+        return YTK_ERR;
+    }
+    if (bad_patch(who, B, ph, pw, Kpad, full_gw, D)) return YTK_ERR;
+    if (W < pw || W % pw || W / pw > full_gw) {
+        ytk::set_error("%s: W %d unsupported (a positive multiple of pw %d, at most full_gw %d patches)", who, W, pw,
+                       full_gw);
+        return YTK_ERR;
+    }
+    return ytk::launch_patchify_f32(images, B, W, ph, pw, Kpad, pos_embed, full_gw, D, A, x,
+                                    static_cast<cudaStream_t>(cuda_stream))
                ? YTK_ERR
                : YTK_OK;
 }
