@@ -9,7 +9,15 @@ The constructors, the `configs` dict and the call contracts mirror kotaro-kinosh
 layout_analyzer,table_cell_detector,table_semantic_parser}.py); the models (DBNet++, PARSeq, RT-DETRv2) run as hand-written sm_90a CUDA kernels behind the C ABI
 in include/yomitoku_b200.h (libytk_b200.so).  Pages may be BGR numpy arrays or already on the GPU: uint8 CUDA tensors or
 a `DevicePages` made by `device_pages` (device_pages.py).
+
+Files in, documents out:
+
+    from yomitoku_b200 import load_image                  # the pages of an image file (every TIFF frame), BGR
+    from yomitoku_b200.export import export_markdown, export_html, export_csv, export_json
+    result.to_markdown(path, img=page)                    # also to_html / to_csv (DocumentAnalyzerSchema)
+    python -m yomitoku_b200 <file-or-dir> -f md -o out    # the command line (cli.py): batched analyze_pages
 """
+from .data import load_image
 from .device_pages import DevicePages, device_pages
 from .document_analyzer import DocumentAnalyzer
 from .layout_analyzer import LayoutAnalyzer
@@ -22,4 +30,5 @@ from .text_detector import TextDetector
 from .text_recognizer import TextRecognizer
 
 __all__ = ["OCR", "TextDetector", "TextRecognizer", "DocumentAnalyzer", "LayoutAnalyzer", "LayoutParser",
-           "TableStructureRecognizer", "CellDetector", "TableSemanticParser", "DevicePages", "device_pages"]
+           "TableStructureRecognizer", "CellDetector", "TableSemanticParser", "DevicePages", "device_pages",
+           "load_image"]

@@ -7,13 +7,62 @@ shrink or grow; the functions here serve the model-level seam), and the crop ext
 `crop_geometry` / `crop_records` below compute the per-quad records (everything that follows from the quads alone).
 """
 from concurrent.futures import ThreadPoolExecutor
+from pathlib import Path
 
 import cv2
 import numpy as np
 import torch
+from PIL import Image
+
+from .base import set_logger
+
+logger = set_logger(__name__, "WARNING")
 
 IMAGENET_MEAN = (0.485, 0.456, 0.406)
 IMAGENET_STD = (0.229, 0.224, 0.225)
+
+SUPPORT_INPUT_FORMAT = ["jpg", "jpeg", "png", "bmp", "tiff", "tif"]
+MIN_IMAGE_SIZE = 32
+WARNING_IMAGE_SIZE = 720
+
+
+# ------------------------------------------------------------------------------------------------ page files
+def validate_image(img):
+    """A page with a side under 32 px is refused; a shorter side under 720 px is read with a warning (reference
+    data/functions.py:19-30)."""
+    h, w = img.shape[:2]
+    if h < MIN_IMAGE_SIZE or w < MIN_IMAGE_SIZE:
+        raise ValueError("Image size is too small.")
+    if min(h, w) < WARNING_IMAGE_SIZE:
+        logger.warning("The image size is small (%dx%d), which may result in reduced OCR accuracy. The process will "
+                       "continue; pages with a shorter side of at least 720 pixels are recommended." % (w, h))
+
+
+def load_image(image_path):
+    """The pages of an image file as a list of BGR uint8 arrays (reference data/functions.py:33-78): jpg, jpeg, png,
+    bmp, tif and tiff, opened with Pillow and converted to RGB; every frame of a TIFF is a page, each checked by
+    `validate_image`.  PDF files are refused: rendering PDF pages is not part of this package."""
+    image_path = Path(image_path)
+    if not image_path.exists():
+        raise FileNotFoundError(f"File not found: {image_path}")
+    ext = image_path.suffix[1:].lower()
+    if ext == "pdf":
+        raise ValueError(f"{image_path}: PDF input is not supported, rendering PDF pages is not part of this package "
+                         f"(it has no PDF renderer); convert the pages to images first")
+    if ext not in SUPPORT_INPUT_FORMAT:
+        raise ValueError(f"Unsupported image format. Supported formats are {SUPPORT_INPUT_FORMAT}")
+    try:
+        img = Image.open(image_path)
+    except Exception:
+        raise ValueError("Invalid image data.") from None
+    frames = getattr(img, "n_frames", 1) if ext in ("tif", "tiff") else 1
+    pages = []
+    for i in range(frames):
+        img.seek(i)
+        rgb = np.asarray(img.convert("RGB"))
+        validate_image(rgb)
+        pages.append(np.ascontiguousarray(rgb[:, :, ::-1]))
+    return pages
 
 
 def shortest_edge_size(h, w, shortest_edge_length, max_length):

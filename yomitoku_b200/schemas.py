@@ -123,6 +123,27 @@ class DocumentAnalyzerSchema(BaseSchema):
     words: List[WordPrediction] = Field(default_factory=list)
     figures: List[FigureSchema] = Field(default_factory=list)
 
+    def to_markdown(self, out_path: str, **kwargs):
+        """export.export_markdown(self, out_path, **kwargs): yomitoku's Markdown file (and figure crops)."""
+        from .export import export_markdown
+        return export_markdown(self, out_path, **kwargs)
+
+    def to_html(self, out_path: str, **kwargs):
+        """export.export_html(self, out_path, **kwargs): yomitoku's HTML element string (not re-indented)."""
+        from .export import export_html
+        return export_html(self, out_path, **kwargs)
+
+    def to_csv(self, out_path: str, **kwargs):
+        """export.export_csv(self, out_path, **kwargs): yomitoku's CSV file (and figure crops)."""
+        from .export import export_csv
+        return export_csv(self, out_path, **kwargs)
+
+    def to_json(self, out_path: str, **kwargs):
+        """The generic BaseSchema.to_json (model_dump, indent 4, keys in field order), unchanged.  yomitoku's
+        `to_json` is its JSON exporter (sorted keys, ignore_line_break, figures, encoding): that file is written by
+        `export.export_json(self, out_path, **kwargs)`."""
+        return super().to_json(out_path, **kwargs)
+
 
 # ------------------------------------------------------------------------------------------------ cell detector
 class CellSchema(BaseSchema):
