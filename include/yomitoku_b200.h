@@ -252,6 +252,15 @@ double ytk_parseq_last_flops(ytk_parseq* h);
 int ytk_parseq_last_steps(ytk_parseq* h);
 /* CUDA-event times (ms) of the last forward: encoder, AR decode, refinement, output copies */
 void ytk_parseq_last_phase_ms(ytk_parseq* h, float* ms4);
+/* test hooks.  set_debug: with on != 0 the next forwards also copy the stages they overwrite in place (no extra
+ * kernels; results and launch counts unchanged).  debug_tensor: copies a stage of the last forward to host fp32
+ * (16-bit operands converted, fp32 as is, integer buffers as int32 bit patterns) at the padded width the engine runs;
+ * shape4 receives rows, cols, 1, 1 (host_out null: shape only).  Names: enc.mem, enc.memkv, enc.x.L (L = 0..depth,
+ * capture), ar.tgt, ar.raw, ar.group_len, ar.rep_cut, dec.klen, dec.kpad, dec.cin, dec.ckv, dec.sa, dec.qc, dec.oc,
+ * dec.mlp, dec.x, dec.out, dec.x_self, dec.x_cross, dec.ctx (the last three: capture), model.q_self, model.ckv0,
+ * model.embed, model.pos_q.  A name the last forward did not produce is an error. */
+int ytk_parseq_set_debug(ytk_parseq* h, int on);
+int ytk_parseq_debug_tensor(ytk_parseq* h, const char* name, float* host_out, long long capacity, int* shape4);
 
 /* op level, for the parity tests: the single-query attention of the AR decoder.  One query per (row, head), head dim
  * D / heads in {32, 48, 64, 96}, fp16 operands with rows of D (queries) and [K | V] rows of 2 * D (keys / values),

@@ -75,41 +75,74 @@ SPECS = {
 
 
 # ----------------------------------------------------------------------------------------------- encoder
-def encoder_forward(sd, spec, images, prefix="encoder."):
-    """reference Encoder.forward / forward_features_dynamic (parseq_transformer.py:206-234). images (B,3,32,W)."""
-    D, heads = spec.embed_dim, spec.enc_heads
-    hd = D // heads
+# The forward is written as a chain of stage functions so that a test can run any one stage on inputs of its choice
+# (in float64, on the inputs a device engine gave that stage) with the same code that produces the fp32 results.
+def layer_norm(sd, name, x, eps):
+    """LayerNorm over the last dim with the parameters `name`.weight / `name`.bias."""
+    return F.layer_norm(x, (x.shape[-1],), sd[name + ".weight"], sd[name + ".bias"], eps)
+
+
+def patch_embed(sd, spec, images, prefix="encoder."):
+    """patch conv -> (B, gh*gw, D) row-major grid + the learned absolute pos_embed cropped to the patch grid
+    (parseq_transformer.py:212-234): grid cell (y, x) takes pos_embed row y * full_gw + x."""
+    D = spec.embed_dim
     x = F.conv2d(images, sd[prefix + "patch_embed.proj.weight"], sd[prefix + "patch_embed.proj.bias"],
                  stride=spec.patch)
     B, _, gh, gw = x.shape
     x = x.flatten(2).transpose(1, 2)                                   # (B, gh*gw, D), row-major grid
     full_gh, full_gw = spec.grid
     pos = sd[prefix + "pos_embed"].reshape(1, full_gh, full_gw, D)[:, :gh, :gw].reshape(1, gh * gw, D)
-    x = x + pos
+    return x + pos
+
+
+def encoder_block(sd, spec, i, x, prefix="encoder."):
+    """timm pre-LN ViT block i: x + proj(attn(LN1 x)), then x + fc2(gelu(fc1(LN2 x))); LayerNorm eps 1e-6."""
+    D, heads = spec.embed_dim, spec.enc_heads
+    hd = D // heads
+    B = x.shape[0]
+    p = "%sblocks.%d." % (prefix, i)
+    h = layer_norm(sd, p + "norm1", x, 1e-6)
+    qkv = F.linear(h, sd[p + "attn.qkv.weight"], sd[p + "attn.qkv.bias"])
+    qkv = qkv.reshape(B, -1, 3, heads, hd).permute(2, 0, 3, 1, 4)   # (3,B,h,N,hd)
+    att = torch.softmax((qkv[0] @ qkv[1].transpose(-1, -2)) * (hd ** -0.5), dim=-1) @ qkv[2]
+    att = att.transpose(1, 2).reshape(B, -1, D)
+    x = x + F.linear(att, sd[p + "attn.proj.weight"], sd[p + "attn.proj.bias"])
+    h = layer_norm(sd, p + "norm2", x, 1e-6)
+    h = F.gelu(F.linear(h, sd[p + "mlp.fc1.weight"], sd[p + "mlp.fc1.bias"]))
+    return x + F.linear(h, sd[p + "mlp.fc2.weight"], sd[p + "mlp.fc2.bias"])
+
+
+def encoder_norm(sd, spec, x, prefix="encoder."):
+    """final LayerNorm of the encoder (eps 1e-6): the decoder's memory."""
+    return layer_norm(sd, prefix + "norm", x, 1e-6)
+
+
+def encoder_forward(sd, spec, images, prefix="encoder."):
+    """reference Encoder.forward / forward_features_dynamic (parseq_transformer.py:206-234). images (B,3,32,W)."""
+    x = patch_embed(sd, spec, images, prefix)
     for i in range(spec.enc_depth):
-        p = "%sblocks.%d." % (prefix, i)
-        h = F.layer_norm(x, (D,), sd[p + "norm1.weight"], sd[p + "norm1.bias"], 1e-6)
-        qkv = F.linear(h, sd[p + "attn.qkv.weight"], sd[p + "attn.qkv.bias"])
-        qkv = qkv.reshape(B, -1, 3, heads, hd).permute(2, 0, 3, 1, 4)   # (3,B,h,N,hd)
-        att = torch.softmax((qkv[0] @ qkv[1].transpose(-1, -2)) * (hd ** -0.5), dim=-1) @ qkv[2]
-        att = att.transpose(1, 2).reshape(B, -1, D)
-        x = x + F.linear(att, sd[p + "attn.proj.weight"], sd[p + "attn.proj.bias"])
-        h = F.layer_norm(x, (D,), sd[p + "norm2.weight"], sd[p + "norm2.bias"], 1e-6)
-        h = F.gelu(F.linear(h, sd[p + "mlp.fc1.weight"], sd[p + "mlp.fc1.bias"]))
-        x = x + F.linear(h, sd[p + "mlp.fc2.weight"], sd[p + "mlp.fc2.bias"])
-    return F.layer_norm(x, (D,), sd[prefix + "norm.weight"], sd[prefix + "norm.bias"], 1e-6)
+        x = encoder_block(sd, spec, i, x, prefix)
+    return encoder_norm(sd, spec, x, prefix)
 
 
 # ----------------------------------------------------------------------------------------------- decoder
-def _mha(sd, p, heads, q_in, kv_in, attn_mask=None, key_padding_mask=None):
-    """torch.nn.MultiheadAttention(batch_first=True) forward (used at parseq_transformer.py:83-92).
-    attn_mask (Lq,Lk) bool, key_padding_mask (B,Lk) bool; True = not allowed."""
+# torch.nn.MultiheadAttention(batch_first=True) forward (used at parseq_transformer.py:83-92) in its three parts:
+# packed in_proj q / (k, v), scaled-dot-product attention with boolean masks (True = masked), out_proj.
+def mha_q(sd, p, q_in):
     D = q_in.shape[-1]
-    hd = D // heads
+    return F.linear(q_in, sd[p + "in_proj_weight"][:D], sd[p + "in_proj_bias"][:D])
+
+
+def mha_kv(sd, p, kv_in):
+    D = kv_in.shape[-1]
     w, b = sd[p + "in_proj_weight"], sd[p + "in_proj_bias"]
-    q = F.linear(q_in, w[:D], b[:D])
-    k = F.linear(kv_in, w[D:2 * D], b[D:2 * D])
-    v = F.linear(kv_in, w[2 * D:], b[2 * D:])
+    return F.linear(kv_in, w[D:2 * D], b[D:2 * D]), F.linear(kv_in, w[2 * D:], b[2 * D:])
+
+
+def mha_attend(q, k, v, heads, attn_mask=None, key_padding_mask=None):
+    """q (B,Lq,D), k / v (B,Lk,D) -> (B,Lq,D).  attn_mask (Lq,Lk) bool, key_padding_mask (B,Lk) bool."""
+    D = q.shape[-1]
+    hd = D // heads
     B, Lq, Lk = q.shape[0], q.shape[1], k.shape[1]
     q = q.reshape(B, Lq, heads, hd).transpose(1, 2)
     k = k.reshape(B, Lk, heads, hd).transpose(1, 2)
@@ -120,30 +153,76 @@ def _mha(sd, p, heads, q_in, kv_in, attn_mask=None, key_padding_mask=None):
     if key_padding_mask is not None:
         s = s.masked_fill(key_padding_mask[:, None, None, :], float("-inf"))
     o = torch.softmax(s, dim=-1) @ v
-    o = o.transpose(1, 2).reshape(B, Lq, D)
+    return o.transpose(1, 2).reshape(B, Lq, D)
+
+
+def mha_out(sd, p, o):
     return F.linear(o, sd[p + "out_proj.weight"], sd[p + "out_proj.bias"])
 
 
-def decode(sd, spec, tgt, memory, tgt_query, tgt_query_mask, tgt_padding_mask=None):
-    """reference PARSeq.decode (parseq.py:133-157) + Decoder.forward with depth 1 and update_content=False on the
-    last (= only) layer (parseq_transformer.py:148-169,101-130): only the query stream is computed."""
+def _mha(sd, p, heads, q_in, kv_in, attn_mask=None, key_padding_mask=None):
+    k, v = mha_kv(sd, p, kv_in)
+    return mha_out(sd, p, mha_attend(mha_q(sd, p, q_in), k, v, heads, attn_mask, key_padding_mask))
+
+
+DEC = "decoder.layers.0."
+
+
+def content_embed(sd, spec, tgt):
+    """LN_c of the content stream of context tokens tgt (B, L) (parseq.py:133-157): position 0 = sqrt(D) E[tgt0]
+    (no positional term), position p >= 1 = pos_queries[p-1] + sqrt(D) E[tgt_p]."""
     D = spec.embed_dim
     L = tgt.shape[1]
     emb = sd["text_embed.embedding.weight"]
     scale = math.sqrt(D)
     null_ctx = scale * emb[tgt[:, :1]]
     content = torch.cat([null_ctx, sd["pos_queries"][:, :L - 1] + scale * emb[tgt[:, 1:]]], dim=1)
-    p = "decoder.layers.0."
-    qn = F.layer_norm(tgt_query, (D,), sd[p + "norm_q.weight"], sd[p + "norm_q.bias"], 1e-5)
-    cn = F.layer_norm(content, (D,), sd[p + "norm_c.weight"], sd[p + "norm_c.bias"], 1e-5)
-    x = tgt_query + _mha(sd, p + "self_attn.", spec.dec_heads, qn, cn, tgt_query_mask, tgt_padding_mask)
-    h = F.layer_norm(x, (D,), sd[p + "norm1.weight"], sd[p + "norm1.bias"], 1e-5)
-    x = x + _mha(sd, p + "cross_attn.", spec.dec_heads, h, memory)
-    h = F.layer_norm(x, (D,), sd[p + "norm2.weight"], sd[p + "norm2.bias"], 1e-5)
-    h = F.linear(F.gelu(F.linear(h, sd[p + "linear1.weight"], sd[p + "linear1.bias"])), sd[p + "linear2.weight"],
-                 sd[p + "linear2.bias"])
-    x = x + h
-    return F.layer_norm(x, (D,), sd["decoder.norm.weight"], sd["decoder.norm.bias"], 1e-5)
+    return layer_norm(sd, DEC + "norm_c", content, 1e-5)
+
+
+def self_attn_sublayer(sd, spec, tgt_query, content_n, attn_mask=None, key_padding_mask=None):
+    """query stream + self-attention of LN_q(query) over the normalised content (parseq_transformer.py:83-87)."""
+    qn = layer_norm(sd, DEC + "norm_q", tgt_query, 1e-5)
+    return tgt_query + _mha(sd, DEC + "self_attn.", spec.dec_heads, qn, content_n, attn_mask, key_padding_mask)
+
+
+def cross_attn_sublayer(sd, spec, x, memory):
+    """x + cross-attention of LN1 x over the encoder memory (parseq_transformer.py:88-92)."""
+    h = layer_norm(sd, DEC + "norm1", x, 1e-5)
+    return x + _mha(sd, DEC + "cross_attn.", spec.dec_heads, h, memory)
+
+
+def mlp_hidden(sd, h):
+    return F.gelu(F.linear(h, sd[DEC + "linear1.weight"], sd[DEC + "linear1.bias"]))
+
+
+def mlp_out(sd, hid):
+    return F.linear(hid, sd[DEC + "linear2.weight"], sd[DEC + "linear2.bias"])
+
+
+def mlp_sublayer(sd, spec, x):
+    """x + linear2(gelu(linear1(LN2 x))) (parseq_transformer.py:93-94)."""
+    return x + mlp_out(sd, mlp_hidden(sd, layer_norm(sd, DEC + "norm2", x, 1e-5)))
+
+
+def final_norm(sd, spec, x):
+    """Decoder.norm (eps 1e-5) of the query stream."""
+    return layer_norm(sd, "decoder.norm", x, 1e-5)
+
+
+def head(sd, out):
+    """classification head over the normalised decoder output: logits (..., num_tokens - 2)."""
+    return F.linear(out, sd["head.weight"], sd["head.bias"])
+
+
+def decode(sd, spec, tgt, memory, tgt_query, tgt_query_mask, tgt_padding_mask=None):
+    """reference PARSeq.decode (parseq.py:133-157) + Decoder.forward with depth 1 and update_content=False on the
+    last (= only) layer (parseq_transformer.py:148-169,101-130): only the query stream is computed."""
+    cn = content_embed(sd, spec, tgt)
+    x = self_attn_sublayer(sd, spec, tgt_query, cn, tgt_query_mask, tgt_padding_mask)
+    x = cross_attn_sublayer(sd, spec, x, memory)
+    x = mlp_sublayer(sd, spec, x)
+    return final_norm(sd, spec, x)
 
 
 def detect_repeat_onset(seq, period_max=8, min_run_p1=8, min_repeats=3):
@@ -181,11 +260,11 @@ def parseq_forward(sd, spec, images, return_aux=False):
     if not spec.decode_ar:
         # parseq.py:252-262: no prior context, the input is just <bos>; all positions are queried at once, no masks
         out = decode(sd, spec, tgt_in[:, :1], memory, pos_q, None)
-        steps.append(F.linear(out, sd["head.weight"], sd["head.bias"]))
+        steps.append(head(sd, out))
     for i in range(S if spec.decode_ar else 0):
         j = i + 1
         out = decode(sd, spec, tgt_in[:, :j], memory, pos_q[:, i:j], causal[i:j, :j])
-        p_i = F.linear(out, sd["head.weight"], sd["head.bias"])
+        p_i = head(sd, out)
         steps.append(p_i)
         if j < S:
             tgt_in[:, j] = p_i[:, 0].argmax(-1)
@@ -216,7 +295,7 @@ def parseq_forward(sd, spec, images, return_aux=False):
             t_in = torch.cat([bos, logits[:, :-1].argmax(-1)], dim=1)
             pad_mask = (t_in == spec.eos_id).int().cumsum(-1) > 0
             out = decode(sd, spec, t_in, memory, pos_q, qmask[:, :t_in.shape[1]], pad_mask)
-            logits = F.linear(out, sd["head.weight"], sd["head.bias"])
+            logits = head(sd, out)
     for b, cut in enumerate(rep_cut):
         if cut is not None and cut < logits.shape[1]:
             logits[b, cut, :] = -30.0

@@ -184,6 +184,10 @@ def _declare_parseq(lib):
     lib.ytk_parseq_last_steps.argtypes = [c_void_p]
     lib.ytk_parseq_last_phase_ms.restype = None
     lib.ytk_parseq_last_phase_ms.argtypes = [c_void_p, c_void_p]
+    lib.ytk_parseq_set_debug.restype = c_int
+    lib.ytk_parseq_set_debug.argtypes = [c_void_p, c_int]
+    lib.ytk_parseq_debug_tensor.restype = c_int
+    lib.ytk_parseq_debug_tensor.argtypes = [c_void_p, ctypes.c_char_p, c_void_p, c_ll, P(c_int)]
 
 
 class YtkDbRun(ctypes.Structure):

@@ -1,6 +1,9 @@
 // extern "C" surface of libytk_b200.so (declared in include/yomitoku_b200.h).
 #include "../../include/yomitoku_b200.h"
 
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
 #include <algorithm>
 #include <climits>
 #include <cmath>
@@ -1453,6 +1456,71 @@ double ytk_parseq_last_flops(ytk_parseq* h) { return h->engine.flops; }
 int ytk_parseq_last_steps(ytk_parseq* h) { return h->engine.last_steps; }
 void ytk_parseq_last_phase_ms(ytk_parseq* h, float* ms4) {
     for (int i = 0; i < 4; ++i) ms4[i] = h->engine.phase_ms[i];
+}
+
+int ytk_parseq_set_debug(ytk_parseq* h, int on) {
+    if (!h) {
+        ytk::set_error("ytk_parseq_set_debug: null handle");
+        return YTK_ERR;
+    }
+    std::lock_guard<std::mutex> lk(h->mu);
+    h->engine.debug = on ? 1 : 0;
+    return YTK_OK;
+}
+
+// host conversion of the 16-bit GEMM operand type (the read-out launches no kernel)
+static float op_bits_to_f32(uint16_t v) {
+#ifdef YTK_OPERAND_BF16
+    __nv_bfloat16_raw r;
+    r.x = v;
+    return __bfloat162float(__nv_bfloat16(r));
+#else
+    __half_raw r;
+    r.x = v;
+    return __half2float(__half(r));
+#endif
+}
+
+int ytk_parseq_debug_tensor(ytk_parseq* h, const char* name, float* host_out, long long capacity, int* shape4) {
+    if (!h || !name || !shape4) {
+        ytk::set_error("ytk_parseq_debug_tensor: null argument");
+        return YTK_ERR;
+    }
+    std::lock_guard<std::mutex> lk(h->mu);
+    DevGuard dev_guard(h->device);
+    ytk::ParseqEngine::View v;
+    if (h->engine.debug_view(name, &v)) return YTK_ERR;
+    const long long cnt = v.rows * v.cols;
+    shape4[0] = (int)v.rows;
+    shape4[1] = v.cols;
+    shape4[2] = shape4[3] = 1;
+    if (!host_out) return YTK_OK;  // shape query
+    if (cnt > capacity) {
+        ytk::set_error("debug tensor '%s' needs %lld floats, capacity %lld", name, cnt, capacity);
+        return YTK_ERR;
+    }
+    const cudaError_t sync = cudaDeviceSynchronize();
+    if (sync != cudaSuccess) {
+        ytk::set_error("ytk_parseq_debug_tensor: device error before the copy: %s", cudaGetErrorString(sync));
+        return YTK_ERR;
+    }
+    cudaError_t err;
+    if (v.kind != 0) {  // fp32 values / int32 bit patterns
+        err = cudaMemcpy(host_out, v.p, cnt * 4, cudaMemcpyDeviceToHost);
+        if (err != cudaSuccess) {
+            ytk::set_error("ytk_parseq_debug_tensor('%s'): copy failed: %s", name, cudaGetErrorString(err));
+            return YTK_ERR;
+        }
+        return YTK_OK;
+    }
+    std::vector<uint16_t> tmp((size_t)cnt);
+    err = cudaMemcpy(tmp.data(), v.p, cnt * 2, cudaMemcpyDeviceToHost);
+    if (err != cudaSuccess) {
+        ytk::set_error("ytk_parseq_debug_tensor('%s'): copy failed: %s", name, cudaGetErrorString(err));
+        return YTK_ERR;
+    }
+    for (long long i = 0; i < cnt; ++i) host_out[i] = op_bits_to_f32(tmp[i]);
+    return YTK_OK;
 }
 
 int ytk_op_assign_best_overlap_f64(const double* word_boxes_dev, int n_words, const double* elem_boxes_dev,

@@ -15,6 +15,7 @@
 #include "parseq_engine.h"
 
 #include <cmath>
+#include <cstdlib>
 #include <cstring>
 #include <memory>
 
@@ -389,8 +390,108 @@ int ParseqEngine::ensure(long long tok, int rows, long long crop_bytes, int grou
     return 0;
 }
 
+int ParseqEngine::ensure_debug(long long T, long long R, int B) {
+    const size_t D = (size_t)m->cfg.D;
+    const size_t encx = (size_t)(m->cfg.enc_depth + 1) * (size_t)T * D * 4, dec = (size_t)R * D * 4,
+                 ctx = (size_t)B * m->S * 4;
+    if (encx > dbg_encx_bytes) {
+        if (dbg_encx) cudaFree(dbg_encx);
+        dbg_encx = nullptr;
+        dbg_encx_bytes = 0;
+        CK(cudaMalloc(&dbg_encx, encx));
+        dbg_encx_bytes = encx;
+    }
+    if (dec > dbg_dec_bytes) {
+        if (dbg_xself) cudaFree(dbg_xself);
+        if (dbg_xcross) cudaFree(dbg_xcross);
+        dbg_xself = dbg_xcross = nullptr;
+        dbg_dec_bytes = 0;
+        CK(cudaMalloc(&dbg_xself, dec));
+        CK(cudaMalloc(&dbg_xcross, dec));
+        dbg_dec_bytes = dec;
+    }
+    if (ctx > dbg_ctx_bytes) {
+        if (dbg_ctx) cudaFree(dbg_ctx);
+        dbg_ctx = nullptr;
+        dbg_ctx_bytes = 0;
+        CK(cudaMalloc(&dbg_ctx, ctx));
+        dbg_ctx_bytes = ctx;
+    }
+    return 0;
+}
+
+int ParseqEngine::debug_view(const std::string& n, View* o) const {
+    const int D = m->cfg.D, S = m->S;
+    auto set = [o](const void* p, long long rows, int cols, int kind) {
+        o->p = p;
+        o->rows = rows;
+        o->cols = cols;
+        o->kind = kind;
+        return 0;
+    };
+    // model constants (padded width D, padded head layout, folded scales)
+    if (n == "model.q_self") return set(m->q_self, S, D, 0);
+    if (n == "model.ckv0") return set(m->ckv0, 1, 2 * D, 0);
+    if (n == "model.embed") return set(m->embed, m->cfg.num_tokens, D, 1);
+    if (n == "model.pos_q") return set(m->pos_q, S, D, 1);
+    const char* why = "unknown name";
+    const bool enc = n.rfind("enc.", 0) == 0, ar_ = n.rfind("ar.", 0) == 0, dec = n.rfind("dec.", 0) == 0;
+    if ((enc || ar_ || dec) && !last.valid) {
+        why = "no forward has completed on this handle since it was created or last failed";
+    } else if (enc) {
+        const long long T = last.T;
+        if (n == "enc.mem") return set(mem, T, D, 0);
+        if (n == "enc.memkv") return set(memkv, T, 2 * D, 0);
+        if (n.rfind("enc.x.", 0) == 0) {
+            char* end = nullptr;
+            const long L = strtol(n.c_str() + 6, &end, 10);
+            if (end && *end == 0 && end != n.c_str() + 6 && L >= 0 && L <= m->cfg.enc_depth) {
+                if (last.captured) return set(dbg_encx + (size_t)L * T * D, T, D, 1);
+                why = "the residual stream is captured only when debug capture was on for the last forward";
+            }
+        }
+    } else if (ar_) {
+        if (!last.ar) {
+            why = "the last forward ran no AR decode (decode_ar == 0)";
+        } else {
+            if (n == "ar.tgt") return set(ar.tgt, last.B, S, 2);
+            if (n == "ar.raw") return set(ar.raw, last.B, S, 2);
+            if (n == "ar.group_len") return set(ar.group_len, last.groups, 1, 2);
+            if (n == "ar.rep_cut") return set(ar.rep_cut, last.B, 1, 2);
+        }
+    } else if (dec) {
+        const long long R = (long long)last.B * S;
+        if (!last.dec) {
+            why = "the last forward ran no full decoder pass (decode_ar == 1 and refine_iters == 0)";
+        } else {
+            if (n == "dec.klen") return set(klen, last.B, 1, 2);
+            if (n == "dec.kpad") return set(kpad, last.B, 1, 2);
+            if (n == "dec.cin") return set(cin, R, D, 0);
+            if (n == "dec.ckv") return set(ckv, R, 2 * D, 0);
+            if (n == "dec.sa") return set(sa, R, D, 0);
+            if (n == "dec.qc") return set(qc, R, D, 0);
+            if (n == "dec.oc") return set(oc, R, D, 0);
+            if (n == "dec.mlp") return set(mlpb, R, m->lin1.N, 0);
+            if (n == "dec.x") return set(x1, R, D, 1);
+            if (n == "dec.out") return set(hb, R, D, 0);
+            if (n == "dec.x_self" || n == "dec.x_cross" || n == "dec.ctx") {
+                if (last.captured) {
+                    if (n == "dec.x_self") return set(dbg_xself, R, D, 1);
+                    if (n == "dec.x_cross") return set(dbg_xcross, R, D, 1);
+                    return set(dbg_ctx, last.B, S, 2);
+                }
+                why = "captured only when debug capture was on for the last forward";
+            }
+        }
+    }
+    set_error("PARSeq debug tensor '%s': %s", n.c_str(), why);
+    return 1;
+}
+
 ParseqEngine::~ParseqEngine() {
     for (void* p : bufs) cudaFree(p);
+    for (void* p : {(void*)dbg_encx, (void*)dbg_xself, (void*)dbg_xcross, (void*)dbg_ctx})
+        if (p) cudaFree(p);
     if (host_flag) cudaFreeHost(host_flag);
     if (st2) cudaStreamDestroy(st2);
     if (ev_fork) cudaEventDestroy(ev_fork);
@@ -428,6 +529,7 @@ int ParseqEngine::forward(const ParseqBatch& b, int* ids_out, float* probs_out, 
     const ParseqCfg& c = m->cfg;
     const int D = c.D, S = m->S, C = m->C;
     const int B = (int)b.descs.size();
+    last = LastRun{};
     if (B == 0) return 0;
     long long T = 0;
     int max_ntok = 0;
@@ -440,6 +542,7 @@ int ParseqEngine::forward(const ParseqBatch& b, int* ids_out, float* probs_out, 
         }
     }
     if (ensure(T, B, b.crops_bytes, b.ngroups)) return 1;
+    if (debug && ensure_debug(T, (long long)B * m->S, B)) return 1;
     flops = 0;
     const int R = B * S;
     const int eos = 0, bos = c.num_tokens - 2, pad_id = c.num_tokens - 1;
@@ -483,7 +586,9 @@ int ParseqEngine::forward(const ParseqBatch& b, int* ids_out, float* probs_out, 
     CK(cudaEventRecord(ev[0], st));
     const int Ti = (int)T;
     if (Lin::run(A_patch, m->Kpatch, Ti, m->patch, x, D, 1, ACT_NONE, x, 1, D, st, &flops)) return 1;
+    if (debug) CK(cudaMemcpyAsync(dbg_encx, x, (size_t)Ti * D * 4, cudaMemcpyDeviceToDevice, st));
     const int hd_e = D / c.enc_heads;
+    size_t dbg_blk = 0;
     for (const EncBlock& bk : m->blocks) {
         if (launch_layernorm(x, Ti, D, m->Dr, bk.ln1.g, bk.ln1.b, 1e-6f, h, nullptr, nullptr, 1, nullptr, 0, 0, st)) return 1;
         if (Lin::run(h, D, Ti, bk.qkv, qkv, 3 * D, 0, ACT_NONE, nullptr, 0, 0, st, &flops)) return 1;
@@ -495,6 +600,8 @@ int ParseqEngine::forward(const ParseqBatch& b, int* ids_out, float* probs_out, 
         if (launch_layernorm(x, Ti, D, m->Dr, bk.ln2.g, bk.ln2.b, 1e-6f, h, nullptr, nullptr, 1, nullptr, 0, 0, st)) return 1;
         if (Lin::run(h, D, Ti, bk.fc1, mlp, bk.fc1.N, 0, ACT_GELU, nullptr, 0, 0, st, &flops)) return 1;
         if (Lin::run(mlp, bk.fc1.N, Ti, bk.fc2, x, D, 1, ACT_NONE, x, 1, D, st, &flops)) return 1;
+        if (debug)
+            CK(cudaMemcpyAsync(dbg_encx + ++dbg_blk * Ti * D, x, (size_t)Ti * D * 4, cudaMemcpyDeviceToDevice, st));
     }
     for (const CropDesc& d : b.descs) flops += 4.0 * d.ntok * (double)d.ntok * D * c.enc_depth;
     // memory = final LayerNorm (fp32 copy into x1-sized scratch only when the caller wants it)
@@ -726,6 +833,7 @@ int ParseqEngine::forward(const ParseqBatch& b, int* ids_out, float* probs_out, 
         // context tokens: raw[row][p-1] is the token at position p >= 1; L (per group) = context length
         const int* raw = (first && c.decode_ar) ? ar.raw : ids;
         const int* glen = first ? (c.decode_ar ? ar.group_len : glen_const + cap_groups) : glen_const;
+        if (debug) CK(cudaMemcpyAsync(dbg_ctx, raw, (size_t)R * 4, cudaMemcpyDeviceToDevice, st));
         if (launch_refine_embed(raw, row_group, glen, B, S, bos, eos, m->embed, m->pos_q, D, m->Dr, m->norm_c.g,
                                 m->norm_c.b, cin, klen, kpad, st))
             return 1;
@@ -742,12 +850,14 @@ int ParseqEngine::forward(const ParseqBatch& b, int* ids_out, float* probs_out, 
         if (Lin::run(sa, D, R, m->self_out, x1, D, 1, ACT_NONE, nullptr, 0, 0, st, &flops)) return 1;
         if (launch_layernorm(x1, R, D, m->Dr, m->norm1.g, m->norm1.b, 1e-5f, hb, nullptr, m->pos_q, S, nullptr, 0, 1, st))
             return 1;
+        if (debug) CK(cudaMemcpyAsync(dbg_xself, x1, (size_t)R * D * 4, cudaMemcpyDeviceToDevice, st));
         if (Lin::run(hb, D, R, m->cross_q, qc, D, 0, ACT_NONE, nullptr, 0, 0, st, &flops)) return 1;
         const op_t* kv = reinterpret_cast<const op_t*>(memkv);
         if (launch_flash_attention(qc, D, R, kv, kv + D, 2 * D, Ti, oc, D, seqs_ref, B, S, c.dec_heads, hd_d, 0, st))
             return 1;
         for (const CropDesc& d : b.descs) flops += 4.0 * S * (double)d.ntok * D;
         if (Lin::run(oc, D, R, m->cross_out, x1, D, 1, ACT_NONE, x1, 1, D, st, &flops)) return 1;
+        if (debug) CK(cudaMemcpyAsync(dbg_xcross, x1, (size_t)R * D * 4, cudaMemcpyDeviceToDevice, st));
         if (launch_layernorm(x1, R, D, m->Dr, m->norm2.g, m->norm2.b, 1e-5f, hb, nullptr, nullptr, 1, nullptr, 0, 0, st))
             return 1;
         if (Lin::run(hb, D, R, m->lin1, mlpb, m->lin1.N, 0, ACT_GELU, nullptr, 0, 0, st, &flops)) return 1;
@@ -792,6 +902,13 @@ int ParseqEngine::forward(const ParseqBatch& b, int* ids_out, float* probs_out, 
     CK(cudaEventRecord(ev[4], st));
     CK(cudaStreamSynchronize(st));
     for (int i = 0; i < 4; ++i) cudaEventElapsedTime(&phase_ms[i], ev[i], ev[i + 1]);
+    last.valid = true;
+    last.captured = debug != 0;
+    last.ar = c.decode_ar != 0;
+    last.dec = n_pass > 0;
+    last.T = T;
+    last.B = B;
+    last.groups = b.ngroups;
     return 0;
 }
 

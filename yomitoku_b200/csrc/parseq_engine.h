@@ -98,11 +98,36 @@ struct ParseqEngine {
     cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};  // start, encoder, AR, refine, end
     float phase_ms[4] = {0, 0, 0, 0};  // encoder, AR decode, refinement, output copies of the last forward
 
+    // Stage read-out for the tests (ytk_parseq_set_debug / ytk_parseq_debug_tensor).  With `debug` on, forward() copies
+    // the stages it overwrites in place (the encoder residual stream after the patch GEMM and after every block, x1
+    // after the self- and cross-attention sub-layers of the decoder pass, the context tokens of the last pass) into
+    // the dbg_* buffers; nothing else changes.  `last` describes the last successful forward, so that a name it did not
+    // produce is refused instead of returning stale data.
+    int debug = 0;
+    struct LastRun {
+        bool valid = false, captured = false, ar = false, dec = false;
+        long long T = 0;
+        int B = 0, groups = 0;
+    } last;
+    float *dbg_encx = nullptr, *dbg_xself = nullptr, *dbg_xcross = nullptr;
+    int* dbg_ctx = nullptr;
+    size_t dbg_encx_bytes = 0, dbg_dec_bytes = 0, dbg_ctx_bytes = 0;
+    struct View {
+        const void* p = nullptr;
+        long long rows = 0;
+        int cols = 0;
+        int kind = 0;  // 0: 16-bit GEMM operand type, 1: fp32, 2: int32
+    };
+    // The buffer behind a stage name of the last forward (or a model constant); 1 + set_error for an unknown name or
+    // one the last forward did not produce.
+    int debug_view(const std::string& name, View* out) const;
+
     int ensure(long long tok, int rows, long long crop_bytes, int groups);
     // Runs encoder + AR decode + refinement.  Outputs (host): ids [rows*S], probs [rows*S], group_len [ngroups];
     // logits_out (optional, host or device): [rows, S, C] fp32 when refine_iters > 0.
     int forward(const ParseqBatch& b, int* ids_out, float* probs_out, int* group_len_out, float* logits_out,
                 int logits_on_device, float* memory_out, cudaStream_t st);
+    int ensure_debug(long long T, long long R, int B);
     ~ParseqEngine();
 };
 

@@ -579,12 +579,13 @@ class PARSeq(_DeviceModel):
         except Exception:
             pass
 
-    def __call__(self, images, max_length=None):
-        return self.forward(images, max_length)
+    def __call__(self, images, max_length=None, memory_out=None):
+        return self.forward(images, max_length, memory_out)
 
-    def forward(self, images, max_length=None):
+    def forward(self, images, max_length=None, memory_out=None):
         """Model-level seam (one reference mini-batch): logits (B, S, C) fp32, S = 101 with refinement, else the
-        number of AR steps run; the repetition patch of parseq.py:301-309 is applied."""
+        number of AR steps run; the repetition patch of parseq.py:301-309 is applied.  memory_out (optional, CPU
+        float32 (B * N, embed_dim), N encoder tokens per image) receives the encoder output."""
         if max_length is not None:
             raise NotImplementedError("max_length is a training-time argument; inference uses None")
         h = self._ensure()
@@ -598,9 +599,18 @@ class PARSeq(_DeviceModel):
         probs = torch.empty((B, S), dtype=torch.float32)
         rep = torch.empty((B,), dtype=torch.int32)
         steps = ctypes.c_int(0)
+        mem = None
+        if memory_out is not None:
+            ph, pw = self.cfg.encoder.patch_size
+            n = B * (Hh // ph) * (W // pw)
+            if memory_out.device.type != "cpu" or memory_out.dtype != torch.float32 or \
+                    not memory_out.is_contiguous() or tuple(memory_out.shape) != (n, self.cfg.encoder.embed_dim):
+                raise ValueError("memory_out must be a contiguous CPU float32 tensor of shape (%d, %d)"
+                                 % (n, self.cfg.encoder.embed_dim))
+            mem = memory_out.data_ptr()
         _lib.check(_lib.lib().ytk_parseq_forward_f32(h, x.data_ptr(), 1 if x.is_cuda else 0, B, W, logits.data_ptr(),
                                                      1 if x.is_cuda else 0, ids.data_ptr(), probs.data_ptr(),
-                                                     ctypes.byref(steps), rep.data_ptr(), None, None))
+                                                     ctypes.byref(steps), rep.data_ptr(), mem, None))
         if self._refine_iters == 0:
             logits = logits[:, : steps.value]
         if self.repetition_stop:
@@ -670,6 +680,23 @@ class PARSeq(_DeviceModel):
         a = (ctypes.c_float * 4)()
         _lib.lib().ytk_parseq_last_phase_ms(self._ensure(), a)
         return dict(zip(("encoder", "ar", "refine", "copy"), [float(v) for v in a]))
+
+    def set_debug(self, on):
+        """Test hook: with `on`, the next forwards also keep the stages the engine overwrites in place (encoder
+        residual stream per block, decoder x1 after each attention sub-layer, the last pass's context tokens)."""
+        _lib.check(_lib.lib().ytk_parseq_set_debug(self._ensure(), 1 if on else 0))
+
+    def debug_tensor(self, name):
+        """Test hook: a stage of the last forward (names in include/yomitoku_b200.h, ytk_parseq_debug_tensor) as a CPU
+        tensor [rows, cols] at the engine's padded width: float32, or int32 for the integer buffers."""
+        h = self._ensure()
+        shape = (ctypes.c_int * 4)()
+        _lib.check(_lib.lib().ytk_parseq_debug_tensor(h, name.encode(), None, 0, shape))
+        buf = torch.empty((shape[0], shape[1]), dtype=torch.float32)
+        _lib.check(_lib.lib().ytk_parseq_debug_tensor(h, name.encode(), buf.data_ptr(), buf.numel(), shape))
+        if name in ("ar.tgt", "ar.raw", "ar.group_len", "ar.rep_cut", "dec.klen", "dec.kpad", "dec.ctx"):
+            return buf.view(torch.int32)
+        return buf
 
 
 # ======================================================================================================== RT-DETRv2
