@@ -526,8 +526,15 @@ int ytk_op_assign_best_overlap_f64(const double* word_boxes_dev, int n_words, co
                                    int n_groups, double overlap_th, int* best_dev, double* ratio_dev,
                                    long long out_capacity, void* cuda_stream);
 
-/* test hook: copies an intermediate activation (by name, see rtdetr_engine.cu) of the LAST forward of batch size n to
- * the host as fp32; shape4 = {n, h, w, c} (token matrices: {1, 1, rows, c}) */
+/* test hooks.  set_debug: with on != 0 the next forwards (either entry) also copy the stages the engine overwrites in
+ * place into buffers the handle owns (plain device copies: no extra kernels; results and launch counts unchanged).
+ * debug_tensor: copies an intermediate activation (by name, see rtdetr_engine.cu) of the LAST forward of batch size n
+ * to the host as fp32 (16-bit operands converted); shape4 = {n, h, w, c} (token matrices: {1, 1, rows, c}); host_out
+ * null: shape only.  Captured names (the last forward must have run with capture on): {fpn0,fpn1,pan0,pan1}.{c1,r0,r1},
+ * aifi.y1, enc.h1, enc.h2, enc.delta, ref0, dec{i}.{x_in,x_in16,ref,qp0,qpos,qkv,att,y1,x1,x1_16,ow,samp,y2,x2,x2_16,
+ * ffn,y3,x3,x3_16,h1,h2,delta} for each decoder layer i, and dec{layers}.ref.  A batch size whose engine has not run
+ * since it was built (or was evicted), and a captured name of a forward without capture, are errors. */
+int ytk_rtdetr_set_debug(ytk_rtdetr* h, int on);
 int ytk_rtdetr_debug_tensor(ytk_rtdetr* h, int n, const char* name, float* host_out, long long capacity, int* shape4);
 
 #ifdef __cplusplus

@@ -92,10 +92,10 @@ def backbone(sd, spec, x):
     return outs
 
 
-def sincos_2d(w, h, dim, temperature):
-    gw, gh = torch.meshgrid(torch.arange(int(w), dtype=torch.float32), torch.arange(int(h), dtype=torch.float32),
-                            indexing="ij")
-    omega = 1.0 / (temperature ** (torch.arange(dim // 4, dtype=torch.float32) / (dim // 4)))
+def sincos_2d(w, h, dim, temperature, device=None, dtype=torch.float32):
+    kw = dict(dtype=dtype, device=device)
+    gw, gh = torch.meshgrid(torch.arange(int(w), **kw), torch.arange(int(h), **kw), indexing="ij")
+    omega = 1.0 / (temperature ** (torch.arange(dim // 4, **kw) / (dim // 4)))
     ow, oh = gw.flatten()[:, None] @ omega[None], gh.flatten()[:, None] @ omega[None]
     return torch.cat([ow.sin(), ow.cos(), oh.sin(), oh.cos()], dim=1)[None]
 
@@ -121,19 +121,32 @@ def _ln(sd, p, x):
     return F.layer_norm(x, (x.shape[-1],), sd[p + ".weight"], sd[p + ".bias"], 1e-5)
 
 
-def aifi_layer(sd, p, src, pos, heads):
+def aifi_attn(sd, p, src, pos, heads):
+    """the AIFI self-attention sub-layer before its norm: src + MHA(q = k = src + pos, v = src)"""
     q = src + pos
-    src = _ln(sd, p + ".norm1", src + mha(sd, p + ".self_attn", q, q, src, heads))
-    ff = F.linear(F.gelu(F.linear(src, sd[p + ".linear1.weight"], sd[p + ".linear1.bias"])), sd[p + ".linear2.weight"],
-                  sd[p + ".linear2.bias"])
-    return _ln(sd, p + ".norm2", src + ff)
+    return src + mha(sd, p + ".self_attn", q, q, src, heads)
+
+
+def ffn(sd, p, x, act):
+    """linear2(act(linear1(x))) of a transformer layer"""
+    return F.linear(_act(F.linear(x, sd[p + ".linear1.weight"], sd[p + ".linear1.bias"]), act), sd[p + ".linear2.weight"],
+                    sd[p + ".linear2.bias"])
+
+
+def aifi_layer(sd, p, src, pos, heads):
+    src = _ln(sd, p + ".norm1", aifi_attn(sd, p, src, pos, heads))
+    return _ln(sd, p + ".norm2", src + ffn(sd, p, src, "gelu"))
+
+
+def repvgg(sd, b, x):
+    """RepVggBlock in its two-branch (training) form: silu(conv3x3 + BN  +  conv1x1 + BN)"""
+    return F.silu(conv_norm(sd, b + ".conv1", x, 1, None) + conv_norm(sd, b + ".conv2", x, 1, None))
 
 
 def csp_rep(sd, p, x, n):
     x1 = conv_norm(sd, p + ".conv1", x, 1, "silu")
     for i in range(n):
-        b = "%s.bottlenecks.%d" % (p, i)
-        x1 = F.silu(conv_norm(sd, b + ".conv1", x1, 1, None) + conv_norm(sd, b + ".conv2", x1, 1, None))
+        x1 = repvgg(sd, "%s.bottlenecks.%d" % (p, i), x1)
     return x1 + conv_norm(sd, p + ".conv2", x, 1, "silu")         # expansion 1.0: conv3 is the identity
 
 
@@ -143,7 +156,8 @@ def hybrid_encoder(sd, spec, feats):
             for i, f in enumerate(feats)]
     B, C, h, w = proj[2].shape
     src = proj[2].flatten(2).permute(0, 2, 1)
-    mem = aifi_layer(sd, p + "encoder.0.layers.0", src, sincos_2d(w, h, C, spec.pe_temperature), spec.heads)
+    mem = aifi_layer(sd, p + "encoder.0.layers.0", src, sincos_2d(w, h, C, spec.pe_temperature, src.device, src.dtype),
+                     spec.heads)
     proj[2] = mem.permute(0, 2, 1).reshape(B, C, h, w)
     inner = [proj[2]]
     for idx in (2, 1):
@@ -197,27 +211,67 @@ def deformable_attention(spec, value, shapes, loc, weights):
     return (torch.cat(sampled, -1) * wts).sum(-1).reshape(B, H * c, Q).permute(0, 2, 1)
 
 
-def ms_deform_attn(sd, spec, p, query, ref4, memory, shapes):
+def deform_value(sd, spec, p, memory):
+    """value_proj of the memory as (B, L, heads, hidden / heads)"""
+    B, _, D = memory.shape
+    return F.linear(memory, sd[p + ".value_proj.weight"], sd[p + ".value_proj.bias"]).reshape(B, -1, spec.heads, D // spec.heads)
+
+
+def deform_offsets_weights(sd, spec, p, query):
+    """sampling offsets (B, Q, heads, P, 2) and softmax attention weights (B, Q, heads, P) of the query"""
     B, Q, D = query.shape
     H, P = spec.heads, sum(spec.num_points)
-    value = F.linear(memory, sd[p + ".value_proj.weight"], sd[p + ".value_proj.bias"]).reshape(B, -1, H, D // H)
     off = F.linear(query, sd[p + ".sampling_offsets.weight"], sd[p + ".sampling_offsets.bias"]).reshape(B, Q, H, P, 2)
     wts = torch.softmax(F.linear(query, sd[p + ".attention_weights.weight"], sd[p + ".attention_weights.bias"])
                         .reshape(B, Q, H, P), dim=-1)
-    scale = torch.tensor([1.0 / n for n in spec.num_points for _ in range(n)], dtype=query.dtype).unsqueeze(-1)
+    return off, wts
+
+
+def deform_locations(spec, ref4, off):
+    """sampling locations in [0, 1]: ref centre + offset / num_points * ref size * offset_scale"""
+    scale = torch.tensor([1.0 / n for n in spec.num_points for _ in range(n)], dtype=off.dtype,
+                         device=off.device).unsqueeze(-1)
     ref = ref4.unsqueeze(2)                                          # (B, Q, 1, 4): the same box for every level
-    loc = ref[:, :, None, :, :2] + off * scale * ref[:, :, None, :, 2:] * spec.offset_scale
-    out = deformable_attention(spec, value, shapes, loc, wts)
+    return ref[:, :, None, :, :2] + off * scale * ref[:, :, None, :, 2:] * spec.offset_scale
+
+
+def deform_core(spec, value, shapes, ref4, off, wts):
+    """the multi-scale deformable attention of given offsets and weights (before output_proj) -> (B, Q, hidden)"""
+    return deformable_attention(spec, value, shapes, deform_locations(spec, ref4, off), wts)
+
+
+def ms_deform_attn(sd, spec, p, query, ref4, memory, shapes):
+    value = deform_value(sd, spec, p, memory)
+    off, wts = deform_offsets_weights(sd, spec, p, query)
+    out = deform_core(spec, value, shapes, ref4, off, wts)
     return F.linear(out, sd[p + ".output_proj.weight"], sd[p + ".output_proj.bias"])
 
 
-def decoder_layer(sd, spec, p, tgt, ref4, memory, shapes, qpos):
+def self_attn_sublayer(sd, spec, p, tgt, qpos):
+    """norm1(tgt + MHA(q = k = tgt + qpos, v = tgt))"""
     q = tgt + qpos
-    tgt = _ln(sd, p + ".norm1", tgt + mha(sd, p + ".self_attn", q, q, tgt, spec.heads))
-    tgt = _ln(sd, p + ".norm2", tgt + ms_deform_attn(sd, spec, p + ".cross_attn", tgt + qpos, ref4, memory, shapes))
-    ff = F.linear(F.relu(F.linear(tgt, sd[p + ".linear1.weight"], sd[p + ".linear1.bias"])), sd[p + ".linear2.weight"],
-                  sd[p + ".linear2.bias"])
-    return _ln(sd, p + ".norm3", tgt + ff)
+    return _ln(sd, p + ".norm1", tgt + mha(sd, p + ".self_attn", q, q, tgt, spec.heads))
+
+
+def cross_attn_sublayer(sd, spec, p, tgt, qpos, ref4, memory, shapes):
+    """norm2(tgt + MSDeformableAttention(tgt + qpos, ref4, memory))"""
+    return _ln(sd, p + ".norm2", tgt + ms_deform_attn(sd, spec, p + ".cross_attn", tgt + qpos, ref4, memory, shapes))
+
+
+def ffn_sublayer(sd, p, tgt):
+    """norm3(tgt + linear2(relu(linear1(tgt))))"""
+    return _ln(sd, p + ".norm3", tgt + ffn(sd, p, tgt, "relu"))
+
+
+def decoder_layer(sd, spec, p, tgt, ref4, memory, shapes, qpos):
+    tgt = self_attn_sublayer(sd, spec, p, tgt, qpos)
+    tgt = cross_attn_sublayer(sd, spec, p, tgt, qpos, ref4, memory, shapes)
+    return ffn_sublayer(sd, p, tgt)
+
+
+def box_refine(sd, p, tgt, ref):
+    """iterative box refinement: sigmoid(bbox MLP(tgt) + inverse_sigmoid(ref))"""
+    return torch.sigmoid(mlp(sd, p, tgt, 3) + inverse_sigmoid(ref))
 
 
 def decoder(sd, spec, feats, aux=None):
@@ -240,7 +294,7 @@ def decoder(sd, spec, feats, aux=None):
     for i in range(spec.num_layers):
         qpos = mlp(sd, p + "query_pos_head", ref, 2)
         tgt = decoder_layer(sd, spec, "%sdecoder.layers.%d" % (p, i), tgt, ref, memory, shapes, qpos)
-        box = torch.sigmoid(mlp(sd, "%sdec_bbox_head.%d" % (p, i), tgt, 3) + inverse_sigmoid(ref))
+        box = box_refine(sd, "%sdec_bbox_head.%d" % (p, i), tgt, ref)
         if i == spec.num_layers - 1:
             logits = F.linear(tgt, sd["%sdec_score_head.%d.weight" % (p, i)], sd["%sdec_score_head.%d.bias" % (p, i)])
             return {"pred_logits": logits, "pred_boxes": box}
@@ -263,7 +317,7 @@ def postprocess(spec, out, orig_wh, threshold):
     logits, boxes = out["pred_logits"], out["pred_boxes"]
     cx, cy, w, h = boxes.unbind(-1)
     xyxy = torch.stack([cx - 0.5 * w, cy - 0.5 * h, cx + 0.5 * w, cy + 0.5 * h], -1)
-    xyxy = xyxy * torch.tensor([orig_wh[0], orig_wh[1]] * 2, dtype=xyxy.dtype)
+    xyxy = xyxy * torch.tensor([orig_wh[0], orig_wh[1]] * 2, dtype=xyxy.dtype, device=xyxy.device)
     scores, index = torch.topk(torch.sigmoid(logits).flatten(1), spec.num_queries, dim=-1)
     labels = index - index // spec.num_classes * spec.num_classes
     sel = xyxy.gather(1, (index // spec.num_classes).unsqueeze(-1).repeat(1, 1, 4))

@@ -17,6 +17,8 @@ def test_library_builds_loads_and_exports_header_symbols():
     assert len(names) >= 15
     for n in names:
         assert hasattr(lib, n), "missing export %s" % n
+    for n in ("ytk_rtdetr_set_debug", "ytk_rtdetr_debug_tensor", "ytk_parseq_set_debug", "ytk_parseq_debug_tensor"):
+        assert n in names                               # the stage read-out hooks are part of the header
     assert lib.ytk_version() >= 1
     assert lib.ytk_launch_count() == 0
     assert isinstance(lib.ytk_last_error(), bytes)

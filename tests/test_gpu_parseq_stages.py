@@ -8,6 +8,7 @@ across stages, and every stage has its own a-priori componentwise bound, compute
 runs some models zero-padded (parseq-tiny: D 368 as 384, heads of 46 as 48): its tensors are read at the padded width,
 the padded columns must be exactly zero, and the comparison runs in the real model's feature space.
 
+The bound rules are implemented in tests/stage_bounds.py (lin, ln, attend), shared with the RT-DETRv2 stage test.
 Notation: u = 2^-11 (fp16 rounding, to nearest), e = 2^-24 (fp32 rounding), g(n) = n 2^-23 (n fp32 additions, each
 within one unit of a 24-bit significand as truncating tensor-core adders give), s = 2^-25 (half the fp16 subnormal
 spacing).  |.| is elementwise, e_x the bound carried by an input x (zero when x is the engine's own stored value).
@@ -56,13 +57,12 @@ import torch
 
 from oracle import parseq as ops
 from oracle import weights
+from stage_bounds import E, LAMBDA, SUB, U, attend, lin, ln
 from yomitoku_b200 import TextRecognizer, _lib
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-U, E, G, SUB = 2.0 ** -11, 2.0 ** -24, 2.0 ** -23, 2.0 ** -25
 SA, CA, DEC = ops.DEC + "self_attn.", ops.DEC + "cross_attn.", ops.DEC
-LAMBDA = 6.0        # composite stages: |d| <= LAMBDA sigma (module docstring)
 RATIOS = {}         # stage -> worst |d| / bound
 LOGIT_BOUNDS = {}   # configuration -> largest logit bound of a teacher-forced AR step (absolute, logits)
 
@@ -129,89 +129,6 @@ def _dbg(m, name):
 
 def _sd64(sd):
     return {k: v.to(DEV, torch.float64) for k, v in sd.items()}
-
-
-# ------------------------------------------------------------------------------------------------------ bounds
-def _prop(e, M, rss):
-    """input bound e through the linear map M^T: worst case e |M|^T, or root-sum-square sqrt(e^2 (M^2)^T)"""
-    return torch.sqrt((e * e) @ (M * M).T) if rss else e @ M.abs().T
-
-
-def lin(x, e_x, W, b, out16, resid=None, e_r=None, gelu=False, rss=False):
-    """float64 x W^T + b (+ resid) (GELU) and its bound (module docstring)."""
-    pre = x @ W.T + b
-    if resid is not None:
-        pre = pre + resid
-    S = x.abs() @ W.abs().T
-    K = (W.shape[1] + 63) // 64 * 64
-    if rss:     # independent weight roundings and accumulation errors: root-sum-square, sqrt(K) g(1) S
-        R = torch.sqrt((x * x) @ (W * W).T)
-        e = (U + E) * R + SUB * x.norm(dim=-1, keepdim=True) + math.sqrt(K) * G * S + \
-            G * (R + b.abs() + (resid.abs() if resid is not None else 0))
-    else:
-        e = (U + E) * S + SUB * x.abs().sum(-1, keepdim=True) + K * G * S + \
-            G * (S + b.abs() + (resid.abs() if resid is not None else 0))
-    if e_x is not None:
-        e = e + _prop(e_x, W, rss)
-    if e_r is not None:
-        e = e + e_r
-    y = pre
-    if gelu:
-        y = torch.nn.functional.gelu(pre)
-        e = 1.13 * e + 5e-7 + E * y.abs()
-    e = e + (U * y.abs() + SUB if out16 else E * y.abs())
-    return y, e
-
-
-def ln(sd, name, x, e_x, eps, out16, rss=False):
-    y = ops.layer_norm(sd, name, x, eps)
-    g, bb = sd[name + ".weight"], sd[name + ".bias"]
-    D = x.shape[-1]
-    mu = x.mean(-1, keepdim=True)
-    r = 1.0 / torch.sqrt(((x - mu) ** 2).mean(-1, keepdim=True) + eps)
-    xh = (x - mu) * r
-    e = g.abs() * r * D * E * x.abs().mean(-1, keepdim=True) + (D + 16) * E * g.abs() * xh.abs() + 2 * E * (y.abs() + bb.abs())
-    if e_x is not None:
-        if rss:
-            m1, m2 = e_x.norm(dim=-1, keepdim=True) / D, (xh * e_x).norm(dim=-1, keepdim=True) / D
-        else:
-            m1, m2 = e_x.mean(-1, keepdim=True), (xh.abs() * e_x).mean(-1, keepdim=True)
-        e = e + g.abs() * r * (e_x + m1 + xh.abs() * m2)
-    if out16:
-        e = e + U * y.abs() + SUB
-    return y, e
-
-
-def attend(q, k, v, heads, e_q=None, e_k=None, e_v=None, amask=None, pmask=None, rss=False):
-    """ops.mha_attend for one batch row (q (Lq, D), k / v (Lk, D)) and its bound."""
-    o = ops.mha_attend(q[None], k[None], v[None], heads, amask, None if pmask is None else pmask[None])[0]
-    Lq, D = q.shape
-    Lk = k.shape[0]
-    hd = D // heads
-    H = lambda t, n: t.reshape(n, heads, hd).transpose(0, 1)      # noqa: E731
-    qh, kh, vh = H(q, Lq), H(k, Lk), H(v, Lk)
-    s = qh @ kh.transpose(-1, -2) / math.sqrt(hd)
-    vis = torch.ones(Lq, Lk, dtype=torch.bool, device=q.device)
-    if amask is not None:
-        vis &= ~amask
-    if pmask is not None:
-        vis = vis & ~pmask[None, :]
-    vis = vis[None].expand(heads, -1, -1)
-    p = torch.softmax(s.masked_fill(~vis, float("-inf")), -1)
-    d = (qh.abs() @ kh.abs().transpose(-1, -2)) * (2 * hd * G) / math.sqrt(hd) + 4 * E * s.abs() + 2.0 ** -21
-    sq = (lambda a, b: torch.sqrt((a * a) @ (b * b).transpose(-1, -2))) if rss else \
-        (lambda a, b: a.abs() @ b.abs().transpose(-1, -2))
-    if e_q is not None:
-        d = d + sq(H(e_q, Lq), kh) / math.sqrt(hd)
-    if e_k is not None:
-        d = d + sq(qh, H(e_k, Lk)) / math.sqrt(hd)
-    dmax = d.masked_fill(~vis, 0).amax(-1, keepdim=True)
-    P = torch.sqrt((p * p) @ (vh * vh)) if rss else p @ vh.abs()
-    e = (torch.exp(2 * dmax) - 1) * P + (U + Lk * G + 8 * E) * P + SUB * (vis.double() @ vh.abs())
-    if e_v is not None:
-        e = e + (torch.sqrt((p * p) @ H(e_v * e_v, Lk)) if rss else p @ H(e_v, Lk))
-    e = e.transpose(0, 1).reshape(Lq, D)
-    return o, e + U * o.abs() + SUB
 
 
 # ------------------------------------------------------------------------------------------------------ encoder

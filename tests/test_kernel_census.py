@@ -17,27 +17,30 @@ G = "tests/test_gpu_glue_kernels.py::"
 DEC = "tests/test_gpu_decoder_kernels.py::"
 DBK = "tests/test_gpu_dbnet_kernels.py::"
 PQD = "tests/test_gpu_parseq_decode_kernels.py::"
+RTS = "tests/test_gpu_rtdetr_stages.py::"
 
 # kernel -> tests that reach it (op-level tests first)
 CENSUS = {
     # rtdetr_ops.cu
-    "pack_input_kernel": [G + "test_engine_input_and_fpn_wiring"],
-    "avgpool2_kernel": [G + "test_avgpool2_vs_float64"],
+    "pack_input_kernel": [G + "test_engine_input_and_fpn_wiring", RTS + "test_backbone_stages"],
+    "avgpool2_kernel": [G + "test_avgpool2_vs_float64", RTS + "test_backbone_stages"],
     "upsample_nearest2_kernel": [G + "test_upsample_nearest2_bitwise", G + "test_engine_input_and_fpn_wiring"],
     "add_f16_kernel": [G + "test_add_f16_bitwise", G + "test_add_table_bitwise", G + "test_engine_input_and_fpn_wiring",
-                       G + "test_engine_aifi_position_embedding"],
+                       G + "test_engine_aifi_position_embedding", RTS + "test_encoder_stages",
+                       RTS + "test_decoder_layer_stages"],
     "mask_invalid_rows_kernel": [G + "test_mask_invalid_exact", G + "test_engine_encoder_selection_wiring"],
     "enc_scores_kernel": [G + "test_enc_scores_exact", G + "test_engine_encoder_selection_wiring"],
     "topk_select_kernel": ["tests/test_gpu_cell_detector.py::test_topk_equals_stable_sort"],
     "gather_queries_kernel": [G + "test_gather_queries_exact", G + "test_engine_encoder_selection_wiring"],
-    "ref_update_kernel": [G + "test_ref_update_vs_float64"],
-    "qpos_l0_kernel": [G + "test_qpos_l0_vs_float64"],
-    "deform_attn_kernel": [DEC + "test_deform_attn_vs_float64"],
-    "copy_cols_kernel": [G + "test_engine_encoder_selection_wiring"],
+    "ref_update_kernel": [G + "test_ref_update_vs_float64", RTS + "test_query_selection_stages",
+                          RTS + "test_decoder_layer_stages"],
+    "qpos_l0_kernel": [G + "test_qpos_l0_vs_float64", RTS + "test_decoder_layer_stages"],
+    "deform_attn_kernel": [DEC + "test_deform_attn_vs_float64", RTS + "test_decoder_layer_stages"],
+    "copy_cols_kernel": [G + "test_engine_encoder_selection_wiring", RTS + "test_decoder_layer_stages"],
     # parseq_ops.cu
     "patchify_u8_kernel": [G + "test_patchify_u8_exact"],
     "patchify_f32_kernel": [G + "test_patchify_f32_exact"],
-    "layernorm_kernel": [DEC + "test_layernorm_vs_float64"],
+    "layernorm_kernel": [DEC + "test_layernorm_vs_float64", RTS + "test_encoder_stages", RTS + "test_decoder_layer_stages"],
     "flash_attn_kernel": ["tests/test_gpu_kernels.py::test_attention_legacy_kernel_still_matches"],
     "single_query_attn_kernel": [DEC + "test_single_query_self_attn_vs_float64",
                                  DEC + "test_single_query_cross_attn_vs_float64"],
@@ -51,19 +54,21 @@ CENSUS = {
     "fill_i32_kernel": ["tests/test_gpu_parseq.py::test_repetition_stop_and_refine_off"],
     # attn_tc.cu, gemm_tc.cu
     "attn_tc_kernel": ["tests/test_gpu_kernels.py::test_attention_tc_vs_torch",
-                       "tests/test_gpu_attention_units.py::test_unit_edges_all_head_dims"],
+                       "tests/test_gpu_attention_units.py::test_unit_edges_all_head_dims",
+                       RTS + "test_encoder_stages", RTS + "test_decoder_layer_stages"],
     "gemm_tc_kernel": ["tests/test_gpu_gemm_variants.py::test_linear_instance_all_activations",
-                       "tests/test_gpu_gemm_variants.py::test_conv"],
+                       "tests/test_gpu_gemm_variants.py::test_conv", RTS + "test_backbone_stages",
+                       RTS + "test_encoder_stages", RTS + "test_decoder_layer_stages"],
     # dbnet_ops.cu
     "preprocess_kernel": [DBK + "test_preprocess_table_vs_float64"],
     "pack_nchw_kernel": ["tests/test_gpu_dbnet.py::test_reference_fixture_through_model_seam"],
-    "maxpool3x3s2_kernel": [DBK + "test_maxpool_bitwise"],
+    "maxpool3x3s2_kernel": [DBK + "test_maxpool_bitwise", RTS + "test_backbone_stages"],
     "upsample_bilinear_kernel": [DBK + "test_upsample_vs_float64"],
     "asf_pool_kernel": [DBK + "test_asf_vs_float64"],
     "asf_gate_kernel": [DBK + "test_asf_vs_float64"],
     "asf_cmean_kernel": [DBK + "test_asf_vs_float64"],
     "asf_apply_kernel": [DBK + "test_asf_vs_float64"],
-    "op_to_f32_kernel": [G + "test_engine_input_and_fpn_wiring", DBK + "test_engine_passes_the_op_arguments"],
+    "op_to_f32_kernel": [DBK + "test_engine_passes_the_op_arguments"],
     # dbpost_ops.cu
     "label_seed_kernel": ["tests/test_gpu_dbpost.py::test_runs_equal_scipy_twin"],
     "label_merge_kernel": ["tests/test_gpu_dbpost.py::test_runs_equal_scipy_twin"],
@@ -81,14 +86,14 @@ CENSUS = {
 
 # kernels no op-level test calls alone: why the listed tests are enough
 REASON = {
-    "pack_input_kernel": "a layout of the input with three real channels: the in-situ check compares it exactly",
-    "copy_cols_kernel": "a column copy of the logits: the in-situ check compares pred_logits with it exactly",
+    "pack_input_kernel": "a layout of the input with three real channels: the in-situ checks compare it exactly",
+    "copy_cols_kernel": "a column copy of the logits: the in-situ checks compare pred_logits with it exactly",
     "flash_attn_kernel": "the legacy attention kernel, selected by impl 1; the engines run attn_tc_kernel",
     "bcast_rows_kernel": "a row copy seeding the refinement K/V cache: a wrong row changes the refined logits",
     "refine_seqs_kernel": "integer descriptors of the refinement attention: a wrong one changes the refined logits",
     "fill_i32_kernel": "an integer fill of the AR state: the repetition and refine-off paths depend on it",
     "pack_nchw_kernel": "the layout of the f32 model seam: the reference fixture through that seam compares its output",
-    "op_to_f32_kernel": "the exact fp16 -> fp32 conversion of the debug download, behind every in-situ comparison",
+    "op_to_f32_kernel": "the exact fp16 -> fp32 conversion of DBNet's debug download, behind its in-situ comparisons",
     "label_seed_kernel": "one stage of the connected-component labelling, compared as a whole against a scipy twin",
     "label_merge_kernel": "one stage of the connected-component labelling, compared as a whole against a scipy twin",
     "page_stats_kernel": "one stage of the connected-component labelling, compared as a whole against a scipy twin",

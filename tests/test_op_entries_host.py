@@ -587,3 +587,11 @@ def test_patchify_f32_refusals(lib, kwargs, fragment):
     _refused(lib, lib.ytk_op_patchify_f32(a["src"], a["n"], a["W"], a["ph"], a["pw"], a["Kpad"], a["pos"],
                                           a["full_gw"], a["D"], a["A"], a["x"], None), fragment)
     assert lib.ytk_launch_count() == before
+
+
+def test_rtdetr_debug_hooks_refuse_null_arguments(lib):
+    shape = (ctypes.c_int * 4)()
+    _refused(lib, lib.ytk_rtdetr_set_debug(None, 1), b"ytk_rtdetr_set_debug: null handle")
+    _refused(lib, lib.ytk_rtdetr_debug_tensor(None, 1, b"c3", None, 0, shape), b"ytk_rtdetr_debug_tensor: null argument")
+    _refused(lib, lib.ytk_rtdetr_debug_tensor(P, 1, None, None, 0, shape), b"ytk_rtdetr_debug_tensor: null argument")
+    _refused(lib, lib.ytk_rtdetr_debug_tensor(P, 1, b"c3", None, 0, None), b"ytk_rtdetr_debug_tensor: null argument")

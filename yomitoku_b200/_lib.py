@@ -234,6 +234,8 @@ def _declare_rtdetr(lib):
     lib.ytk_rtdetr_forward_f32.argtypes = [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p]
     lib.ytk_rtdetr_flops.restype = ctypes.c_double
     lib.ytk_rtdetr_flops.argtypes = [c_void_p, c_int]
+    lib.ytk_rtdetr_set_debug.restype = c_int
+    lib.ytk_rtdetr_set_debug.argtypes = [c_void_p, c_int]
     lib.ytk_rtdetr_debug_tensor.restype = c_int
     lib.ytk_rtdetr_debug_tensor.argtypes = [c_void_p, c_int, ctypes.c_char_p, c_void_p, c_ll, P(c_int)]
 

@@ -1599,6 +1599,7 @@ struct ytk_rtdetr {
     std::mutex mu;
     int device = 0;
     cudaEvent_t last_done = nullptr;   // buffers of an engine are shared by all calls: order them (see ytk_dbnet)
+    int debug = 0;                     // ytk_rtdetr_set_debug: forwards also capture the stages overwritten in place
     // ytk_rtdetr_forward_u8: device copy of host pages, and the resize scratch (records, coefficients, intermediates)
     uint8_t* pages = nullptr;
     size_t pages_cap = 0;
@@ -1625,7 +1626,7 @@ static int rt_reserve(ytk_rtdetr* h, uint8_t** buf, size_t* cap, size_t bytes, c
 // Runs the engine on its packed input and copies the outputs (the common tail of both forward entries).
 static int rt_finish(ytk_rtdetr* h, ytk::RtdetrEngine* e, int n, float* pred_logits, float* pred_boxes, int out_on_device,
                      cudaStream_t st) {
-    if (e->run(st)) return YTK_ERR;
+    if (e->run(st, h->debug != 0)) return YTK_ERR;
     const int K = h->model.cfg.num_queries, C = h->model.cfg.num_classes;
     const cudaMemcpyKind kind = out_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
     cudaError_t err = cudaMemcpyAsync(pred_logits, e->out_logits, (size_t)n * K * C * 4, kind, st);
@@ -1800,33 +1801,58 @@ double ytk_rtdetr_flops(ytk_rtdetr* h, int n) {
     return e ? e->flops : -1.0;
 }
 
-int ytk_rtdetr_debug_tensor(ytk_rtdetr* h, int n, const char* name, float* host_out, long long capacity, int* shape4) {
-    std::lock_guard<std::mutex> lk(h->mu);
-    DevGuard dev_guard(h->device);
-    ytk::RtdetrEngine* e = rt_engine(h, n);
-    if (!e) return YTK_ERR;
-    auto it = e->dbg.find(name);
-    if (it == e->dbg.end() || !it->second.p) {
-        ytk::set_error("no debug tensor named '%s'", name);
+int ytk_rtdetr_set_debug(ytk_rtdetr* h, int on) {
+    if (!h) {
+        ytk::set_error("ytk_rtdetr_set_debug: null handle");
         return YTK_ERR;
     }
-    const ytk::DebugTensor& t = it->second;
+    std::lock_guard<std::mutex> lk(h->mu);
+    h->debug = on ? 1 : 0;
+    return YTK_OK;
+}
+
+int ytk_rtdetr_debug_tensor(ytk_rtdetr* h, int n, const char* name, float* host_out, long long capacity, int* shape4) {
+    if (!h || !name || !shape4) {
+        ytk::set_error("ytk_rtdetr_debug_tensor: null argument");
+        return YTK_ERR;
+    }
+    std::lock_guard<std::mutex> lk(h->mu);
+    DevGuard dev_guard(h->device);
+    // never build an engine here: a fresh one has run nothing, and an evicted one's results are gone
+    auto eit = h->engines.find(n);
+    if (eit == h->engines.end()) {
+        ytk::set_error("RT-DETRv2 debug tensor '%s': no engine for batch size %d (never run, or evicted)", name, n);
+        return YTK_ERR;
+    }
+    ytk::DebugTensor t;
+    if (eit->second->debug_view(name, &t)) return YTK_ERR;
     const long long cnt = (long long)t.n * t.h * t.w * t.c;
-    shape4[0] = t.n; shape4[1] = t.h; shape4[2] = t.w; shape4[3] = t.c;
+    shape4[0] = t.n;
+    shape4[1] = t.h;
+    shape4[2] = t.w;
+    shape4[3] = t.c;
+    if (!host_out) return YTK_OK;  // shape query
     if (cnt > capacity) {
         ytk::set_error("debug tensor '%s' needs %lld floats, capacity %lld", name, cnt, capacity);
         return YTK_ERR;
     }
-    cudaDeviceSynchronize();
+    const cudaError_t sync = cudaDeviceSynchronize();
+    if (sync != cudaSuccess) {
+        ytk::set_error("ytk_rtdetr_debug_tensor: device error before the copy: %s", cudaGetErrorString(sync));
+        return YTK_ERR;
+    }
+    cudaError_t err;
     if (t.f32) {
-        if (cudaMemcpy(host_out, t.p, cnt * 4, cudaMemcpyDeviceToHost) != cudaSuccess) return YTK_ERR;
+        err = cudaMemcpy(host_out, t.p, cnt * 4, cudaMemcpyDeviceToHost);
     } else {
-        float* tmp = nullptr;
-        if (cudaMalloc(&tmp, cnt * 4) != cudaSuccess) return YTK_ERR;
-        ytk::launch_op_to_f32(t.p, tmp, cnt, 0);
-        cudaError_t err = cudaMemcpy(host_out, tmp, cnt * 4, cudaMemcpyDeviceToHost);
-        cudaFree(tmp);
-        if (err != cudaSuccess) return YTK_ERR;
+        std::vector<uint16_t> tmp((size_t)cnt);
+        err = cudaMemcpy(tmp.data(), t.p, cnt * 2, cudaMemcpyDeviceToHost);
+        if (err == cudaSuccess)
+            for (long long i = 0; i < cnt; ++i) host_out[i] = op_bits_to_f32(tmp[i]);
+    }
+    if (err != cudaSuccess) {
+        ytk::set_error("ytk_rtdetr_debug_tensor('%s'): copy failed: %s", name, cudaGetErrorString(err));
+        return YTK_ERR;
     }
     return YTK_OK;
 }

@@ -333,6 +333,16 @@ int RtdetrEngine::alloc(const std::string& name, long long rows, int c, bool f32
     return 0;
 }
 
+void RtdetrEngine::capture(const std::string& name, const void* src, long long rows, int c, bool f32, int n, int h,
+                           int w) {
+    Capture& k = caps[name];
+    k.after = steps.size();
+    k.src = src;
+    k.bytes = (size_t)rows * c * (f32 ? 4 : 2);
+    k.t = n ? DebugTensor{nullptr, n, h, w, c, f32} : DebugTensor{nullptr, 1, 1, (int)rows, c, f32};
+    cap_order.push_back(&k);
+}
+
 int RtdetrEngine::conv(const ConvW& cw, const void* in, int n, int h, int w, long long in_ld, void* out, long long ldc,
                        int act, const void* resid, long long ldr) {
     ConvGeom g{n, h, w, cw.Cin, in_ld, cw.k, cw.k, cw.stride, cw.pad, cw.dil, cw.Cout};
@@ -377,8 +387,11 @@ int RtdetrEngine::csp(const RtCsp& c, const std::string& name, const void* cat, 
         alloc(name + ".x2", rows, D, false, &x2, n, h, w))
         return 1;
     if (conv(c.conv1, cat, n, h, w, 2 * D, t1, D, ACT_SILU)) return 1;
+    capture(name + ".c1", t1, rows, D, false, n, h, w);
     if (conv(c.rep[0], t1, n, h, w, D, t2, D, ACT_SILU)) return 1;
+    capture(name + ".r0", t2, rows, D, false, n, h, w);
     if (conv(c.rep[1], t2, n, h, w, D, t1, D, ACT_SILU)) return 1;
+    capture(name + ".r1", t1, rows, D, false, n, h, w);
     if (conv(c.rep[2], t1, n, h, w, D, t2, D, ACT_SILU)) return 1;
     if (conv(c.conv2, cat, n, h, w, 2 * D, x2, D, ACT_SILU)) return 1;
     steps.push_back([=](cudaStream_t st) { return launch_rt_add(t2, x2, nullptr, D, 1, out, rows, st); });
@@ -422,18 +435,19 @@ int RtdetrEngine::build(const RtdetrModel& model, int n) {
             const int ho = bk.pool ? h / 2 : h, wo = bk.pool ? w / 2 : w;
             const std::string nm = "res" + std::to_string(s) + "." + std::to_string(b);
             void *t1, *t2, *o, *sc = nullptr;
-            if (alloc("", (long long)N * h * w, planes[s], false, &t1) || alloc("", (long long)N * ho * wo, planes[s], false, &t2) ||
+            if (alloc(nm + ".a", (long long)N * h * w, planes[s], false, &t1, N, h, w) ||
+                alloc(nm + ".b", (long long)N * ho * wo, planes[s], false, &t2, N, ho, wo) ||
                 alloc(nm, (long long)N * ho * wo, planes[s] * 4, false, &o, N, ho, wo))
                 return 1;
             if (conv(bk.a, x, N, h, w, cch, t1, planes[s], ACT_RELU)) return 1;
             if (conv(bk.b, t1, N, h, w, planes[s], t2, planes[s], ACT_RELU)) return 1;
             const void* res = x;
             if (bk.has_short) {
-                if (alloc("", (long long)N * ho * wo, planes[s] * 4, false, &sc)) return 1;
+                if (alloc(nm + ".short", (long long)N * ho * wo, planes[s] * 4, false, &sc, N, ho, wo)) return 1;
                 const void* sin = x;
                 if (bk.pool) {
                     void* pl;
-                    if (alloc("", (long long)N * ho * wo, cch, false, &pl)) return 1;
+                    if (alloc(nm + ".pool", (long long)N * ho * wo, cch, false, &pl, N, ho, wo)) return 1;
                     const void* xin = x;
                     const int hh = h, ww = w, cc = cch;
                     steps.push_back([=](cudaStream_t st) { return launch_rt_avgpool2(xin, pl, N, hh, ww, cc, st); });
@@ -505,6 +519,7 @@ int RtdetrEngine::build(const RtdetrModel& model, int n) {
     });
     flops += 4.0 * N * (double)T5 * T5 * D;
     if (linear(model.aifi_out, aatt, D, (int)R5, ay, D, true, ACT_NONE, p5, false, D)) return 1;
+    capture("aifi.y1", ay, R5, D, true);
     steps.push_back([=](cudaStream_t st) {
         return launch_layernorm(reinterpret_cast<float*>(ay), (int)R5, D, D, mp->aifi_n1.g, mp->aifi_n1.b, 1e-5f, as16,
                                 reinterpret_cast<float*>(as32), nullptr, 1, nullptr, 0, 0, st);
@@ -573,10 +588,14 @@ int RtdetrEngine::build(const RtdetrModel& model, int n) {
     if (linear(model.enc_box0, tgt16, D, (int)RQ, h1, D, false, ACT_RELU) || linear(model.enc_box1, h1, D, (int)RQ, h2, D, false, ACT_RELU) ||
         linear(model.enc_box2, h2, D, (int)RQ, delta, 4, true, ACT_NONE))
         return 1;
+    capture("enc.h1", h1, RQ, D, false);
+    capture("enc.h2", h2, RQ, D, false);
+    capture("enc.delta", delta, RQ, 4, true);
     steps.push_back([=](cudaStream_t st) {
         return launch_rt_ref_update(reinterpret_cast<float*>(delta), 4, reinterpret_cast<float*>(asel),
                                     reinterpret_cast<float*>(ref), (int)RQ, st);
     });
+    capture("ref0", ref, RQ, 4, true);
     // ---- decoder layers (rtdetrv2_decoder.py:225-303, 402-444)
     void *qp0, *qp16, *tq, *qkv, *att, *y, *ow, *samp, *ffn, *lg;
     const int n_ow = c.heads * 3 * c.num_points * 3;
@@ -596,50 +615,74 @@ int RtdetrEngine::build(const RtdetrModel& model, int n) {
     op_t* qkvh = reinterpret_cast<op_t*>(qkv);
     for (int i = 0; i < c.num_layers; ++i) {
         const RtDecLayer* L = &model.layers[i];
+        const std::string dn = "dec" + std::to_string(i);
+        capture(dn + ".x_in", tgt32, RQ, D, true);
+        capture(dn + ".x_in16", tgt16, RQ, D, false);
+        capture(dn + ".ref", ref, RQ, 4, true);
         steps.push_back([=](cudaStream_t st) {
             return launch_rt_qpos_l0(reinterpret_cast<float*>(ref), mp->qpos0_w, mp->qpos0_b, 2 * D, qp0, (int)RQ, st);
         });
+        capture(dn + ".qp0", qp0, RQ, 2 * D, false);
         if (linear(model.qpos1, qp0, 2 * D, (int)RQ, qp16, D, false, ACT_NONE)) return 1;
+        capture(dn + ".qpos", qp16, RQ, D, false);
         steps.push_back([=](cudaStream_t st) { return launch_rt_add(tgt16, qp16, nullptr, D, 1, tq, RQ, st); });
         if (linear(L->qk, tq, D, (int)RQ, qkvh, 3 * D, false, ACT_NONE)) return 1;
         if (linear(L->v, tgt16, D, (int)RQ, qkvh + 2 * D, 3 * D, false, ACT_NONE)) return 1;
+        capture(dn + ".qkv", qkv, RQ, 3 * D, false);
         steps.push_back([=](cudaStream_t st) {
             return launch_flash_attention(qkvh, 3 * D, RQ, qkvh + D, qkvh + 2 * D, 3 * D, RQ, att, D, seqq, N, K, c.heads,
                                           D / c.heads, 0, st);
         });
         flops += 4.0 * N * (double)K * K * D;
+        capture(dn + ".att", att, RQ, D, false);
         if (linear(L->out, att, D, (int)RQ, y, D, true, ACT_NONE, tgt32, true, D)) return 1;
+        capture(dn + ".y1", y, RQ, D, true);
         steps.push_back([=](cudaStream_t st) {
             return launch_layernorm(reinterpret_cast<float*>(y), (int)RQ, D, D, L->n1.g, L->n1.b, 1e-5f, tgt16,
                                     reinterpret_cast<float*>(tgt32), nullptr, 1, nullptr, 0, 0, st);
         });
+        capture(dn + ".x1", tgt32, RQ, D, true);
+        capture(dn + ".x1_16", tgt16, RQ, D, false);
         // multi-scale deformable cross-attention
         steps.push_back([=](cudaStream_t st) { return launch_rt_add(tgt16, qp16, nullptr, D, 1, tq, RQ, st); });
         if (linear(L->ow, tq, D, (int)RQ, ow, n_ow, true, ACT_NONE)) return 1;
+        capture(dn + ".ow", ow, RQ, n_ow, true);
         steps.push_back([=](cudaStream_t st) {
             return launch_rt_deform_attn(reinterpret_cast<float*>(ow), n_ow, reinterpret_cast<float*>(ref), val,
                                          (long long)c.num_layers * D, i * D, lv, N, K, c.heads, D / c.heads, c.offset_scale,
                                          samp, D, st);
         });
+        capture(dn + ".samp", samp, RQ, D, false);
         if (linear(L->cross_out, samp, D, (int)RQ, y, D, true, ACT_NONE, tgt32, true, D)) return 1;
+        capture(dn + ".y2", y, RQ, D, true);
         steps.push_back([=](cudaStream_t st) {
             return launch_layernorm(reinterpret_cast<float*>(y), (int)RQ, D, D, L->n2.g, L->n2.b, 1e-5f, tgt16,
                                     reinterpret_cast<float*>(tgt32), nullptr, 1, nullptr, 0, 0, st);
         });
+        capture(dn + ".x2", tgt32, RQ, D, true);
+        capture(dn + ".x2_16", tgt16, RQ, D, false);
         if (linear(L->lin1, tgt16, D, (int)RQ, ffn, c.ffn, false, ACT_RELU)) return 1;
+        capture(dn + ".ffn", ffn, RQ, c.ffn, false);
         if (linear(L->lin2, ffn, c.ffn, (int)RQ, y, D, true, ACT_NONE, tgt32, true, D)) return 1;
+        capture(dn + ".y3", y, RQ, D, true);
         steps.push_back([=](cudaStream_t st) {
             return launch_layernorm(reinterpret_cast<float*>(y), (int)RQ, D, D, L->n3.g, L->n3.b, 1e-5f, tgt16,
                                     reinterpret_cast<float*>(tgt32), nullptr, 1, nullptr, 0, 0, st);
         });
+        capture(dn + ".x3", tgt32, RQ, D, true);
+        capture(dn + ".x3_16", tgt16, RQ, D, false);
         // iterative box refinement (:428-441)
         if (linear(L->box0, tgt16, D, (int)RQ, h1, D, false, ACT_RELU) || linear(L->box1, h1, D, (int)RQ, h2, D, false, ACT_RELU) ||
             linear(L->box2, h2, D, (int)RQ, delta, 4, true, ACT_NONE))
             return 1;
+        capture(dn + ".h1", h1, RQ, D, false);
+        capture(dn + ".h2", h2, RQ, D, false);
+        capture(dn + ".delta", delta, RQ, 4, true);
         steps.push_back([=](cudaStream_t st) {
             return launch_rt_ref_update(reinterpret_cast<float*>(delta), 4, nullptr, reinterpret_cast<float*>(ref), (int)RQ, st);
         });
     }
+    capture("dec" + std::to_string(c.num_layers) + ".ref", ref, RQ, 4, true);
     if (linear(model.score_last, tgt16, D, (int)RQ, lg, 8, true, ACT_NONE)) return 1;
     steps.push_back([=](cudaStream_t st) {
         return launch_rt_copy_cols(reinterpret_cast<float*>(lg), 8, C, out_logits, RQ, st);
@@ -647,17 +690,57 @@ int RtdetrEngine::build(const RtdetrModel& model, int n) {
     return 0;
 }
 
-int RtdetrEngine::run(cudaStream_t st) {
-    for (auto& s : steps)
-        if (s(st)) {
+int RtdetrEngine::run(cudaStream_t st, bool debug) {
+    ran = captured = false;
+    if (debug)
+        for (auto& kv : caps)
+            if (!kv.second.t.p) CK(cudaMalloc(&kv.second.t.p, kv.second.bytes));
+    size_t next = 0;   // cap_order is in build order, so `after` never decreases along it
+    auto copy_until = [&](size_t step) {
+        for (; debug && next < cap_order.size() && cap_order[next]->after <= step; ++next) {
+            const Capture& k = *cap_order[next];
+            CK(cudaMemcpyAsync(k.t.p, k.src, k.bytes, cudaMemcpyDeviceToDevice, st));
+        }
+        return 0;
+    };
+    for (size_t i = 0; i < steps.size(); ++i) {
+        if (copy_until(i)) return 1;
+        if (steps[i](st)) {
             if (!last_error()[0]) set_error("RT-DETRv2 step launch failed: %s", cudaGetErrorString(cudaGetLastError()));
             return 1;
         }
+    }
+    if (copy_until(steps.size())) return 1;
+    ran = true;
+    captured = debug;
     return 0;
+}
+
+int RtdetrEngine::debug_view(const std::string& name, DebugTensor* out) const {
+    const char* why;
+    auto it = dbg.find(name);
+    auto ct = caps.find(name);
+    if (it == dbg.end() && ct == caps.end()) {
+        why = "unknown name";
+    } else if (!ran) {
+        why = "no forward of this batch size has completed since its engine was built";
+    } else if (it != dbg.end()) {
+        *out = it->second;
+        return 0;
+    } else if (!captured) {
+        why = "captured only when debug capture was on for the last forward of this batch size";
+    } else {
+        *out = ct->second.t;
+        return 0;
+    }
+    set_error("RT-DETRv2 debug tensor '%s' (batch size %d): %s", name.c_str(), N, why);
+    return 1;
 }
 
 RtdetrEngine::~RtdetrEngine() {
     for (void* p : bufs) cudaFree(p);
+    for (auto& kv : caps)
+        if (kv.second.t.p) cudaFree(kv.second.t.p);
 }
 
 }  // namespace ytk

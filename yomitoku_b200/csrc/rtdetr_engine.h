@@ -83,12 +83,31 @@ struct RtdetrEngine {
     std::vector<void*> bufs;
     std::vector<std::function<int(cudaStream_t)>> steps;
     std::map<std::string, DebugTensor> dbg;
+    // Stage read-out for the tests (ytk_rtdetr_set_debug / ytk_rtdetr_debug_tensor).  Stages the engine later overwrites
+    // in place are registered as captures: with `debug` on, run() copies each into its own buffer (allocated on the
+    // first such run, owned by the engine) right after the step that produced it.  With `debug` off the captures
+    // neither allocate nor run.  `ran` / `captured` describe the last run, so that a stage it did not produce is refused
+    // instead of read as zeros or stale data.
+    struct Capture {
+        size_t after = 0;      // runs before step `after` (after all steps built before it)
+        const void* src = nullptr;
+        DebugTensor t;         // t.p: the capture buffer (null until the first run with capture on)
+        size_t bytes = 0;
+    };
+    std::map<std::string, Capture> caps;
+    std::vector<const Capture*> cap_order;
+    bool ran = false, captured = false;
     int build(const RtdetrModel& model, int n);
-    int run(cudaStream_t st);
+    int run(cudaStream_t st, bool debug = false);
+    // The buffer behind a stage name of the last run; 1 + set_error for an unknown name or one the last run did not
+    // produce.
+    int debug_view(const std::string& name, DebugTensor* out) const;
     ~RtdetrEngine();
 
   private:
     int alloc(const std::string& name, long long rows, int c, bool f32, void** out, int n = 0, int h = 0, int w = 0);
+    void capture(const std::string& name, const void* src, long long rows, int c, bool f32, int n = 0, int h = 0,
+                 int w = 0);
     int conv(const ConvW& cw, const void* in, int n, int h, int w, long long in_ld, void* out, long long ldc, int act,
              const void* resid = nullptr, long long ldr = 0);
     int linear(const RtLinear& w, const void* A, long long lda, int M, void* out, long long ldc, bool out_f32, int act,

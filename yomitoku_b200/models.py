@@ -900,11 +900,17 @@ class RTDETRv2(_DeviceModel):
     def flops(self, n=1):
         return _lib.lib().ytk_rtdetr_flops(self._ensure(), n)
 
+    def set_debug(self, on):
+        """Test hook: with `on`, the next forwards also keep the stages the engine overwrites in place (CSP steps, the
+        AIFI residual sum, the encoder box head, every decoder layer's buffers); see ytk_rtdetr_debug_tensor."""
+        _lib.check(_lib.lib().ytk_rtdetr_set_debug(self._ensure(), 1 if on else 0))
+
     def debug_tensor(self, n, name):
         """Intermediate activation of the last forward of batch size n (test hook) as a numpy array."""
-        cap = 64 << 20
-        buf = torch.empty(cap, dtype=torch.float32)
+        h = self._ensure()
         shape = (ctypes.c_int * 4)()
-        _lib.check(_lib.lib().ytk_rtdetr_debug_tensor(self._ensure(), n, name.encode(), buf.data_ptr(), cap, shape))
+        _lib.check(_lib.lib().ytk_rtdetr_debug_tensor(h, n, name.encode(), None, 0, shape))
         dims = [int(v) for v in shape]
-        return buf[: dims[0] * dims[1] * dims[2] * dims[3]].reshape(dims).numpy().copy()
+        buf = np.empty(dims, dtype=np.float32)
+        _lib.check(_lib.lib().ytk_rtdetr_debug_tensor(h, n, name.encode(), buf.ctypes.data, buf.size, shape))
+        return buf
