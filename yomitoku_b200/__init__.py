@@ -16,10 +16,14 @@ Files in, documents out:
     from yomitoku_b200.export import export_markdown, export_html, export_csv, export_json
     result.to_markdown(path, img=page)                    # also to_html / to_csv (DocumentAnalyzerSchema)
     python -m yomitoku_b200 <file-or-dir> -f md -o out    # the command line (cli.py): batched analyze_pages
+
+Fields out of forms (extractor.py): `extract(parser(page)[0], schema)` or `TableSemanticParser.extract_pages(pages,
+schema)` with a YAML `ExtractionSchema`, and `python -m yomitoku_b200.extract <dir> -s schema.yaml -o out` (extract.py).
 """
 from .data import load_image
 from .device_pages import DevicePages, device_pages
 from .document_analyzer import DocumentAnalyzer
+from .extractor import ExtractionSchema, extract
 from .layout_analyzer import LayoutAnalyzer
 from .layout_parser import LayoutParser
 from .ocr import OCR
@@ -31,4 +35,4 @@ from .text_recognizer import TextRecognizer
 
 __all__ = ["OCR", "TextDetector", "TextRecognizer", "DocumentAnalyzer", "LayoutAnalyzer", "LayoutParser",
            "TableStructureRecognizer", "CellDetector", "TableSemanticParser", "DevicePages", "device_pages",
-           "load_image"]
+           "load_image", "ExtractionSchema", "extract"]

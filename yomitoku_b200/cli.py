@@ -188,6 +188,30 @@ def _check_input(path):
     return path
 
 
+def page_batches(path, pages_str, batch_size):
+    """The selected pages (--pages) of every file under `path`, in lists of up to `batch_size`.  The next list is
+    decoded in a worker thread while the caller works on the current one.  Under a directory, a file that cannot be
+    read as a page image is logged and skipped."""
+    pages = _pages(input_files(path), pages_str, skip_unreadable=path.is_dir())
+
+    def next_batch():
+        batch = []
+        for page in pages:
+            batch.append(page)
+            if len(batch) == batch_size:
+                break
+        return batch
+
+    with ThreadPoolExecutor(max_workers=1) as decoder:
+        pending = decoder.submit(next_batch)
+        while True:
+            batch = pending.result()
+            if not batch:
+                return
+            pending = decoder.submit(next_batch)
+            yield batch
+
+
 def run(args, analyzer):
     """Analyses every page under `args.arg1` with `analyzer.analyze_pages`, `args.batch` pages per call, and writes
     the outputs.  The next batch is decoded in a worker thread while the analyzer runs on the current one.  Returns the
@@ -197,41 +221,25 @@ def run(args, analyzer):
     os.makedirs(args.outdir, exist_ok=True)
     logger.info(f"Output directory: {args.outdir}")
 
-    pages = _pages(input_files(path), args.pages, skip_unreadable=path.is_dir())
-
-    def next_batch():
-        batch = []
-        for page in pages:
-            batch.append(page)
-            if len(batch) == args.batch:
-                break
-        return batch
-
     written, combined = [], {}
     start, n_pages = time.time(), 0
-    with ThreadPoolExecutor(max_workers=1) as decoder:
-        pending = decoder.submit(next_batch)
-        while True:
-            batch = pending.result()
-            if not batch:
-                break
-            pending = decoder.submit(next_batch)
-            results = analyzer.analyze_pages([p.img for p in batch])
-            for page, result in zip(batch, results):
-                stem = "%s_%s" % (_sanitize_path_component(page.file.parent.name), page.file.stem)
-                out_path = os.path.join(args.outdir, "%s_p%d.%s" % (stem, page.index + 1, fmt))
-                if not args.combine:
-                    _export_page(args, fmt, result, page.img, out_path)
-                    written.append(out_path)
-                    logger.info(f"Output file: {out_path}")
-                    continue
-                combined.setdefault(page.file, []).append(_convert_page(args, fmt, result, page.img, out_path))
-                if page.last:
-                    out_path = os.path.join(args.outdir, "%s.%s" % (stem, fmt))
-                    save_merged(fmt, merge_all_pages(fmt, combined.pop(page.file)), out_path, args.encoding)
-                    written.append(out_path)
-                    logger.info(f"Output file: {out_path}")
-            n_pages += len(batch)
+    for batch in page_batches(path, args.pages, args.batch):
+        results = analyzer.analyze_pages([p.img for p in batch])
+        for page, result in zip(batch, results):
+            stem = "%s_%s" % (_sanitize_path_component(page.file.parent.name), page.file.stem)
+            out_path = os.path.join(args.outdir, "%s_p%d.%s" % (stem, page.index + 1, fmt))
+            if not args.combine:
+                _export_page(args, fmt, result, page.img, out_path)
+                written.append(out_path)
+                logger.info(f"Output file: {out_path}")
+                continue
+            combined.setdefault(page.file, []).append(_convert_page(args, fmt, result, page.img, out_path))
+            if page.last:
+                out_path = os.path.join(args.outdir, "%s.%s" % (stem, fmt))
+                save_merged(fmt, merge_all_pages(fmt, combined.pop(page.file)), out_path, args.encoding)
+                written.append(out_path)
+                logger.info(f"Output file: {out_path}")
+        n_pages += len(batch)
     logger.info("%d page(s) in %.2f sec" % (n_pages, time.time() - start))
     return written
 

@@ -240,6 +240,11 @@ class TableSemanticContentsSchema(BaseSchema):
         from .document_analyzer import is_contained
         return [c for c in self.cells.values() if c.role != "group" and is_contained(box, c.box, threshold=0.5)]
 
+    def search_cells_by_query(self, query):
+        """Non-group cells whose text contains `query`, half- and full-width spaces ignored on both sides."""
+        q = _strip_spaces(query)
+        return [c for c in self.cells.values() if c.contents and c.role != "group" and q in _strip_spaces(c.contents)]
+
     def search_kv_items_by_key(self, key):
         """[{"key": key cells, "value": value cell}] of the items whose key text contains `key` (spaces ignored), then
         for every grid column whose header text contains it one {"key": header cells, "value": []} per grid row - the

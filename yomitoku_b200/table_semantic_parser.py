@@ -350,3 +350,11 @@ class TableSemanticParser:
                         device=self.device)
         return [semantic_page(r.words, ts, lay.paragraphs, None, grid_only, kv_only)
                 for r, ts, lay in zip(ocr, tables, layouts)]
+
+    def extract_pages(self, pages, schema, normalize=True, simple=False):
+        """The fields of an extraction schema (extractor.py; an ExtractionSchema, a dict in its form or a YAML path)
+        from every page: `parse_pages` on the batch, then `extractor.extract` on each page's result.  Returns one dict
+        per page, each equal to `extract(self(page)[0], schema, normalize, simple)`."""
+        from .extractor import as_schema, extract
+        schema = as_schema(schema)
+        return [extract(r, schema, normalize, simple) for r in self.parse_pages(pages)]
