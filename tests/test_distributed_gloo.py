@@ -1,5 +1,6 @@
 """CPU, world_size 2 over gloo: the multi-GPU plumbing (weight broadcast, group balancing, crop scatter, result
-gather) with a stand-in recognizer - the exchange logic is independent of the model."""
+gather) with a stand-in recognizer - the exchange logic is independent of the model.  Every crop source (records cut
+"on the device", the crop arena, packed host canvases) takes the same planned exchange."""
 import os
 import socket
 import sys
@@ -55,7 +56,7 @@ def _worker(rank, world, port, q):
             canv = [rng.integers(0, 256, size=(32, w, 3), dtype=np.uint8) for w in widths]
             groups.append((canv, [max(widths)] * n))
         costs = [sum(4 * (p // 8) for p in g[1]) for g in groups]
-        all_costs = par.gather_costs(costs)
+        all_costs = par.all_gather_objects(costs, "plan")
         assert all_costs[rank] == costs and len(all_costs) == world
         assign = par.balance_groups(all_costs, world)
         loads = [0.0] * world
@@ -64,13 +65,6 @@ def _worker(rank, world, port, q):
                 loads[d] += all_costs[r][gi]
         before = max(sum(c) for c in all_costs)
         assert max(loads) < before            # balancing helped
-        work = par.exchange_groups(groups, assign[rank])
-        assert sum(1 for w in work if w[0] == rank) == sum(1 for d in assign[rank] if d == rank)
-        res = [_fake_recognise(w[2]) for w in work]
-        back = par.return_results(work, res, len(groups))
-        for (canv, _), (ids, probs) in zip(groups, back):
-            eid, ep = _fake_recognise(canv)
-            assert np.array_equal(ids, eid) and np.array_equal(probs, ep)
         q.put((rank, "ok", loads))
     except Exception as e:  # pragma: no cover
         import traceback
@@ -80,20 +74,13 @@ def _worker(rank, world, port, q):
 
 
 class _StubModel:
-    """Stands in for models.PARSeq: both device entry points, computed from the crop pixels on the host."""
+    """Stands in for models.PARSeq's packed device entry, computed from the crop pixels on the host."""
     refine_iters = 1
     max_label_length = 100
 
     def __init__(self, cfg):
         self.cfg = cfg
         self.calls = 0
-
-    def pack_crops(self, canvases, padded, groups):
-        return canvases, sum(c.size for c in canvases), None, 0
-
-    def run_packed(self, buf, total, descs, n, n_groups, stream=None):
-        ids, probs = _fake_recognise(buf)
-        return ids, probs, np.full((n_groups,), 101, np.int32)
 
     def run_packed_ptr(self, ptr, on_device, total, descs, n, n_groups, stream=None):
         import ctypes
@@ -105,12 +92,40 @@ class _StubModel:
         return ids, probs, np.full((n_groups,), 101, np.int32)
 
 
+def _exchange_spy(par_mod, moved):
+    """Wraps parallel.exchange_canvases_planned: records the split sizes of every crop scatter."""
+    orig = par_mod.exchange_canvases_planned
+
+    def spy(canv, send_splits, recv_splits, out=None):
+        assert isinstance(canv, torch.Tensor) and canv.dtype == torch.uint8     # one flat buffer, never host lists
+        # the receive buffer is the tail of the recognizer's work buffer: own and received crops go through ONE
+        # packed recognizer call
+        assert out is not None and out.numel() == sum(recv_splits)
+        moved.append(([int(b) for b in send_splits], [int(b) for b in recv_splits]))
+        return orig(canv, send_splits, recv_splits, out=out)
+
+    par_mod.exchange_canvases_planned = spy
+
+
+def _check_one_scatter(par_mod, moved, rank):
+    """Rank 0 hands several groups to rank 1 as one buffer (the balancer may send a small group of rank 1 the other
+    way); what one rank sends is what the other receives."""
+    assert len(moved) == 1
+    send, recv = moved[0]
+    assert send[rank] == 0 and recv[rank] == 0
+    assert (send[1] > 0) if rank == 0 else (recv[0] > 0)
+    assert par_mod.STATS["exchange_calls"] == 1
+    assert par_mod.STATS["exchange_bytes_sent"] == sum(send) and par_mod.STATS["exchange_bytes_received"] == sum(recv)
+
+
 def _worker_pipeline(rank, world, port, q):
-    """BatchedOCR._run_groups across 2 ranks with crops that live in the shared arena (stub recognizer)."""
+    """BatchedOCR._run_groups across 2 ranks with crops that live in the shared page-locked arena (stub recognizer):
+    the leaving canvases are gathered from the arena and take the planned exchange."""
     sys.path.insert(0, ROOT)
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
+        from yomitoku_b200 import parallel as par_mod
         from yomitoku_b200 import pipeline as pl
         from yomitoku_b200.config import TextRecognizerPARSeqLargeV41Config, to_config
         cfg = to_config(TextRecognizerPARSeqLargeV41Config())
@@ -123,23 +138,28 @@ def _worker_pipeline(rank, world, port, q):
         rng = np.random.default_rng(10 + rank)
         arena = pl._SharedBuf(1 << 20)
         n_groups = 7 if rank == 0 else 1
-        groups, expect, off = [], [], 0
+        groups, expect, offs, sizes = [], [], [], []
         for gi in range(n_groups):
             n = int(rng.integers(1, 5))
             widths = (rng.integers(9, 30, size=n) * 8).tolist()
-            offs = []
             canv = []
             for w in widths:
                 c = rng.integers(0, 256, size=(32, w, 3), dtype=np.uint8)
+                off = (offs[-1] + sizes[-1] + 96 * 3) if offs else 0      # gaps: canvases need not be back to back
                 arena.np[off:off + c.size] = c.reshape(-1)
                 offs.append(off)
-                off += c.size
+                sizes.append(c.size)
                 canv.append(c)
-            groups.append((widths, [max(widths)] * n, np.asarray(offs, np.int64)))
+            groups.append((widths, [max(widths)] * n, np.arange(len(offs) - n, len(offs))))
             expect.append(_fake_recognise(canv))
-        res = ocr._run_groups(groups, None, arena, 32)
+        moved = []
+        _exchange_spy(par_mod, moved)
+        calls0 = Rec.model.calls
+        res = ocr._run_groups(groups, pl._FlatCrops(arena.torch, offs, sizes))
+        assert Rec.model.calls - calls0 == 1          # own + received groups: one packed call
         for (ids, probs, glen), (eid, ep) in zip(res, expect):
             assert np.array_equal(ids, eid) and np.array_equal(probs, ep) and glen == 101
+        _check_one_scatter(par_mod, moved, rank)
         arena.close()
         q.put((rank, "ok", None))
     except Exception:  # pragma: no cover
@@ -197,36 +217,18 @@ def _worker_pipeline_dev(rank, world, port, q):
             groups.append((widths, [max(widths)] * len(b), np.asarray(b, np.int64)))
             expect.append(_fake_recognise([ds.data[i] for i in b]))
         moved = []
-        orig_x = par_mod.exchange_canvases_planned
-
-        def spy(canv, send_splits, recv_splits, out=None):
-            assert isinstance(canv, torch.Tensor) and canv.dtype == torch.uint8     # one flat buffer, never host lists
-            # the receive buffer is the tail of the recognizer's work buffer: own and received crops go through ONE
-            # packed recognizer call
-            assert out is not None and out.numel() == sum(recv_splits)
-            moved.append(([int(b) for b in send_splits], [int(b) for b in recv_splits]))
-            return orig_x(canv, send_splits, recv_splits, out=out)
-
-        par_mod.exchange_canvases_planned = spy
-        par_mod.exchange_groups = None              # the host-staged scatter must not be used any more
+        _exchange_spy(par_mod, moved)
         # the three phases separately, as stream() runs them (planner / recognizer / assembly thread)
-        lv = np.zeros(len(geoms), np.int64)
-        dplan = ocr._plan_groups_dist(groups, geoms, lv)
-        assert dplan["moves"] and (rank != 0 or len(dplan["send"]) > 0)     # rank 0 (8 groups) must hand some over
+        src = pl._RecordCrops(geoms, None, np.ascontiguousarray(page)[None])
+        dplan = ocr._plan_groups_dist(groups, src)
+        assert isinstance(dplan, dict) and (rank != 0 or len(dplan["send"]) > 0)   # rank 0 (8 groups) hands some over
         calls0 = Rec.model.calls
-        pending = ocr._run_groups_dist_dev(groups, geoms, np.ascontiguousarray(page)[None], None, lv, dplan)
+        pending = ocr._run_planned(dplan, src)
         assert Rec.model.calls - calls0 == 1          # own + received groups: one packed call
         res = ocr._finish_results(pending)
         for (ids, probs, glen), (eid, ep) in zip(res, expect):
             assert np.array_equal(ids, eid) and np.array_equal(probs, ep) and glen == 101
-        # rank 0 (8 groups) hands several groups to rank 1 (2 groups) as one buffer (the balancer may send a small
-        # group of rank 1 the other way); what one rank sends is what the other receives
-        assert len(moved) == 1
-        send, recv = moved[0]
-        assert send[rank] == 0 and recv[rank] == 0
-        assert (send[1] > 0) if rank == 0 else (recv[0] > 0)
-        assert par_mod.STATS["exchange_calls"] == 1
-        assert par_mod.STATS["exchange_bytes_sent"] == sum(send) and par_mod.STATS["exchange_bytes_received"] == sum(recv)
+        _check_one_scatter(par_mod, moved, rank)
         # and the one-call wrapper gives the same
         res2 = ocr._run_groups_dev(groups, geoms, np.ascontiguousarray(page)[None], None)
         for (ids, probs, glen), (eid, ep) in zip(res2, expect):
@@ -262,6 +264,7 @@ def _worker_pipeline_balanced(rank, world, port, q):
         from yomitoku_b200 import parallel as par
         from yomitoku_b200 import pipeline as pl
         from yomitoku_b200.config import TextRecognizerPARSeqLargeV41Config, to_config
+        from yomitoku_b200.models import pack_canvases
         cfg = to_config(TextRecognizerPARSeqLargeV41Config())
 
         class Rec:
@@ -271,8 +274,8 @@ def _worker_pipeline_balanced(rank, world, port, q):
         def forbidden(*a, **k):
             raise AssertionError("no exchange expected for balanced ranks")
 
-        par.exchange_groups = forbidden
-        par.return_results = forbidden
+        par.exchange_canvases_planned = forbidden
+        par.exchange_results_planned = forbidden
         ocr = pl.BatchedOCR(None, Rec(), workers=1)
         rng = np.random.default_rng(5)                    # same widths on both ranks: equal costs
         groups, expect = [], []
@@ -280,9 +283,13 @@ def _worker_pipeline_balanced(rank, world, port, q):
             widths = (rng.integers(9, 30, size=3) * 8).tolist()
             canv = [np.random.default_rng(100 * rank + 10 * gi + j).integers(0, 256, size=(32, w, 3), dtype=np.uint8)
                     for j, w in enumerate(widths)]
-            groups.append((canv, [max(widths)] * 3))
+            groups.append((canv, [max(widths)] * 3, np.arange(3 * gi, 3 * gi + 3)))
             expect.append(_fake_recognise(canv))
-        res = ocr._run_groups(groups, None, None, 32)
+        # host canvases, packed into one buffer as prepare_pooled does
+        canvases = [c for g in groups for c in g[0]]
+        buf, _, offs = pack_canvases(canvases)
+        groups = [([c.shape[1] for c in g[0]], g[1], g[2]) for g in groups]
+        res = ocr._run_groups(groups, pl._FlatCrops(buf, offs, [c.size for c in canvases]))
         for (ids, probs, glen), (eid, ep) in zip(res, expect):
             assert np.array_equal(ids, eid) and np.array_equal(probs, ep) and glen == 101
         q.put((rank, "ok", None))
@@ -321,7 +328,7 @@ def test_pipeline_groups_arena_world2():
         assert status == "ok", status
 
 
-def test_crop_scatter_gather_world2():
+def test_broadcast_and_balance_world2():
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
     port = _free_port()

@@ -155,13 +155,3 @@ def test_recognizer_call_device_crops_equals_host_crops():
     d, _ = rec(page, None)
     assert a.contents == b.contents and a.directions == b.directions and np.allclose(a.scores, b.scores, atol=1e-6)
     assert c.contents == d.contents
-
-
-def test_host_canvases_copy():
-    """The page-locked host copy of device-cut canvases used for the cross-rank exchange (pipeline._HostCanvases)."""
-    from yomitoku_b200.pipeline import _HostCanvases
-    t = torch.arange(0, 100000, dtype=torch.int32, device="cuda").to(torch.uint8)
-    s = torch.cuda.Stream()
-    for st in (None, s):
-        h = _HostCanvases(t, st)
-        assert h.np.dtype == np.uint8 and np.array_equal(h.np, t.cpu().numpy())

@@ -1,8 +1,8 @@
 """GPU, world_size 2 over NCCL (skipped on single-GPU boxes): the crop scatter on hardware.  Rank 0 owns many mini-batch
 groups, rank 1 few; `BatchedOCR._run_groups_dev` balances them with the GPU-to-GPU all_to_all (device canvases, no host
 staging) and every rank must get back, for each of its own groups, exactly the ids / probabilities a single-rank run
-(`_run_groups_dev_local` on the same records) produces - bit for bit, since a crop's result does not depend on which
-GPU recognises it (same kernels, same padded width, same group)."""
+(`_run_chunks` of the single-rank plan on the same records) produces - bit for bit, since a crop's result does not
+depend on which GPU recognises it (same kernels, same padded width, same group)."""
 import os
 import socket
 import sys
@@ -33,7 +33,7 @@ def _worker(rank, world, port, q):
         from yomitoku_b200 import TextRecognizer
         from yomitoku_b200 import parallel as par
         from yomitoku_b200.data import crop_geometry
-        from yomitoku_b200.pipeline import BatchedOCR
+        from yomitoku_b200.pipeline import BatchedOCR, _RecordCrops
         from yomitoku_b200.synth import peaked_parseq_state_dict, synthetic_page
         from yomitoku_b200.text_recognizer import plan_mini_batches
         rec = TextRecognizer(model_name="parseq-tiny-dynw-v4", from_pretrained=False, device="cuda:%d" % rank,
@@ -50,7 +50,8 @@ def _worker(rank, world, port, q):
         padded, _ = rec._collate_widths(widths, plan)
         groups = [([widths[i] for i in b], [padded[i] for i in b], np.asarray(b, np.int64)) for b in plan]
         pages_dev = torch.from_numpy(np.ascontiguousarray(page))[None].cuda()
-        ref = ocr._run_groups_dev_local(groups, geoms, pages_dev, None)
+        # the single-rank plan and chunk runner: no collective
+        ref = ocr._run_chunks(ocr._plan_groups_dev(groups, geoms), _RecordCrops(geoms, None, pages_dev))
         x0 = dict(par.STATS)
         got = ocr._run_groups_dev(groups, geoms, pages_dev, None)
         moved = par.STATS["exchange_bytes_sent"] - x0["exchange_bytes_sent"]

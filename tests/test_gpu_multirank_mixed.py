@@ -1,7 +1,7 @@
 """GPU, world_size 2 over NCCL (skipped on single-GPU boxes): the crop scatter for a batch of pages of different sizes.
 Each rank holds its pages as one flat device buffer with a page table; the groups that leave a rank are cut from that
 table before the all_to_all, and every rank must get back, for each of its own groups, exactly the ids / probabilities a
-single-rank run (`_run_groups_dev_local` on the same records and pages) produces."""
+single-rank run (`_run_chunks` of the single-rank plan on the same records and pages) produces."""
 import os
 import sys
 
@@ -26,7 +26,7 @@ def _worker(rank, world, port, q):
         from yomitoku_b200 import TextRecognizer
         from yomitoku_b200 import parallel as par
         from yomitoku_b200.data import crop_geometry, page_table
-        from yomitoku_b200.pipeline import BatchedOCR
+        from yomitoku_b200.pipeline import BatchedOCR, _RecordCrops
         from yomitoku_b200.synth import peaked_parseq_state_dict, synthetic_page
         from yomitoku_b200.text_recognizer import plan_mini_batches
         rec = TextRecognizer(model_name="parseq-tiny-dynw-v4", from_pretrained=False, device="cuda:%d" % rank,
@@ -49,7 +49,8 @@ def _worker(rank, world, port, q):
         table, _ = page_table([p.shape[:2] for p in pages])
         flat = torch.from_numpy(np.concatenate([p.reshape(-1) for p in pages])).cuda()
         pages_dev = (flat, table)
-        ref = ocr._run_groups_dev_local(groups, geoms, pages_dev, None)
+        # the single-rank plan and chunk runner: no collective
+        ref = ocr._run_chunks(ocr._plan_groups_dev(groups, geoms), _RecordCrops(geoms, None, pages_dev))
         x0 = dict(par.STATS)
         got = ocr._run_groups_dev(groups, geoms, pages_dev, None)
         moved = par.STATS["exchange_bytes_sent"] - x0["exchange_bytes_sent"]

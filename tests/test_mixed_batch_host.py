@@ -193,7 +193,8 @@ def _words(results):
 
 
 @pytest.mark.parametrize("device_crops,workers,source_downscale", [(True, 2, False), (False, 2, False),
-                                                                   (True, 1, False), (True, 2, True)])
+                                                                   (True, 1, False), (True, 2, True),
+                                                                   (False, 1, False)])
 def test_mixed_batch_equals_batches_of_one_through_tables(monkeypatch, device_crops, workers, source_downscale):
     det, rec, calls = _stub_models(monkeypatch, source_downscale)
     mixed = _mixed_pages()

@@ -510,6 +510,33 @@ def _parseq_random_state_dict(cfg, seed=0):
     return sd
 
 
+def pack_canvases(canvases):
+    """Crop canvases back to back in one uint8 buffer (page-locked when CUDA is available), the layout a packed
+    recognizer call reads.  Returns (buffer, bytes used, byte offset of every canvas)."""
+    sizes = np.asarray([c.size for c in canvases], np.int64)
+    offs = np.cumsum(sizes) - sizes
+    total = int(sizes.sum())
+    buf = torch.empty(max(total, 1), dtype=torch.uint8, pin_memory=torch.cuda.is_available())
+    nb = buf.numpy()
+    for o, c in zip(offs.tolist(), canvases):
+        nb[o:o + c.size] = np.ascontiguousarray(c).reshape(-1)
+    return buf, total, offs
+
+
+def crop_descriptors(cfg, pix_off, widths, padded_widths, groups):
+    """The ytk_crop records of one packed recognizer call (numpy, np.dtype(_lib.YtkCrop)), crops in packing order:
+    canvas byte offset, canvas width, padded width and mini-batch index per crop; every crop's encoder tokens follow
+    those of the crops before it.  cfg: the recognizer config (patch size, canvas height)."""
+    ph, pw = cfg.encoder.patch_size
+    gh = cfg.data.img_size[0] // ph
+    wp = np.asarray(padded_widths, np.int64)
+    ntok = gh * (wp // pw)
+    descs = np.zeros(len(wp), dtype=np.dtype(_lib.YtkCrop))
+    descs["pix_off"], descs["w"], descs["wp"] = pix_off, widths, wp
+    descs["tok_off"], descs["ntok"], descs["group"] = np.cumsum(ntok) - ntok, ntok, groups
+    return descs
+
+
 class PARSeq(_DeviceModel):
     """reference models/parseq.py:49-311.  `model(images)` takes (B,3,32,W) fp32 in [-1,1] and returns logits
     (B, S, C); `recognize_crops` is the fused ragged path that returns only (ids, probs)."""
@@ -621,36 +648,16 @@ class PARSeq(_DeviceModel):
         return logits
 
     def pack_crops(self, canvases, padded_widths, groups):
-        """Packs canvases into one pinned uint8 buffer + ytk_crop descriptors (host side of recognize_crops)."""
-        n = len(canvases)
-        ph, pw = self.cfg.encoder.patch_size
-        gh = self.cfg.data.img_size[0] // ph
-        sizes = [int(c.shape[0] * c.shape[1] * 3) for c in canvases]
-        total = int(sum(sizes))
-        buf = torch.empty(max(total, 1), dtype=torch.uint8, pin_memory=torch.cuda.is_available())
-        nb = buf.numpy()
-        descs = (_lib.YtkCrop * max(n, 1))()
-        off = tok = 0
-        for i, c in enumerate(canvases):
-            nb[off:off + sizes[i]] = np.ascontiguousarray(c).reshape(-1)
-            wp = int(padded_widths[i])
-            ntok = gh * (wp // pw)
-            descs[i] = _lib.YtkCrop(off, int(c.shape[1]), wp, tok, ntok, int(groups[i]))
-            off += sizes[i]
-            tok += ntok
-        return buf, total, descs, tok
+        """Packs canvases into one pinned uint8 buffer + ytk_crop descriptors (host side of recognize_crops).
+        Returns (buffer, bytes used, descriptors, encoder tokens); the descriptors are a record array, so a crop's
+        fields read as attributes (`d.pix_off`) as they do on a ytk_crop struct."""
+        buf, total, offs = pack_canvases(canvases)
+        descs = crop_descriptors(self.cfg, offs, [c.shape[1] for c in canvases], padded_widths, groups)
+        return buf, total, descs.view(np.recarray), int(descs["ntok"].sum())
 
     def run_packed(self, buf, total, descs, n, n_groups, stream=None):
         """Device call on a packed crop buffer (torch uint8 tensor, pinned host or cuda)."""
-        h = self._ensure()
-        S = self.max_label_length + 1
-        ids = np.empty((n, S), dtype=np.int32)
-        probs = np.empty((n, S), dtype=np.float32)
-        glen = np.empty((max(n_groups, 1),), dtype=np.int32)
-        _lib.check(_lib.lib().ytk_parseq_forward_crops(h, buf.data_ptr(), 1 if buf.is_cuda else 0, total, descs, n,
-                                                       n_groups, ids.ctypes.data, probs.ctypes.data, glen.ctypes.data,
-                                                       _stream_ptr(stream)))
-        return ids, probs, glen[:n_groups]
+        return self.run_packed_ptr(buf.data_ptr(), 1 if buf.is_cuda else 0, total, descs, n, n_groups, stream)
 
     def run_packed_ptr(self, ptr, on_device, total, descs, n, n_groups, stream=None):
         """Device call on `total` bytes of crop canvases at address `ptr` (page-locked host or device memory); descs is

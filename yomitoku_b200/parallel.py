@@ -9,9 +9,9 @@ What crosses the fabric (SURVEY.md section 8e) - never inside a forward pass:
                              assignment, descriptors - exchanged one batch ahead by the planner threads), data plane
                              `exchange_canvases_planned`: ONE all_to_all_single of device uint8 canvases over NCCL;
   * the result gather        (ids int32, probs fp32) per crop back to the owning rank over a second gloo group
-                             (`BatchedOCR._finish_results`, assembly thread).
-  * `exchange_groups` / `return_results`: the host-staged variant for crops cut by OpenCV on the host
-                             (`YTK_DEVICE_CROPS=0`).
+                             (`exchange_results_planned`, `BatchedOCR._finish_results`, assembly thread).
+Crops cut on the device leave from HBM as they are; crops cut by OpenCV on the host (`YTK_DEVICE_CROPS=0`) are
+gathered and uploaded once, then take the same exchange.
 Pages are sharded by rank for detection (page p -> rank p // pages_per_rank); that needs no communication.
 """
 import numpy as np
@@ -63,25 +63,6 @@ def balance_groups(costs_by_rank, world, tolerance=0.03):
             load[r] -= c
             load[dst] += c
     return assign
-
-
-def _all_to_all_bytes(send_chunks):
-    """send_chunks[k]: 1-D uint8 torch tensor for rank k.  Returns the list of received uint8 tensors."""
-    world = dist.get_world_size()
-    device = _dev()
-    sizes = torch.tensor([c.numel() for c in send_chunks], dtype=torch.int64, device=device)
-    recv_sizes = torch.empty(world, dtype=torch.int64, device=device)
-    dist.all_to_all_single(recv_sizes, sizes)
-    rs = recv_sizes.tolist()
-    send = torch.cat([c.to(device) for c in send_chunks]) if sum(c.numel() for c in send_chunks) else \
-        torch.empty(0, dtype=torch.uint8, device=device)
-    recv = torch.empty(int(sum(rs)), dtype=torch.uint8, device=device)
-    dist.all_to_all_single(recv, send, output_split_sizes=rs, input_split_sizes=sizes.tolist())
-    out, off = [], 0
-    for n in rs:
-        out.append(recv[off:off + n].cpu())
-        off += n
-    return out
 
 
 STATS = {"exchange_calls": 0, "exchange_bytes_sent": 0, "exchange_bytes_received": 0, "exchange_ms": 0.0,
@@ -147,90 +128,3 @@ def exchange_results_planned(send, send_splits, recv_splits):
     STATS["results_ms"] += (time.perf_counter() - t0) * 1e3
     STATS["results_bytes_sent"] = STATS.get("results_bytes_sent", 0) + int(send.size)
     return recv.numpy()
-
-
-def _pack_group(canvases, padded, gid):
-    """-> uint8 tensor: header int32 [n, gid], per crop int32 [w, wp], then the canvases back to back."""
-    n = len(canvases)
-    meta = np.array([n, gid] + [v for c, p in zip(canvases, padded) for v in (c.shape[1], p)], dtype=np.int32)
-    body = [np.ascontiguousarray(c).reshape(-1) for c in canvases]
-    return torch.from_numpy(np.concatenate([meta.view(np.uint8)] + body)) if n else torch.from_numpy(meta.view(np.uint8).copy())
-
-
-def _unpack_groups(buf, height=32):
-    """Inverse of a concatenation of _pack_group blobs -> list of (gid, canvases, padded)."""
-    a = buf.numpy()
-    out, off = [], 0
-    while off < a.size:
-        n, gid = a[off:off + 8].view(np.int32)
-        off += 8
-        wm = a[off:off + 8 * n].view(np.int32).reshape(n, 2)
-        off += 8 * n
-        canv = []
-        for w, _ in wm:
-            sz = height * int(w) * 3
-            canv.append(a[off:off + sz].reshape(height, int(w), 3))
-            off += sz
-        out.append((int(gid), canv, [int(p) for _, p in wm]))
-    return out
-
-
-def exchange_groups(groups, assign_row, height=32):
-    """groups: list of (canvases, padded_widths) this rank owns; assign_row[g] = destination rank.
-    Returns work = list of (owner_rank, owner_gid, canvases, padded) this rank must recognise (own groups first)."""
-    world, rank = dist.get_world_size(), dist.get_rank()
-    chunks = [[] for _ in range(world)]
-    for g, (canv, padded) in enumerate(groups):
-        if assign_row[g] != rank:
-            chunks[assign_row[g]].append(_pack_group(canv, padded, g))
-    send = [torch.cat(c) if c else torch.empty(0, dtype=torch.uint8) for c in chunks]
-    recv = _all_to_all_bytes(send)
-    work = [(rank, g, canv, padded) for g, (canv, padded) in enumerate(groups) if assign_row[g] == rank]
-    for src, blob in enumerate(recv):
-        for gid, canv, padded in _unpack_groups(blob, height):
-            work.append((src, gid, canv, padded))
-    return work
-
-
-def return_results(work, results, n_groups_local, S=101):
-    """work as returned by exchange_groups; results[i] = (ids int32 (n,S), probs f32 (n,S)) for work[i].
-    Sends every foreign group's result back to its owner; returns out[g] = (ids, probs) for the local groups."""
-    world, rank = dist.get_world_size(), dist.get_rank()
-    out = [None] * n_groups_local
-    chunks = [[] for _ in range(world)]
-    for (owner, gid, canv, _), (ids, probs) in zip(work, results):
-        if owner == rank:
-            out[gid] = (ids, probs)
-        else:
-            head = np.array([gid, ids.shape[0]], dtype=np.int32).view(np.uint8)
-            chunks[owner].append(torch.from_numpy(np.concatenate(
-                [head, np.ascontiguousarray(ids, dtype=np.int32).view(np.uint8).reshape(-1),
-                 np.ascontiguousarray(probs, dtype=np.float32).view(np.uint8).reshape(-1)])))
-    send = [torch.cat(c) if c else torch.empty(0, dtype=torch.uint8) for c in chunks]
-    for blob in _all_to_all_bytes(send):
-        a, off = blob.numpy(), 0
-        while off < a.size:
-            gid, n = a[off:off + 8].view(np.int32)
-            off += 8
-            ids = a[off:off + 4 * n * S].view(np.int32).reshape(n, S).copy()
-            off += 4 * n * S
-            probs = a[off:off + 4 * n * S].view(np.float32).reshape(n, S).copy()
-            off += 4 * n * S
-            out[int(gid)] = (ids, probs)
-    return out
-
-
-def gather_costs(local_costs):
-    """all_gather of the per-group costs -> costs_by_rank (list of lists), identical on every rank."""
-    world = dist.get_world_size()
-    device = _dev()
-    n = torch.tensor([len(local_costs)], dtype=torch.int64, device=device)
-    ns = [torch.zeros(1, dtype=torch.int64, device=device) for _ in range(world)]
-    dist.all_gather(ns, n)
-    m = int(max(t.item() for t in ns))
-    mine = torch.zeros(max(m, 1), dtype=torch.int64, device=device)
-    if local_costs:
-        mine[:len(local_costs)] = torch.tensor(local_costs, dtype=torch.int64, device=device)
-    allc = [torch.zeros_like(mine) for _ in range(world)]
-    dist.all_gather(allc, mine)
-    return [allc[r][:int(ns[r].item())].tolist() for r in range(world)]

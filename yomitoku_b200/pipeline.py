@@ -207,7 +207,7 @@ def _host_stage(args):
             widths.append(c.shape[1])
         else:
             spill.append(c)
-    return quads, scores, _ArenaRef(widths, spill, ds.data[0].shape[0]), ds.content_widths, len(ds), \
+    return quads, scores, _ArenaRef(widths, spill), ds.content_widths, len(ds), \
         (t0, t1, time.perf_counter())
 
 
@@ -221,20 +221,19 @@ class _Runs:
 class _ArenaRef:
     """What a worker sends back instead of canvases: the widths of the crops it wrote into its arena slice."""
 
-    def __init__(self, widths, spill, height):
-        self.widths, self.spill, self.height = widths, spill, height
+    def __init__(self, widths, spill):
+        self.widths, self.spill = widths, spill
 
 
 class _PageCrops:
     """Crops of one page living in the shared arena at absolute byte offsets `offs` (list-like over canvases)."""
 
-    def __init__(self, arena_np, base, ref):
+    def __init__(self, arena_np, base, widths, height):
         self.arena_np = arena_np
-        self.height = ref.height
-        self.widths = list(ref.widths)
-        sizes = np.asarray(self.widths, dtype=np.int64) * (3 * self.height)
-        self.offs = (base + np.concatenate([[0], np.cumsum(sizes)[:-1]])).astype(np.int64) if len(sizes) else \
-            np.zeros((0,), np.int64)
+        self.height = height
+        self.widths = list(widths)
+        sizes = np.asarray(self.widths, dtype=np.int64) * (3 * height)
+        self.offs = base + np.cumsum(sizes) - sizes
 
     def __len__(self):
         return len(self.widths)
@@ -254,10 +253,82 @@ class _PageGeoms:
         self.levels = levels if levels is not None else np.zeros(len(geoms), np.int64)   # source_downscale pyramid level
         self.base = base
         self.widths = geoms["canvas_w"].tolist()
-        self.height = int(geoms["canvas_h"][0]) if len(geoms) else 32
 
     def __len__(self):
         return len(self.widths)
+
+
+# Where the pixels of a packed recognizer call come from.  Groups of crops are (widths, padded widths, crop indices
+# into a source); a source gives, for crop indices `idx` in packing order, the byte layout of their canvases
+# (`layout(idx) -> (bytes, offsets)`, host only, so a chunk is planned ahead of the GPU) and a flat buffer holding them
+# there (`fill(idx, stream)`).  `pack_layout` / `pack` do the same with the canvases back to back on the compute
+# device: what the crop scatter sends.
+
+class _FlatCrops:
+    """Canvases already sitting in one flat uint8 tensor at byte offsets `offs` (`nbytes` each): the page-locked crop
+    arena, a batch's host canvases packed by `prepare_pooled`, or the receive buffer of the crop scatter.  A chunk is
+    read in place: the recognizer gets the span from its first to its last byte."""
+
+    def __init__(self, buf, offs, nbytes):
+        self.buf = buf
+        self.offs = np.asarray(offs, np.int64)
+        self.nbytes = np.asarray(nbytes, np.int64)
+
+    @property
+    def on_device(self):
+        return 1 if self.buf.is_cuda else 0
+
+    def _span(self, idx):
+        o = self.offs[idx]
+        return int(o.min()), int((o + self.nbytes[idx]).max())
+
+    def layout(self, idx):
+        lo, hi = self._span(idx)
+        return hi - lo, self.offs[idx] - lo
+
+    def fill(self, idx, stream=None):
+        lo, hi = self._span(idx)
+        return self.buf[lo:hi]
+
+    def pack_layout(self, idx):
+        size = self.nbytes[idx]
+        return int(size.sum()), np.cumsum(size) - size
+
+    def pack(self, idx, stream=None):
+        """Gathers the canvases on the host and uploads them once (the buffer is a host one here)."""
+        import torch
+        from . import parallel as par
+        host = self.buf.numpy()
+        flat = np.concatenate([host[o:o + n] for o, n in zip(self.offs[idx].tolist(), self.nbytes[idx].tolist())])
+        return torch.from_numpy(flat).to(par._dev(), non_blocking=True)
+
+
+class _RecordCrops:
+    """Crops that exist only as ytk_crop_geom records (+ source_downscale levels) of the pages in HBM: the canvases of
+    a chunk are cut on the device, one extraction per pyramid level (models.extract_crops_pyramid)."""
+    on_device = 1
+
+    def __init__(self, geoms, levels=None, pages_dev=None):
+        self.geoms = geoms
+        self.levels = levels if levels is not None else np.zeros(len(geoms), np.int64)
+        # pyramid level -> pages; the levels above 0 are built on first use
+        self.pages = pages_dev if isinstance(pages_dev, dict) or pages_dev is None else {0: pages_dev}
+
+    def layout(self, idx):
+        from .models import plan_crop_offsets
+        return plan_crop_offsets(self.geoms[idx], self.levels[idx])
+
+    def fill(self, idx, stream=None):
+        from . import models
+        with _span("recognize.crops_device"):
+            return models.extract_crops_pyramid(self.pages, self.geoms[idx], self.levels[idx], stream)[0]
+
+    pack_layout, pack = layout, fill
+
+
+def _multi_rank():
+    import torch.distributed as dist
+    return dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1
 
 
 class BatchedOCR:
@@ -390,219 +461,184 @@ class BatchedOCR:
         maps = [plan.prob_map(out.numpy(), i) for i in range(len(pages))]
         return np.stack(maps) if len(set(plan.inputs)) == 1 else maps
 
-    def _run_groups_local(self, groups, stream=None):
-        """groups: list of (canvases, padded_widths).  One packed device call per <= max_tokens chunk (chunks end on
-        group boundaries).  Returns per group (ids, probs, group_len)."""
-        rec = self.recognizer
-        cfg = rec._cfg
+    def _group_tokens(self, g):
+        """Encoder tokens of one group (widths, padded widths, ...): what the chunking counts against max_tokens."""
+        cfg = self.recognizer._cfg
         ph, pw = cfg.encoder.patch_size
-        gh = cfg.data.img_size[0] // ph
-        out = [None] * len(groups)
-        start = 0
-        while start < len(groups):
-            end, tok = start, 0
-            while end < len(groups):
-                gtok = sum(gh * (p // pw) for p in groups[end][1])
-                if end > start and tok + gtok > self.max_tokens:
-                    break
-                tok += gtok
-                end += 1
-            canv = [c for g in groups[start:end] for c in g[0]]
-            pad = [p for g in groups[start:end] for p in g[1]]
-            grp = [k for k, g in enumerate(groups[start:end]) for _ in g[0]]
-            buf, total, descs, _ = rec.model.pack_crops(canv, pad, grp)
-            ids, probs, glen = rec.model.run_packed(buf, total, descs, len(canv), end - start, stream=stream)
-            off = 0
-            for k in range(start, end):
-                n = len(groups[k][0])
-                out[k] = (ids[off:off + n], probs[off:off + n], int(glen[k - start]))
-                off += n
-            start = end
-        return out
+        return (cfg.data.img_size[0] // ph) * (int(np.sum(g[1])) // pw)
 
-    def _run_groups_arena(self, groups, arena, height, stream=None):
-        """Like _run_groups_local for crops that already sit in the page-locked arena: groups = (widths, padded widths,
-        absolute arena offsets).  Descriptors are built with numpy; the device call copies one span of the arena."""
-        from . import _lib
-        rec = self.recognizer
-        cfg = rec._cfg
-        ph, pw = cfg.encoder.patch_size
-        gh = cfg.data.img_size[0] // ph
-        out = [None] * len(groups)
-        gtok = [gh * (int(np.sum(g[1])) // pw) for g in groups]
-        dt = np.dtype(_lib.YtkCrop)
-        start = 0
+    def _plan_chunks(self, groups, src):
+        """Host-only plan of the packed recognizer calls for `groups` (crop indices into `src`): <= max_tokens chunks
+        ending on group boundaries, each with its crop indices, canvas bytes and ytk_crop descriptors.
+        `BatchedOCR.stream` runs this for batch i + 1 in its own thread while batch i is on the GPU."""
+        from .models import crop_descriptors
+        gtok = [self._group_tokens(g) for g in groups]
+        chunks, start = [], 0
         while start < len(groups):
             end, tok = start, 0
             while end < len(groups) and not (end > start and tok + gtok[end] > self.max_tokens):
                 tok += gtok[end]
                 end += 1
             sel = groups[start:end]
-            w = np.concatenate([np.asarray(g[0], np.int64) for g in sel])
-            wp = np.concatenate([np.asarray(g[1], np.int64) for g in sel])
-            offs = np.concatenate([g[2] for g in sel])
-            n = w.shape[0]
-            lo = int(offs.min())
-            hi = int((offs + w * (3 * height)).max())
-            ntok = gh * (wp // pw)
-            descs = np.zeros(n, dtype=dt)
-            descs["pix_off"] = offs - lo
-            descs["w"] = w
-            descs["wp"] = wp
-            descs["tok_off"] = np.cumsum(ntok) - ntok
-            descs["ntok"] = ntok
-            descs["group"] = np.repeat(np.arange(end - start), [len(g[0]) for g in sel])
-            with _span("recognize.device"):
-                ids, probs, glen = rec.model.run_packed_ptr(arena.np.ctypes.data + lo, 0, hi - lo, descs, n, end - start,
-                                                            stream=stream)
-            off = 0
-            for k in range(start, end):
-                m = len(groups[k][0])
-                out[k] = (ids[off:off + m], probs[off:off + m], int(glen[k - start]))
-                off += m
+            sizes = [len(g[1]) for g in sel]
+            idx = np.concatenate([np.asarray(g[2], np.int64) for g in sel])
+            total, pix_off = src.layout(idx)
+            descs = crop_descriptors(self.recognizer._cfg, pix_off, np.concatenate([g[0] for g in sel]),
+                                     np.concatenate([g[1] for g in sel]), np.repeat(np.arange(end - start), sizes))
+            chunks.append({"idx": idx, "total": total, "descs": descs, "sizes": sizes})
             start = end
+        return chunks
+
+    def _run_chunks(self, chunks, src, stream=None):
+        """One packed recognizer call per planned chunk, its pixels taken from `src`.  Returns per group
+        (ids, probs, group_len)."""
+        model = self.recognizer.model
+        out = []
+        for ch in chunks:
+            canv = src.fill(ch["idx"], stream)
+            with _span("recognize.device"):
+                ids, probs, glen = model.run_packed_ptr(canv.data_ptr(), src.on_device, ch["total"], ch["descs"],
+                                                        len(ch["descs"]), len(ch["sizes"]), stream=stream)
+            del canv
+            off = 0
+            for k, m in enumerate(ch["sizes"]):
+                out.append((ids[off:off + m], probs[off:off + m], int(glen[k])))
+                off += m
         return out
 
-    def _run_groups_dev(self, groups, geoms, pages_dev, stream=None, levels=None, plan=None):
-        """Groups whose crops exist only as records: groups = (widths, padded widths, record indices into `geoms`).
-        Single rank: cut on the device and recognised without leaving HBM (`_run_groups_dev_local`).  With
-        torch.distributed the call has three phases that `stream()` runs in three different threads -
-        `_plan_groups_dist` (host: costs, balancing and descriptors over a gloo group), `_run_groups_dist_dev`
-        (device: the leaving groups are cut into one buffer ordered by destination and travel GPU-to-GPU with ONE
-        all_to_all_single over NCCL / NVLink; own and received groups are recognised) and `_finish_results` (host: ids /
-        probabilities of groups recognised elsewhere come back over a second gloo group).  No canvas touches the host
-        on any rank.  This wrapper runs the three phases back to back."""
-        import torch.distributed as dist
-        if not (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1):
-            return self._run_groups_dev_local(groups, geoms, pages_dev, stream, levels, plan)
-        lv = levels if levels is not None else np.zeros(len(geoms), np.int64)
-        dplan = plan if isinstance(plan, dict) else self._plan_groups_dist(groups, geoms, lv)
-        return self._finish_results(self._run_groups_dist_dev(groups, geoms, pages_dev, stream, lv, dplan))
+    def _plan_groups_dev(self, groups, geoms, levels=None):
+        """`_plan_chunks` for groups whose crops exist only as records; `_run_groups_dev` takes the result as `plan`."""
+        return self._plan_chunks(groups, _RecordCrops(geoms, levels))
 
-    def _plan_groups_dist(self, groups, geoms, levels):
+    def _run_groups_dev(self, groups, geoms, pages_dev, stream=None, levels=None, plan=None):
+        """`_run_groups` for groups whose crops exist only as records: groups = (widths, padded widths, record indices
+        into `geoms`), the canvases are cut on the device and never touch the host.  `plan`: `_plan_groups_dev(groups,
+        geoms, levels)` on one rank, prepared ahead of time."""
+        return self._run_groups(groups, _RecordCrops(geoms, levels, pages_dev), stream, plan)
+
+    def _run_groups(self, groups, src, stream=None, plan=None):
+        """Recognise groups whose pixels come from `src`; results come back in `groups` order.  One rank: the chunks of
+        `_plan_chunks`.  With torch.distributed the call has three phases that `stream()` runs in three different
+        threads - `_plan_groups_dist` (host: costs, balancing and layouts over a gloo group), `_run_planned` (device:
+        the leaving groups are packed into one buffer ordered by destination and travel GPU-to-GPU with ONE
+        all_to_all_single over NCCL / NVLink; own and received groups are recognised in one packed call) and
+        `_finish_results` (host: ids / probabilities of groups recognised elsewhere come back over a second gloo
+        group).  This runs the three back to back."""
+        if plan is None:
+            plan = self._plan_groups_dist(groups, src) if _multi_rank() else self._plan_chunks(groups, src)
+        return self._finish_results(self._run_planned(plan, src, stream))
+
+    def _plan_groups_dist(self, groups, src):
         """Phase 1 (host only; collectives on the "plan" gloo group): every rank learns all group costs, derives the
         same assignment, and tells the others what it will send - after this no rank needs another control message
-        before its device work."""
+        before its device work.  When nothing moves this is the single-rank chunk plan."""
         import torch.distributed as dist
         from . import parallel as par
-        from .models import plan_crop_offsets
-        cfg = self.recognizer._cfg
-        ph, pw = cfg.encoder.patch_size
-        gh = cfg.data.img_size[0] // ph
         world, rank = dist.get_world_size(), dist.get_rank()
-        costs = [gh * (int(np.sum(g[1])) // pw) + ROW_COST_TOKENS * len(g[1]) for g in groups]
+        costs = [self._group_tokens(g) + ROW_COST_TOKENS * len(g[1]) for g in groups]
         assign_all = par.balance_groups(par.all_gather_objects(costs, "plan"), world)
         if all(dst == r for r, row in enumerate(assign_all) for dst in row):
-            return {"dist": True, "moves": False, "plan": self._plan_groups_dev(groups, geoms, levels)}
+            return self._plan_chunks(groups, src)
         assign = assign_all[rank]
-        mine = [k for k in range(len(groups)) if assign[k] == rank]
+        height = self.recognizer._cfg.data.img_size[0]
+
+        def packed(ks):
+            """Crop indices of groups ks and the layout `src.pack` gives them: (idx, bytes, rows (k, w, wp, offs))."""
+            idx = np.concatenate([groups[k][2] for k in ks])
+            total, offs = src.pack_layout(idx)
+            rows, j = [], 0
+            for k in ks:
+                m = len(groups[k][1])
+                rows.append((k, np.asarray(groups[k][0], np.int64), np.asarray(groups[k][1], np.int64), offs[j:j + m]))
+                j += m
+            return idx, total, rows
+
         send, outgoing, send_splits = [], {}, [0] * world
         for dst in range(world):
             ks = [k for k in range(len(groups)) if assign[k] == dst and dst != rank]
-            if not ks:
-                continue
-            idx = np.concatenate([groups[k][2] for k in ks])
-            sel, lvs = geoms[idx].copy(), levels[idx]
-            total, offs = plan_crop_offsets(sel, lvs)
-            send.append((dst, sel, lvs, total))
-            send_splits[dst] = total
-            rows, j = [], 0
-            for k in ks:
-                m = len(groups[k][0])
-                rows.append((k, np.asarray(groups[k][0], np.int64), np.asarray(groups[k][1], np.int64), offs[j:j + m]))
-                j += m
-            outgoing[dst] = {"bytes": total, "groups": rows}
+            if ks:       # ascending destination = the order of the split sizes
+                idx, send_splits[dst], rows = packed(ks)
+                send.append((idx, send_splits[dst]))
+                outgoing[dst] = {"bytes": send_splits[dst], "groups": rows}
         everyone = par.all_gather_objects(outgoing, "plan")
-        recv_splits, foreign, work, base = [0] * world, [], [], 0
-        for src in range(world):
-            d = everyone[src].get(rank) if src != rank else None
-            if d is None:
-                continue
-            recv_splits[src] = int(d["bytes"])
-            for gid, w, wp, offs in d["groups"]:
-                foreign.append((w, wp, base + offs))
-                work.append((src, int(gid)))
-            base += int(d["bytes"])
         # ONE packed recognizer call for own + received groups: a single work buffer [own canvases | received canvases]
         # (two calls would run the 101-step decode loop twice, and its cost is mostly per step, not per row)
-        mine_total, mine_sel, mine_lv, unified, owner = 0, None, None, [], []
-        if mine:
-            idx = np.concatenate([groups[k][2] for k in mine])
-            mine_sel, mine_lv = geoms[idx].copy(), levels[idx]
-            mine_total, offs = plan_crop_offsets(mine_sel, mine_lv)
-            j = 0
-            for k in mine:
-                m = len(groups[k][0])
-                unified.append((np.asarray(groups[k][0], np.int64), np.asarray(groups[k][1], np.int64), offs[j:j + m]))
-                owner.append((rank, k))
-                j += m
-        unified += [(w, wp, mine_total + offs) for w, wp, offs in foreign]
-        owner += work
+        mine = [k for k in range(len(groups)) if assign[k] == rank]
+        mine_idx, mine_total, rows = packed(mine) if mine else (None, 0, [])
+        work = [(w, wp, offs) for _, w, wp, offs in rows]
+        owner = [(rank, k) for k in mine]
+        recv_splits, base = [0] * world, mine_total
+        for src_rank in range(world):
+            d = everyone[src_rank].get(rank) if src_rank != rank else None
+            if d is None:
+                continue
+            recv_splits[src_rank] = int(d["bytes"])
+            work += [(w, wp, base + offs) for _, w, wp, offs in d["groups"]]
+            owner += [(src_rank, int(gid)) for gid, _, _, _ in d["groups"]]
+            base += int(d["bytes"])
+        # the work buffer's canvases, numbered in group order: the groups become (widths, padded widths, indices)
+        offs = np.concatenate([g[2] for g in work]) if work else np.zeros(0, np.int64)
+        widths = np.concatenate([g[0] for g in work]) if work else np.zeros(0, np.int64)
+        starts = np.cumsum([0] + [len(g[0]) for g in work])
+        work = [(w, wp, np.arange(starts[i], starts[i + 1])) for i, (w, wp, _) in enumerate(work)]
+        work_src = _FlatCrops(None, offs, widths * (3 * height))
         # phase 3 is planned here too: a group's result is m rows of (S int32 ids, S float32 probabilities) + its int32
         # decode length, so every rank knows the byte counts of the result exchange before anything runs
         S = int(self.recognizer.model.max_label_length) + 1
         back_splits, expect_splits, expect = [0] * world, [0] * world, {}
-        for (src, _), (w, _, _) in zip(work, foreign):
-            back_splits[src] += len(w) * S * 8 + 4
+        for (src_rank, _), (w, _, _) in zip(owner, work):
+            if src_rank != rank:
+                back_splits[src_rank] += len(w) * S * 8 + 4
         for k in range(len(groups)):
             if assign[k] != rank:
-                expect.setdefault(assign[k], []).append((k, len(groups[k][0])))
-                expect_splits[assign[k]] += len(groups[k][0]) * S * 8 + 4
-        return {"dist": True, "moves": True, "mine_sel": mine_sel, "mine_lv": mine_lv, "mine_total": mine_total,
-                "send": send, "send_splits": send_splits, "recv_splits": recv_splits, "unified": unified,
-                "owner": owner, "n_groups": len(groups),
+                expect.setdefault(assign[k], []).append((k, len(groups[k][1])))
+                expect_splits[assign[k]] += len(groups[k][1]) * S * 8 + 4
+        return {"mine_idx": mine_idx, "mine_total": mine_total, "send": send, "send_splits": send_splits,
+                "recv_splits": recv_splits, "work_offs": work_src.offs, "work_bytes": work_src.nbytes,
+                "chunks": self._plan_chunks(work, work_src), "owner": owner, "n_groups": len(groups),
                 "results": {"S": S, "back_splits": back_splits, "expect_splits": expect_splits, "expect": expect}}
 
-    def _run_groups_dist_dev(self, groups, geoms, pages_dev, stream, levels, dplan):
-        """Phase 2 (device): returns a `_PendingResults` (own groups done, results of foreign groups to hand back)."""
+    def _run_planned(self, plan, src, stream=None):
+        """Phase 2 (device).  plan: a chunk list (one rank, or nothing moves) -> the group results; a
+        `_plan_groups_dist` dict -> a `_PendingResults` (own groups done, results of foreign groups to hand back)."""
+        if not isinstance(plan, dict):
+            return self._run_chunks(plan, src, stream)
+        import contextlib
+
         import torch
         import torch.distributed as dist
+        from . import models
         from . import parallel as par
-        from .models import concat_device_buffers, extract_crops_pyramid
-        pages = pages_dev if isinstance(pages_dev, dict) else {0: pages_dev}
-        if not dplan["moves"]:
-            return _PendingResults(self._run_groups_dev_local(groups, geoms, pages, stream, levels, dplan["plan"]), None,
-                                   None)
-        cfg = self.recognizer._cfg
-        rank = dist.get_rank()
-        ctx = torch.cuda.stream(stream) if stream is not None else _NullCtx()
-        with ctx:
-            parts = []
-            for dst, sel, lvs, total in dplan["send"]:      # ascending destination = the order of the split sizes
-                canv_d, total_d, _ = extract_crops_pyramid(pages, sel, lvs, stream)
-                assert total_d == total
-                parts.append((canv_d, total_d))
-            some = next(iter(pages.values()))
-            device = getattr(some[0] if isinstance(some, tuple) else some, "device", "cpu")
+        device = par._dev()
+        with torch.cuda.stream(stream) if stream is not None else contextlib.nullcontext():
+            parts = [(src.pack(idx, stream), total) for idx, total in plan["send"]]
             if parts:
-                canv = concat_device_buffers(parts, stream)
+                canv = models.concat_device_buffers(parts, stream)
                 if len(parts) == 1:
                     canv = canv[: parts[0][1]]
             else:
                 canv = torch.empty(0, dtype=torch.uint8, device=device)
-            mine_total = dplan["mine_total"]
-            work = torch.empty(mine_total + int(sum(dplan["recv_splits"])), dtype=torch.uint8, device=device)
+            mine_total = plan["mine_total"]
+            work = torch.empty(mine_total + int(sum(plan["recv_splits"])), dtype=torch.uint8, device=device)
             if mine_total:
-                own, total_m, _ = extract_crops_pyramid(pages, dplan["mine_sel"], dplan["mine_lv"], stream)
-                assert total_m == mine_total
+                own = src.pack(plan["mine_idx"], stream)
                 work[:mine_total].copy_(own[:mine_total], non_blocking=True)
                 del own
-            par.exchange_canvases_planned(canv, dplan["send_splits"], dplan["recv_splits"], out=work[mine_total:])
-        res = self._run_groups_buf(dplan["unified"], work, cfg.data.img_size[0], stream) if dplan["unified"] else []
-        out, back = [None] * dplan["n_groups"], []
-        for (src, gid), (ids, probs, glen) in zip(dplan["owner"], res):
-            if src == rank:
-                out[gid] = (ids, probs, glen)
+            par.exchange_canvases_planned(canv, plan["send_splits"], plan["recv_splits"], out=work[mine_total:])
+        res = self._run_chunks(plan["chunks"], _FlatCrops(work, plan["work_offs"], plan["work_bytes"]), stream)
+        rank = dist.get_rank()
+        out, back = [None] * plan["n_groups"], []
+        for (src_rank, gid), r in zip(plan["owner"], res):
+            if src_rank == rank:
+                out[gid] = r
             else:
-                back.append((src, gid, ids, probs, glen))
-        return _PendingResults(out, back, dplan["results"])
+                back.append((src_rank, gid) + r)
+        return _PendingResults(out, back, plan["results"])
 
     def _finish_results(self, pending):
         """Phase 3 (host; collectives on the "results" gloo group): results of the groups this rank sent away."""
         if isinstance(pending, list):
             return pending
-        if pending.back is None:
-            return pending.out
         from . import parallel as par
         rp = pending.plan
         S = rp["S"]
@@ -629,175 +665,32 @@ class BatchedOCR:
             raise RuntimeError("crop scatter: no result came back for groups %s" % missing[:8])
         return pending.out
 
-    def _run_groups_buf(self, groups, buf, height, stream=None):
-        """groups = (widths, padded widths, byte offsets into `buf`), `buf` a flat uint8 tensor on the compute device
-        (the receive buffer of the crop scatter): one packed recognizer call per <= max_tokens chunk."""
-        from . import _lib
-        rec = self.recognizer
-        cfg = rec._cfg
-        ph, pw = cfg.encoder.patch_size
-        gh = cfg.data.img_size[0] // ph
-        out = [None] * len(groups)
-        gtok = [gh * (int(np.sum(g[1])) // pw) for g in groups]
-        dt = np.dtype(_lib.YtkCrop)
-        start = 0
-        while start < len(groups):
-            end, tok = start, 0
-            while end < len(groups) and not (end > start and tok + gtok[end] > self.max_tokens):
-                tok += gtok[end]
-                end += 1
-            sel = groups[start:end]
-            w = np.concatenate([np.asarray(g[0], np.int64) for g in sel])
-            wp = np.concatenate([np.asarray(g[1], np.int64) for g in sel])
-            offs = np.concatenate([g[2] for g in sel])
-            n = w.shape[0]
-            ntok = gh * (wp // pw)
-            descs = np.zeros(n, dtype=dt)
-            descs["pix_off"] = offs
-            descs["w"] = w
-            descs["wp"] = wp
-            descs["tok_off"] = np.cumsum(ntok) - ntok
-            descs["ntok"] = ntok
-            descs["group"] = np.repeat(np.arange(end - start), [len(g[0]) for g in sel])
-            with _span("recognize.device"):
-                ids, probs, glen = rec.model.run_packed_ptr(buf.data_ptr(), 1, int(buf.numel()), descs, n, end - start,
-                                                            stream=stream)
-            off = 0
-            for k in range(start, end):
-                m = len(groups[k][0])
-                out[k] = (ids[off:off + m], probs[off:off + m], int(glen[k - start]))
-                off += m
-            start = end
-        return out
-
-    def _plan_groups_dev(self, groups, geoms, levels=None):
-        """Host-side planning of `_run_groups_dev_local` (no device call): <= max_tokens chunks ending on group
-        boundaries, with the records, padded widths and recognizer descriptors of every chunk.  `BatchedOCR.stream` runs
-        this for batch i + 1 in its own thread while batch i is on the GPU."""
-        from . import _lib
-        lv = levels if levels is not None else np.zeros(len(geoms), np.int64)
-        cfg = self.recognizer._cfg
-        ph, pw = cfg.encoder.patch_size
-        gh = cfg.data.img_size[0] // ph
-        gtok = [gh * (int(np.sum(g[1])) // pw) for g in groups]
-        dt = np.dtype(_lib.YtkCrop)
-        chunks, start = [], 0
-        while start < len(groups):
-            end, tok = start, 0
-            while end < len(groups) and not (end > start and tok + gtok[end] > self.max_tokens):
-                tok += gtok[end]
-                end += 1
-            chunk = groups[start:end]
-            idx = np.concatenate([g[2] for g in chunk])
-            wp = np.concatenate([np.asarray(g[1], np.int64) for g in chunk])
-            sel = geoms[idx].copy()
-            n = sel.shape[0]
-            ntok = gh * (wp // pw)
-            descs = np.zeros(n, dtype=dt)
-            descs["w"] = sel["canvas_w"]
-            descs["wp"] = wp
-            descs["tok_off"] = np.cumsum(ntok) - ntok
-            descs["ntok"] = ntok
-            descs["group"] = np.repeat(np.arange(end - start), [len(g[0]) for g in chunk])
-            chunks.append({"start": start, "end": end, "sel": sel, "lv": lv[idx], "descs": descs, "n": n,
-                           "sizes": [len(g[0]) for g in chunk]})
-            start = end
-        return chunks
-
-    def _run_groups_dev_local(self, groups, geoms, pages_dev, stream=None, levels=None, plan=None):
-        """This rank's share of `_run_groups_dev`: the canvases of a <= max_tokens chunk are cut on the device
-        (ytk_extract_crops_table_u8, one call per source_downscale pyramid level) in group order and go to PARSeq without
-        leaving HBM.  `plan` = `_plan_groups_dev(groups, geoms, levels)` when it was prepared ahead of time."""
-        from .models import extract_crops_pyramid
-        pages = pages_dev if isinstance(pages_dev, dict) else {0: pages_dev}
-        rec = self.recognizer
-        if plan is None:
-            plan = self._plan_groups_dev(groups, geoms, levels)
-        out = [None] * len(groups)
-        for ch in plan:
-            with _span("recognize.crops_device"):
-                canv, total, offs = extract_crops_pyramid(pages, ch["sel"], ch["lv"], stream)
-            ch["descs"]["pix_off"] = offs
-            with _span("recognize.device"):
-                ids, probs, glen = rec.model.run_packed_ptr(canv.data_ptr(), 1, total, ch["descs"], ch["n"],
-                                                            ch["end"] - ch["start"], stream=stream)
-            del canv
-            off = 0
-            for k, m in zip(range(ch["start"], ch["end"]), ch["sizes"]):
-                out[k] = (ids[off:off + m], probs[off:off + m], int(glen[k - ch["start"]]))
-                off += m
-        return out
-
-    def _run_groups(self, groups, stream=None, arena=None, height=32):
-        """Recognise groups, spreading them over all ranks when torch.distributed is initialised (crop scatter /
-        result gather over NCCL, yomitoku_b200/parallel.py); results come back in `groups` order.  Groups are
-        (canvases, padded widths) or, with `arena`, (widths, padded widths, arena offsets); only groups that leave this
-        rank are ever materialised as pixel arrays."""
-        import torch.distributed as dist
-
-        def run_mine(ks):
-            sel = [groups[k] for k in ks]
-            if arena is not None:
-                return self._run_groups_arena(sel, arena, height, stream)
-            return self._run_groups_local(sel, stream)
-
-        if not (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1):
-            return run_mine(range(len(groups)))
-
-        def pixels(ks):
-            if arena is None:
-                return [groups[k][0] for k in ks]
-            an = arena.np
-            return [[an[int(o):int(o) + height * int(w) * 3].reshape(height, int(w), 3)
-                     for w, o in zip(groups[k][0], groups[k][2])] for k in ks]
-
-        return self._run_groups_dist(groups, pixels, run_mine, stream)
-
-    def _run_groups_dist(self, groups, pixels, run_mine, stream=None):
-        """The multi-rank part of `_run_groups` / `_run_groups_dev`.  groups[k][1] = padded widths (the cost);
-        pixels(ks) -> canvases (host arrays) of the groups ks that leave this rank; run_mine(ks) -> results of the
-        groups ks that stay.  Balances whole groups across ranks, scatters the leaving ones, recognises own + received
-        groups, returns every group's (ids, probs, group_len) to its owner."""
-        import torch.distributed as dist
-        from . import parallel as par
-        cfg = self.recognizer._cfg
-        ph, pw = cfg.encoder.patch_size
-        gh = cfg.data.img_size[0] // ph
-        rank = dist.get_rank()
-        costs = [gh * (int(np.sum(g[1])) // pw) + ROW_COST_TOKENS * len(g[1]) for g in groups]
-        assign_all = par.balance_groups(par.gather_costs(costs), dist.get_world_size())
-        if all(dst == r for r, row in enumerate(assign_all) for dst in row):
-            # balanced already (every rank computes the same table from the same gathered costs): nothing moves, so
-            # the two all_to_all rounds of the scatter / gather are skipped on all ranks alike
-            return list(run_mine(range(len(groups))))
-        assign = assign_all[rank]
-        leaving = [k for k in range(len(groups)) if assign[k] != rank]
-        mine = [k for k in range(len(groups)) if assign[k] == rank]        # exchange_groups lists own groups first
-        pix = dict(zip(leaving, pixels(leaving))) if leaving else {}
-        send = [(pix.get(k), g[1]) for k, g in enumerate(groups)]
-        work = par.exchange_groups(send, assign, cfg.data.img_size[0])
-        res = list(run_mine(mine)) if mine else []
-        foreign = work[len(mine):]
-        if foreign:
-            res = res + self._run_groups_local([(w[2], w[3]) for w in foreign], stream)
-        S = cfg.max_label_length + 1
-        # group_len travels as an extra column pair so that refine_iters == 0 keeps working across ranks
-        packed = []
-        for (ids, probs, glen) in res:
-            packed.append((np.concatenate([ids, np.full((ids.shape[0], 1), glen, np.int32)], axis=1),
-                           np.concatenate([probs, np.zeros((probs.shape[0], 1), np.float32)], axis=1)))
-        back = par.return_results(work, packed, len(groups), S + 1)
-        return [(i[:, :S], p[:, :S], int(i[0, S]) if len(i) else 0) for i, p in back]
+    def _crop_source(self, per_page, arena, pages_dev):
+        """The pixel source of a batch's crops: records cut on the device, the arena the workers wrote, or - for host
+        canvas lists (no worker pool, or a page whose arena slice spilled) - one page-locked buffer packed here."""
+        pages = [p[0] for p in per_page]
+        if pages_dev is not None and all(isinstance(p, _PageGeoms) for p in pages):
+            if not pages:
+                return _RecordCrops(np.zeros(0, CROP_GEOM_DTYPE), None, pages_dev)
+            return _RecordCrops(np.concatenate([p.geoms for p in pages]), np.concatenate([p.levels for p in pages]),
+                                pages_dev)
+        height = self.recognizer._cfg.data.img_size[0]
+        if arena is not None and all(isinstance(p, _PageCrops) for p in pages):
+            widths = np.asarray([w for p in pages for w in p.widths], np.int64)
+            offs = np.concatenate([p.offs for p in pages]) if pages else np.zeros(0, np.int64)
+            return _FlatCrops(arena.torch, offs, widths * (3 * height))
+        from .models import pack_canvases
+        canvases = [c for p in pages for c in p]
+        buf, _, offs = pack_canvases(canvases)
+        return _FlatCrops(buf, offs, [c.size for c in canvases])
 
     def prepare_pooled(self, per_page, arena=None, pages_dev=None):
         """Host-only half of `recognize_pooled`: the reference grouping of every page (bucketing order, mini-batch plan,
-        padded widths) flattened into the group list of the batch, plus - for device-cut crops on a single rank - the
-        chunk plan of the packed recognizer call.  No device call, so it can run ahead of the GPU."""
+        padded widths) flattened into the group list of the batch, the batch's pixel source and the plan of its packed
+        recognizer calls (over all ranks with torch.distributed).  No device call, so it can run ahead of the GPU."""
         rec = self.recognizer
         cfg = rec._cfg
-        in_arena = arena is not None and all(isinstance(p[0], _PageCrops) for p in per_page)
-        in_dev = pages_dev is not None and all(isinstance(p[0], _PageGeoms) for p in per_page)
-        groups, owner, orders = [], [], []
+        groups, owner, orders, base = [], [], [], 0
         for pi, (canv, cw, n_quads) in enumerate(per_page):
             order = None
             if rec.batch_bucketing and len(canv) == n_quads and len(canv) > 1:
@@ -808,64 +701,42 @@ class BatchedOCR:
                                      getattr(cfg.data, "max_batch_size", None))
             padded, _ = rec._collate_widths(widths, plan)
             for b in plan:
-                if in_dev:     # (widths, padded widths, record indices): the pixels are cut on the device
-                    groups.append(([widths[i] for i in b], [padded[i] for i in b], canv.base + np.asarray(b, np.int64)))
-                elif in_arena:   # (widths, padded widths, arena offsets): no pixel is touched on the host
-                    groups.append(([widths[i] for i in b], [padded[i] for i in b], canv.offs[b]))
-                else:
-                    groups.append(([canv[i] for i in b], [padded[i] for i in b]))
+                groups.append(([widths[i] for i in b], [padded[i] for i in b], base + np.asarray(b, np.int64)))
                 owner.append(pi)
             orders.append(order)
-        prep = {"groups": groups, "owner": owner, "orders": orders, "in_dev": in_dev, "in_arena": in_arena,
-                "n_pages": len(per_page), "height": per_page[0][0].height if in_arena and per_page else 32}
-        if in_dev:
-            prep["geoms"] = np.concatenate([p[0].geoms for p in per_page]) if per_page else np.zeros(0, CROP_GEOM_DTYPE)
-            prep["levels"] = np.concatenate([p[0].levels for p in per_page]) if per_page else np.zeros(0, np.int64)
-            import torch.distributed as dist
-            if not (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1):
-                prep["plan"] = self._plan_groups_dev(groups, prep["geoms"], prep["levels"])
-            else:       # costs / balancing / descriptors now, in this (planner) thread, over the host-side group
-                prep["plan"] = self._plan_groups_dist(groups, prep["geoms"], prep["levels"])
-        return prep
+            base += len(widths)
+        src = self._crop_source(per_page, arena, pages_dev)
+        plan = self._plan_groups_dist(groups, src) if _multi_rank() else self._plan_chunks(groups, src)
+        return {"groups": groups, "owner": owner, "orders": orders, "n_pages": len(per_page), "src": src,
+                "plan": plan}
 
     def run_prepared(self, prep, stream=None, arena=None, pages_dev=None, finish=True):
-        """Device half of `recognize_pooled`.  finish=True: returns per page (ids, probs, order) with rows in the page's
-        *plan* order, exactly like TextRecognizer._run_plan.  finish=False (`stream()` with several ranks): returns the
-        raw group results, possibly pending on other ranks - `finish_prepared` completes them in another thread."""
-        groups = prep["groups"]
-        if prep["in_dev"]:
-            plan = prep.get("plan")
-            if isinstance(plan, dict):
-                lv = prep["levels"]
-                raw = self._run_groups_dist_dev(groups, prep["geoms"], pages_dev, stream, lv, plan)
-            else:
-                raw = self._run_groups_dev(groups, prep["geoms"], pages_dev, stream, prep["levels"], plan)
-        else:
-            raw = self._run_groups(groups, stream, arena if prep["in_arena"] else None, prep["height"])
+        """Device half of `recognize_pooled` (`arena` / `pages_dev`: those given to `prepare_pooled`, whose source
+        holds them).  finish=True: returns per page (ids, probs, order) with rows in the page's *plan* order, exactly
+        like TextRecognizer._run_plan.  finish=False (`stream()` with several ranks): returns the raw group results,
+        possibly pending on other ranks - `finish_prepared` completes them in another thread."""
+        raw = self._run_planned(prep["plan"], prep["src"], stream)
         return self.finish_prepared(prep, raw) if finish else raw
 
     def finish_prepared(self, prep, raw):
+        pages = self._gather_pages(self._finish_results(raw), prep["owner"], prep["n_pages"])
+        return [(ids, probs, order) for (ids, probs), order in zip(pages, prep["orders"])]
+
+    def _gather_pages(self, res, owner, n_pages):
+        """Group results + the page of every group -> per page (ids, probs), rows in plan order, the positions a
+        `refine_iters == 0` model never produced filled like the host path does."""
         rec = self.recognizer
-        cfg = rec._cfg
-        res = self._finish_results(raw)
-        owner, orders = prep["owner"], prep["orders"]
-        S = cfg.max_label_length + 1
+        S = rec._cfg.max_label_length + 1
         out = []
-        for pi in range(prep["n_pages"]):
+        for pi in range(n_pages):
             mine = [r for r, o in zip(res, owner) if o == pi]
             if not mine:
-                out.append((np.zeros((0, S), np.int32), np.zeros((0, S), np.float32), orders[pi]))
+                out.append((np.zeros((0, S), np.int32), np.zeros((0, S), np.float32)))
                 continue
-            ids = np.concatenate([m[0] for m in mine]).copy()
-            probs = np.concatenate([m[1] for m in mine]).copy()
-            if rec.model.refine_iters == 0:
-                k = 0
-                for m in mine:
-                    n = m[0].shape[0]
-                    ids[k:k + n, m[2]:] = rec.tokenizer.eos_id
-                    probs[k:k + n, m[2]:] = 1.0
-                    k += n
-            out.append((ids, probs, orders[pi]))
+            ids = np.concatenate([m[0] for m in mine])
+            probs = np.concatenate([m[1] for m in mine])
+            rec._eos_tail(ids, probs, np.repeat([m[2] for m in mine], [len(m[0]) for m in mine]))
+            out.append((ids, probs))
         return out
 
     def recognize_pooled(self, per_page, stream=None, arena=None, pages_dev=None):
@@ -1039,7 +910,7 @@ class BatchedOCR:
             for i, h in enumerate(host):
                 ref = h[2]
                 if isinstance(ref, _ArenaRef):
-                    crops = _PageCrops(an, i * handle.cap, ref)
+                    crops = _PageCrops(an, i * handle.cap, ref.widths, self.recognizer._cfg.data.img_size[0])
                     if ref.spill:       # arena slice too small for this page: generic path now, larger slices next time
                         crops = [crops[k] for k in range(len(crops))] + list(ref.spill)
                         self.crop_cap = max(self.crop_cap, 2 * handle.cap)
@@ -1109,27 +980,17 @@ class BatchedOCR:
                 owner.append(pi)
             base += len(retry)
         if not groups:
-            import torch.distributed as dist
-            if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+            if _multi_rank():
                 # the balancing round is a collective: a rank without retries still takes part in it
                 self._run_groups_dev([], np.zeros(0, CROP_GEOM_DTYPE), pages_dev, stream, np.zeros(0, np.int64))
             return
         res = self._run_groups_dev(groups, np.concatenate(geoms2), pages_dev, stream, np.concatenate(levels2))
         S = cfg.max_label_length + 1
-        for pi, (ids, probs, order) in enumerate(rec_out):
-            mine = [r for r, o in zip(res, owner) if o == pi]
-            if not mine:
+        second = self._gather_pages(res, owner, len(rec_out))
+        for (ids, probs, _), (r_ids, r_probs), (retry, pos, scores) in zip(rec_out, second, retries):
+            if not len(r_ids):
                 continue
-            r_ids = np.concatenate([m[0] for m in mine]).copy()
-            r_probs = np.concatenate([m[1] for m in mine]).copy()
-            if rec.model.refine_iters == 0:
-                k = 0
-                for m in mine:
-                    r_ids[k:k + m[0].shape[0], m[2]:] = rec.tokenizer.eos_id
-                    r_probs[k:k + m[0].shape[0], m[2]:] = 1.0
-                    k += m[0].shape[0]
             _, r_scores = rec.tokenizer.decode_ids(r_ids, r_probs)
-            retry, pos, scores = retries[pi]
             for j, i in enumerate(retry):
                 k = int(pos[i])
                 if r_scores[j] > scores[k] and r_scores[j] >= thresh:
@@ -1142,15 +1003,8 @@ class BatchedOCR:
         _t.__enter__()
         r = self.recognizer
         from .schemas import WordPrediction
-        for (quads, scores, canv, cw, n, *_), (ids, probs, order) in zip(host, rec_out):
-            if n == 0:
-                p, s, d = [], [], []
-            else:
-                pts = [quads[i] for i in order] if order is not None else quads
-                p, s, d = r.postprocess_ids(ids, probs, pts[:n])
-                if order is not None:
-                    inv = np.argsort(order)
-                    p, s, d = [p[i] for i in inv], [s[i] for i in inv], [d[i] for i in inv]
+        for (quads, scores, *_), (ids, probs, order) in zip(host, rec_out):
+            p, s, d = r._decode_in_order(ids, probs, quads, order)
             # same pairing as ocr_aggregate (reference ocr.py:6-24); the values are produced by this module with
             # the right types, so the pydantic models are built without re-validating every coordinate
             words = [_fast_word(WordPrediction, q, c, dd, float(ds), float(rs))
@@ -1292,22 +1146,6 @@ class _Handle:
         self.done = threading.Event()       # set once the batch has been recognised (or abandoned)
 
 
-class _HostCanvases:
-    """Device-cut canvases brought to the host (page-locked) for the cross-rank exchange; quacks like the crop arena."""
-
-    def __init__(self, canv_dev, stream=None):
-        import torch
-        self.torch = torch.empty(canv_dev.shape, dtype=torch.uint8, pin_memory=True)
-        if stream is not None:
-            with torch.cuda.stream(stream):
-                self.torch.copy_(canv_dev, non_blocking=True)
-            stream.synchronize()
-        else:
-            self.torch.copy_(canv_dev)
-            torch.cuda.current_stream().synchronize()
-        self.np = self.torch.numpy()
-
-
 _WORD_FIELDS = frozenset(("points", "content", "direction", "rec_score", "det_score"))
 
 
@@ -1329,14 +1167,6 @@ class _PendingResults:
 
     def __init__(self, out, back, plan):
         self.out, self.back, self.plan = out, back, plan
-
-
-class _NullCtx:
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *a):
-        return False
 
 
 class _Done:

@@ -149,15 +149,32 @@ class TextRecognizer(BaseModule):
         """All mini-batches of `plan` in one packed device call; returns (ids, probs) in `canvases` order."""
         flat = [i for b in plan for i in b]
         padded, group = self._collate_widths(canvases, plan)
+        group = np.asarray([group[i] for i in flat], np.int64)
         ids, probs, glen = self.model.recognize_crops([canvases[i] for i in flat], [padded[i] for i in flat],
-                                                      [group[i] for i in flat], len(plan))
-        if self.model.refine_iters == 0:
-            # the reference's output then has only `steps run` positions per mini-batch: cut what follows
-            for k, i in enumerate(flat):
-                L = int(glen[group[i]])
-                ids[k, L:] = self.tokenizer.eos_id
-                probs[k, L:] = 1.0
+                                                      group.tolist(), len(plan))
+        self._eos_tail(ids, probs, glen[group])
         return flat, ids, probs
+
+    def _eos_tail(self, ids, probs, lens):
+        """With refine_iters == 0 the reference's output has only the positions its mini-batch's AR loop ran: row r
+        keeps lens[r] positions, the rest reads as EOS with probability 1.  In place."""
+        if self.model.refine_iters == 0:
+            cut = np.arange(ids.shape[1])[None, :] >= np.asarray(lens, np.int64)[:, None]
+            ids[cut] = self.tokenizer.eos_id
+            probs[cut] = 1.0
+
+    def _decode_in_order(self, ids, probs, points, order):
+        """Rows of (ids, probs) in plan order -> (texts, scores, directions) in detection order.  order: the bucketing
+        order the plan followed (None: detection order).  The reference pairs the rows with the points in plan order
+        (:271-283, 364-373); with dropped quads `points` is longer than the rows, exactly as there."""
+        if not len(ids):
+            return [], [], []
+        pts = [points[i] for i in order] if order is not None else points
+        p, s, d = self.postprocess_ids(ids, probs, pts[:len(ids)])
+        if order is not None:
+            inverse = np.argsort(order)
+            p, s, d = [p[i] for i in inverse], [s[i] for i in inverse], [d[i] for i in inverse]
+        return p, s, d
 
     def postprocess_ids(self, ids, probs, points):
         pred, score = self.tokenizer.decode_ids(ids, probs)
@@ -207,23 +224,11 @@ class TextRecognizer(BaseModule):
         pages[k] = the page at pyramid level k (models.extract_crops_pyramid), levels[r] = level of record r; padded[r] / group[r] =
         padded width and mini-batch index of record r.  Returns (ids, probs) with the positions a `refine_iters == 0`
         model never produced filled like the host path does."""
-        from . import _lib, models
-        n = len(sel)
-        canv, base, pix_off = models.extract_crops_pyramid(pages, sel, levels)
-        ph, pw = self._cfg.encoder.patch_size
-        gh = self._cfg.data.img_size[0] // ph
-        wp = np.asarray(padded, np.int64)
-        ntok = gh * (wp // pw)
-        descs = np.zeros(n, dtype=np.dtype(_lib.YtkCrop))
-        descs["pix_off"], descs["w"], descs["wp"] = pix_off, sel["canvas_w"], wp
-        descs["tok_off"], descs["ntok"] = np.cumsum(ntok) - ntok, ntok
-        descs["group"] = group
-        ids, probs, glen = self.model.run_packed_ptr(canv.data_ptr(), 1, base, descs, n, n_groups)
-        if self.model.refine_iters == 0:
-            for k in range(n):
-                L = int(glen[group[k]])
-                ids[k, L:] = self.tokenizer.eos_id
-                probs[k, L:] = 1.0
+        from . import models
+        canv, total, pix_off = models.extract_crops_pyramid(pages, sel, levels)
+        descs = models.crop_descriptors(self._cfg, pix_off, sel["canvas_w"], padded, group)
+        ids, probs, glen = self.model.run_packed_ptr(canv.data_ptr(), 1, total, descs, len(sel), n_groups)
+        self._eos_tail(ids, probs, glen[np.asarray(group, np.int64)])
         return ids, probs
 
     def _device_records(self, img, points, dp=None):
@@ -260,11 +265,7 @@ class TextRecognizer(BaseModule):
         padded, group = self._collate_widths(widths, plan)
         ids, probs = self._run_records(pages, geoms[flat].copy(), levels[flat], [padded[i] for i in flat],
                                        [group[i] for i in flat], len(plan))
-        pts = [points[i] for i in order] if order is not None else points
-        p, s, d = self.postprocess_ids(ids, probs, pts[:n])
-        if order is not None:
-            inverse = np.argsort(order)
-            p, s, d = [p[i] for i in inverse], [s[i] for i in inverse], [d[i] for i in inverse]
+        p, s, d = self._decode_in_order(ids, probs, points, order)
         if self.rec_orientation_fallback:
             self._device_orientation_fallback(pages, geoms, levels, points, p, s, d)
         return TextRecognizerSchema(contents=p, scores=s, points=points, directions=d)
@@ -312,18 +313,8 @@ class TextRecognizer(BaseModule):
         if n == 0:
             preds, scores, directions = [], [], []
         else:
-            # the reference pairs batch k's results with points[offset:offset+len] of the (possibly sorted) point
-            # list (:271-283, 364-373); with dropped quads `points` is longer than the dataset, exactly as there
-            pts = [points[i] for i in order] if order is not None else points
-            flat, ids, probs = self._run_plan(dataset.data, plan)
-            p, s, d = self.postprocess_ids(ids, probs, pts[: len(flat)])
-            if order is not None:
-                inverse = np.argsort(order)
-                preds = [p[i] for i in inverse]
-                scores = [s[i] for i in inverse]
-                directions = [d[i] for i in inverse]
-            else:
-                preds, scores, directions = p, s, d
+            _, ids, probs = self._run_plan(dataset.data, plan)
+            preds, scores, directions = self._decode_in_order(ids, probs, points, order)
         if self.rec_orientation_fallback and n:
             self._apply_orientation_fallback(dataset, points, preds, scores, directions)
         results = TextRecognizerSchema(contents=preds, scores=scores, points=points, directions=directions)
