@@ -197,8 +197,10 @@ int ytk_dbnet_forward_f32(ytk_dbnet* h, const float* x_nchw, int x_on_device, in
                           int out_on_device, void* cuda_stream);
 /* algorithmic conv FLOPs (2*MAC) of one forward at this shape (roofline accounting) */
 double ytk_dbnet_flops(ytk_dbnet* h, int n_pages, int Hn, int Wn);
-/* test hook: copy a named intermediate activation (NHWC) of the last run at this shape to host fp32.
- * shape4 receives n,h,w,c.  Names: stem, pool, layer1..layer4, layerL.B, f1..f4, fuse, asf_a, bin1, bin2, prob. */
+/* test hook: copy a named intermediate activation (NHWC) of the last run at this shape to host fp32 (16-bit operands
+ * converted).  shape4 receives n,h,w,c; host_out null: shape only.  The shape must have run: a shape with no engine
+ * (never run, or evicted from the engine cache) is an error, as is an unknown name.
+ * Names: stem, pool, layer1..layer4, layerL.B, f1..f4, fuse, asf_a, bin1, bin2, prob. */
 int ytk_dbnet_debug_tensor(ytk_dbnet* h, int n_pages, int Hn, int Wn, const char* name, float* host_out,
                            long long capacity, int* shape4);
 

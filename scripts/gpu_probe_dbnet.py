@@ -13,6 +13,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from oracle import dbnet as odb  # noqa: E402
 from oracle import weights  # noqa: E402
 from yomitoku_b200 import _lib  # noqa: E402
+from yomitoku_b200.models import DBNet  # noqa: E402
 
 L = _lib.lib()
 out = []
@@ -21,17 +22,6 @@ out = []
 def log(**kw):
     out.append(kw)
     print(json.dumps(kw), flush=True)
-
-
-def debug(h, n, H, W, name):
-    shape = (ctypes.c_int * 4)()
-    cap = n * H * W * 64 + 16
-    buf = torch.empty(cap, dtype=torch.float32)
-    st = L.ytk_dbnet_debug_tensor(h, n, H, W, name.encode(), buf.data_ptr(), cap, shape)
-    if st != 0:
-        raise RuntimeError(L.ytk_last_error().decode())
-    n_, h_, w_, c_ = list(shape)
-    return buf[: n_ * h_ * w_ * c_].reshape(n_, h_, w_, c_)
 
 
 def cmp(name, got, ref):
@@ -44,12 +34,8 @@ def cmp(name, got, ref):
 def main():
     torch.manual_seed(0)
     sd = weights.make_dbnet_state_dict(seed=1)
-    tab, keep = _lib.tensor_table(sd)
-    h = ctypes.c_void_p()
-    st = L.ytk_dbnet_create(tab, len(tab), 1280, 1600, ctypes.byref(h))
-    if st != 0:
-        log(fatal=L.ytk_last_error().decode())
-        return
+    model = DBNet().load_state_dict(sd)     # shortest 1280, limit 1600
+    h = model._ensure()
     # ---------------- model-level seam on a small input, with intermediates
     H, W = 256, 384
     x = torch.randn(1, 3, H, W)
@@ -63,11 +49,11 @@ def main():
     with torch.inference_mode():
         p = "backbone.body."
         s = F.relu(odb._bn(sd, p + "bn1", F.conv2d(x, sd[p + "conv1.weight"], stride=2, padding=3)))
-        cmp("stem", debug(h, 1, H, W, "stem"), s.permute(0, 2, 3, 1))
-        cmp("pool", debug(h, 1, H, W, "pool"), F.max_pool2d(s, 3, 2, 1).permute(0, 2, 3, 1))
+        cmp("stem", model.debug_tensor(1, H, W, "stem"), s.permute(0, 2, 3, 1))
+        cmp("pool", model.debug_tensor(1, H, W, "pool"), F.max_pool2d(s, 3, 2, 1).permute(0, 2, 3, 1))
         feats = odb.backbone_features(sd, x)
         for k in ("layer1", "layer2", "layer3", "layer4"):
-            cmp(k, debug(h, 1, H, W, k), feats[k].permute(0, 2, 3, 1))
+            cmp(k, model.debug_tensor(1, H, W, k), feats[k].permute(0, 2, 3, 1))
         ref = odb.decoder_forward(sd, feats)
     cmp("prob small", prob, ref[:, 0])
     # ---------------- full-size page through the fused u8 path
@@ -115,7 +101,7 @@ def main():
         ms = e0.elapsed_time(e1) / iters
         fl = L.ytk_dbnet_flops(h, n, Hn, Wn)
         log(name="time dbnet n=%d" % n, ms=ms, pages_per_s=n / ms * 1e3, gflop=fl / 1e9, tflops=fl / ms / 1e9)
-    L.ytk_dbnet_destroy(h)
+    model._release()
 
 
 if __name__ == "__main__":

@@ -11,7 +11,6 @@ head of an untrained net amplifies noise, trained weights are smoother):
                      IoU >= 0.5 (nothing lost / merged / split), box counts within 3 %;
                      (b) random head: the device's actual error field superimposed on a realistic probability map,
                      every box is found again with IoU >= 0.9 and corner coordinates within 2 px."""
-import ctypes
 import os
 
 import numpy as np
@@ -22,7 +21,7 @@ import torch.nn.functional as F
 from oracle import dbnet as odb
 from oracle import pipeline as opipe
 from oracle import weights
-from yomitoku_b200 import TextDetector, _lib
+from yomitoku_b200 import TextDetector
 from yomitoku_b200.postprocessor import DBnetPostProcessor
 from yomitoku_b200.synth import synthetic_page, synthetic_prob_map
 
@@ -35,16 +34,6 @@ def det():
     d = TextDetector(from_pretrained=False, device="cuda")
     d.model.load_state_dict(weights.make_dbnet_state_dict(seed=1))
     return d
-
-
-def _debug(model, n, H, W, name):
-    L = _lib.lib()
-    shape = (ctypes.c_int * 4)()
-    cap = n * H * W * 64 + 16
-    buf = torch.empty(cap, dtype=torch.float32)
-    _lib.check(L.ytk_dbnet_debug_tensor(model._ensure(), n, H, W, name.encode(), buf.data_ptr(), cap, shape))
-    n_, h_, w_, c_ = list(shape)
-    return buf[: n_ * h_ * w_ * c_].reshape(n_, h_, w_, c_)
 
 
 def _prob_close(got, ref):
@@ -72,7 +61,7 @@ def test_backbone_and_prob_vs_oracle(det):
         feats = odb.backbone_features(sd, x)
         ref = odb.decoder_forward(sd, feats)
     for k in ("layer1", "layer2", "layer3", "layer4"):
-        got = _debug(det.model, 2, H, W, k)
+        got = det.model.debug_tensor(2, H, W, k)
         r = feats[k].permute(0, 2, 3, 1)
         print("[dbnet] %s rel Frobenius %.5f" % (k, ((got - r).norm() / r.norm()).item()))
         assert ((got - r).norm() / r.norm()).item() < 0.015, k

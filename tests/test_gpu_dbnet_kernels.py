@@ -504,16 +504,6 @@ def test_head_vs_float64(H, W, n):
 
 
 # ======================================================================================================== engine wiring
-def _debug(model, n, H, W, name):
-    L = _lib.lib()
-    shape = (ctypes.c_int * 4)()
-    cap = n * H * W * 64 + 16
-    buf = torch.empty(cap, dtype=torch.float32)
-    _lib.check(L.ytk_dbnet_debug_tensor(model._ensure(), n, H, W, name.encode(), buf.data_ptr(), cap, shape))
-    n_, h_, w_, c_ = list(shape)
-    return buf[: n_ * h_ * w_ * c_].reshape(n_, h_, w_, c_)
-
-
 def test_engine_passes_the_op_arguments():
     """The engine's max-pool and channel-mean map at 1184 x 1600, n = 2, against the same checks on its own
     intermediates: the arguments it passes are the ones the op-level cases cover."""
@@ -524,12 +514,12 @@ def test_engine_passes_the_op_arguments():
     H, W = 1184, 1600
     x = torch.randn(2, 3, H, W, generator=torch.Generator().manual_seed(5))
     d.model(x)
-    stem = _debug(d.model, 2, H, W, "stem").to(DEV)
-    pool = _debug(d.model, 2, H, W, "pool").to(DEV)
+    stem = d.model.debug_tensor(2, H, W, "stem").to(DEV)
+    pool = d.model.debug_tensor(2, H, W, "pool").to(DEV)
     want = F.max_pool2d(stem.permute(0, 3, 1, 2), 3, 2, 1).permute(0, 2, 3, 1)
     assert torch.equal(pool, want)
-    a = _debug(d.model, 2, H, W, "asf_a").to(DEV)
-    m = _debug(d.model, 2, H, W, "asf_m")[..., 0].to(DEV).double()
+    a = d.model.debug_tensor(2, H, W, "asf_a").to(DEV)
+    m = d.model.debug_tensor(2, H, W, "asf_m")[..., 0].to(DEV).double()
     e = "decoder.concat_attention.enhanced_attention."
     wt = dict(w1=sd[e + "channel_wise.1.weight"].reshape(16, 64), w2=sd[e + "channel_wise.3.weight"].reshape(64, 16),
               sp3=sd[e + "spatial_wise.0.weight"].reshape(9), sp1=float(sd[e + "spatial_wise.2.weight"].reshape(-1)[0]),

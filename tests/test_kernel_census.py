@@ -68,7 +68,6 @@ CENSUS = {
     "asf_gate_kernel": [DBK + "test_asf_vs_float64"],
     "asf_cmean_kernel": [DBK + "test_asf_vs_float64"],
     "asf_apply_kernel": [DBK + "test_asf_vs_float64"],
-    "op_to_f32_kernel": [DBK + "test_engine_passes_the_op_arguments"],
     # dbpost_ops.cu
     "label_seed_kernel": ["tests/test_gpu_dbpost.py::test_runs_equal_scipy_twin"],
     "label_merge_kernel": ["tests/test_gpu_dbpost.py::test_runs_equal_scipy_twin"],
@@ -93,7 +92,6 @@ REASON = {
     "refine_seqs_kernel": "integer descriptors of the refinement attention: a wrong one changes the refined logits",
     "fill_i32_kernel": "an integer fill of the AR state: the repetition and refine-off paths depend on it",
     "pack_nchw_kernel": "the layout of the f32 model seam: the reference fixture through that seam compares its output",
-    "op_to_f32_kernel": "the exact fp16 -> fp32 conversion of DBNet's debug download, behind its in-situ comparisons",
     "label_seed_kernel": "one stage of the connected-component labelling, compared as a whole against a scipy twin",
     "label_merge_kernel": "one stage of the connected-component labelling, compared as a whole against a scipy twin",
     "page_stats_kernel": "one stage of the connected-component labelling, compared as a whole against a scipy twin",

@@ -590,8 +590,18 @@ def test_patchify_f32_refusals(lib, kwargs, fragment):
 
 
 def test_rtdetr_debug_hooks_refuse_null_arguments(lib):
+    """The debug hooks of all three handles (RT-DETRv2, DBNet, PARSeq) refuse a null handle, name or shape4."""
     shape = (ctypes.c_int * 4)()
     _refused(lib, lib.ytk_rtdetr_set_debug(None, 1), b"ytk_rtdetr_set_debug: null handle")
     _refused(lib, lib.ytk_rtdetr_debug_tensor(None, 1, b"c3", None, 0, shape), b"ytk_rtdetr_debug_tensor: null argument")
     _refused(lib, lib.ytk_rtdetr_debug_tensor(P, 1, None, None, 0, shape), b"ytk_rtdetr_debug_tensor: null argument")
     _refused(lib, lib.ytk_rtdetr_debug_tensor(P, 1, b"c3", None, 0, None), b"ytk_rtdetr_debug_tensor: null argument")
+    dbnet = b"ytk_dbnet_debug_tensor: null argument"
+    _refused(lib, lib.ytk_dbnet_debug_tensor(None, 1, 32, 32, b"stem", None, 0, shape), dbnet)
+    _refused(lib, lib.ytk_dbnet_debug_tensor(P, 1, 32, 32, None, None, 0, shape), dbnet)
+    _refused(lib, lib.ytk_dbnet_debug_tensor(P, 1, 32, 32, b"stem", None, 0, None), dbnet)
+    _refused(lib, lib.ytk_parseq_set_debug(None, 1), b"ytk_parseq_set_debug: null handle")
+    parseq = b"ytk_parseq_debug_tensor: null argument"
+    _refused(lib, lib.ytk_parseq_debug_tensor(None, b"enc.mem", None, 0, shape), parseq)
+    _refused(lib, lib.ytk_parseq_debug_tensor(P, None, None, 0, shape), parseq)
+    _refused(lib, lib.ytk_parseq_debug_tensor(P, b"enc.mem", None, 0, None), parseq)

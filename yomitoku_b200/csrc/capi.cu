@@ -5,11 +5,12 @@
 #include <cuda_fp16.h>
 
 #include <algorithm>
+#include <array>
 #include <climits>
 #include <cmath>
 #include <cstddef>
 #include <cstdlib>
-#include <cstring>
+#include <initializer_list>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -43,86 +44,263 @@ struct DevGuard {
     DevGuard& operator=(const DevGuard&) = delete;
 };
 
-struct ytk_parseq {
-    ytk::ParseqModel model;
-    ytk::ParseqEngine engine;
-    std::mutex mu;
-    int device = 0;  // the device current at create(); every later call binds the calling thread to it
-};
-
-struct ytk_dbnet {
-    ytk::DbnetModel model;
-    // launch plans + activation buffers per input shape (n, Hn, Wn); least recently used ones are dropped beyond
-    // max_engines (YTK_DBNET_MAX_ENGINES, default 6) so that a stream of differently sized pages cannot exhaust HBM
-    std::map<std::tuple<int, int, int>, std::unique_ptr<ytk::DbnetEngine>> engines;
-    std::map<std::tuple<int, int, int>, unsigned long long> last_use;
-    unsigned long long tick = 0;
-    int max_engines = 6;
+// What every model handle holds: the lock that serialises calls on it and the device current at create(), which every
+// later call binds the calling thread to.
+struct Handle {
     std::mutex mu;
     int device = 0;
-    int shortest = 1280, limit = 1600;
-    void* stage = nullptr;  // device staging for host inputs
-    size_t stage_bytes = 0;
-    // The staging buffer and an engine's input / activation / probability buffers are shared by all calls on this
-    // handle.  A call that leaves its output on the device returns while its kernels are still queued, so every call
-    // first makes its stream wait for the previous call's last operation (recorded here), whatever stream that was on.
-    cudaEvent_t last_done = nullptr;
+    Handle() { cudaGetDevice(&device); }
 };
 
-static void order_after_previous(ytk_dbnet* h, cudaStream_t st) {
-    if (h->last_done) cudaStreamWaitEvent(st, h->last_done, 0);
-}
-static void mark_done(ytk_dbnet* h, cudaStream_t st) {
-    if (!h->last_done) cudaEventCreateWithFlags(&h->last_done, cudaEventDisableTiming);
-    if (h->last_done) cudaEventRecord(h->last_done, st);
-}
+// One call on a handle: holds its lock and binds the calling thread to its device for the call's duration.
+struct HandleCall {
+    std::lock_guard<std::mutex> lock;
+    DevGuard dev;
+    explicit HandleCall(Handle* h) : lock(h->mu), dev(h->device) {}
+};
 
-static ytk::DbnetEngine* get_engine(ytk_dbnet* h, int n, int Hn, int Wn) {
-    auto key = std::make_tuple(n, Hn, Wn);
-    h->last_use[key] = ++h->tick;
-    auto it = h->engines.find(key);
-    if (it != h->engines.end()) return it->second.get();
-    while ((int)h->engines.size() >= h->max_engines && !h->engines.empty()) {
-        auto victim = h->engines.begin();
-        for (auto e = h->engines.begin(); e != h->engines.end(); ++e)
-            if (h->last_use[e->first] < h->last_use[victim->first]) victim = e;
-        cudaDeviceSynchronize();  // its last run may still be in flight on some stream
-        h->last_use.erase(victim->first);
-        h->engines.erase(victim);
+// A device buffer a handle owns and grows on demand (OrderedHandle::reserve).
+struct DevBuf {
+    uint8_t* p = nullptr;
+    size_t cap = 0;
+    ~DevBuf() {
+        if (p) cudaFree(p);
     }
-    auto e = std::make_unique<ytk::DbnetEngine>();
-    if (e->build(h->model, n, Hn, Wn)) return nullptr;
-    ytk::DbnetEngine* p = e.get();
-    h->engines[key] = std::move(e);
-    return p;
-}
+};
 
-static int ensure_stage(ytk_dbnet* h, size_t bytes) {
-    if (h->stage_bytes >= bytes) return 0;
-    if (h->last_done) cudaEventSynchronize(h->last_done);  // the previous call may still be reading the old buffer
-    if (h->stage) cudaFree(h->stage);
-    h->stage = nullptr;
-    h->stage_bytes = 0;
-    if (cudaMalloc(&h->stage, bytes) != cudaSuccess) {
-        ytk::set_error("cudaMalloc(%zu) for input staging failed", bytes);
-        return 1;
+// A handle whose calls share device buffers (staging buffers, an engine's input / activation / output buffers).  A call
+// that leaves its output on the device returns while its kernels are still queued, so every call first makes its
+// stream wait for the previous call's last operation (recorded in last_done), whatever stream that was on.  Its
+// destroy waits on last_done before the buffers are freed.
+struct OrderedHandle : Handle {
+    cudaEvent_t last_done = nullptr;
+    ~OrderedHandle() {
+        if (last_done) cudaEventDestroy(last_done);
     }
-    h->stage_bytes = bytes;
-    return 0;
-}
+
+    void order_after_previous(cudaStream_t st) {
+        if (last_done) cudaStreamWaitEvent(st, last_done, 0);
+    }
+    void mark_done(cudaStream_t st) {
+        if (!last_done) cudaEventCreateWithFlags(&last_done, cudaEventDisableTiming);
+        if (last_done) cudaEventRecord(last_done, st);
+    }
+    // Grows `buf` to `bytes`; the previous call may still be reading the old buffer.
+    int reserve(DevBuf& buf, size_t bytes, const char* what) {
+        if (buf.cap >= bytes) return 0;
+        if (last_done) cudaEventSynchronize(last_done);
+        if (buf.p) cudaFree(buf.p);
+        buf.cap = 0;
+        if (cudaMalloc(&buf.p, bytes) != cudaSuccess) {
+            buf.p = nullptr;
+            ytk::set_error("cudaMalloc(%zu) for the %s failed", bytes, what);
+            return 1;
+        }
+        buf.cap = bytes;
+        return 0;
+    }
+};
+
+// Launch plans + activation buffers per input shape.  Beyond `capacity` engines the least recently used one is dropped,
+// so that a stream of differently shaped inputs cannot exhaust HBM.
+template <class Key, class Engine>
+struct EngineCache {
+    struct Slot {
+        std::unique_ptr<Engine> engine;
+        unsigned long long used = 0;
+    };
+    std::map<Key, Slot> slots;
+    unsigned long long tick = 0;
+    int capacity;  // >= 1
+    explicit EngineCache(int cap) : capacity(cap) {}
+
+    // The engine of `key` if there is one; never builds.
+    Engine* find(const Key& key) const {
+        auto it = slots.find(key);
+        return it == slots.end() ? nullptr : it->second.engine.get();
+    }
+    // The engine of `key`, built by Engine::build(args...) if there is none; null if the build fails.
+    template <class... Args>
+    Engine* get(const Key& key, const Args&... args) {
+        auto it = slots.find(key);
+        if (it != slots.end()) {
+            it->second.used = ++tick;
+            return it->second.engine.get();
+        }
+        while ((int)slots.size() >= capacity) {
+            auto victim = std::min_element(slots.begin(), slots.end(), [](const auto& a, const auto& b) {
+                return a.second.used < b.second.used;
+            });
+            cudaDeviceSynchronize();  // its last run may still be in flight on some stream
+            slots.erase(victim);
+        }
+        auto e = std::make_unique<Engine>();
+        if (e->build(args...)) return nullptr;
+        Engine* p = e.get();
+        slots[key] = Slot{std::move(e), ++tick};
+        return p;
+    }
+};
+
+struct ytk_parseq : Handle {
+    ytk::ParseqModel model;
+    ytk::ParseqEngine engine;
+};
+
+struct ytk_dbnet : OrderedHandle {
+    ytk::DbnetModel model;
+    // per input shape (n, Hn, Wn); YTK_DBNET_MAX_ENGINES (read at create) sets the capacity
+    EngineCache<std::tuple<int, int, int>, ytk::DbnetEngine> engines{6};
+    int shortest = 1280, limit = 1600;
+    DevBuf stage;  // device staging for host inputs
+};
+
+struct ytk_rtdetr : OrderedHandle {
+    ytk::RtdetrModel model;
+    EngineCache<int, ytk::RtdetrEngine> engines{4};  // per batch size
+    int debug = 0;  // ytk_rtdetr_set_debug: forwards also capture the stages overwritten in place
+    // ytk_rtdetr_forward_u8: device copy of host pages, and the resize scratch (records, coefficients, intermediates)
+    DevBuf pages, scratch;
+};
 
 static int finish_forward(ytk_dbnet* h, ytk::DbnetEngine* e, float* prob_out, int out_on_device, cudaStream_t st) {
     if (e->run(st)) return YTK_ERR;
     const size_t bytes = (size_t)e->N * e->Hn * e->Wn * sizeof(float);
     cudaError_t err = cudaMemcpyAsync(prob_out, e->prob, bytes,
                                       out_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st);
-    mark_done(h, st);
+    h->mark_done(st);
     if (err == cudaSuccess && !out_on_device) err = cudaStreamSynchronize(st);
     if (err != cudaSuccess) {
         ytk::set_error("DBNet output copy failed: %s", cudaGetErrorString(err));
         return YTK_ERR;
     }
     return YTK_OK;
+}
+
+// Runs the engine on its packed input and copies the outputs (the common tail of both RT-DETRv2 forward entries).
+static int rt_finish(ytk_rtdetr* h, ytk::RtdetrEngine* e, int n, float* pred_logits, float* pred_boxes, int out_on_device,
+                     cudaStream_t st) {
+    if (e->run(st, h->debug != 0)) return YTK_ERR;
+    const int K = h->model.cfg.num_queries, C = h->model.cfg.num_classes;
+    const cudaMemcpyKind kind = out_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+    cudaError_t err = cudaMemcpyAsync(pred_logits, e->out_logits, (size_t)n * K * C * 4, kind, st);
+    if (err == cudaSuccess) err = cudaMemcpyAsync(pred_boxes, e->boxes, (size_t)n * K * 16, kind, st);
+    h->mark_done(st);
+    if (err == cudaSuccess && !out_on_device) err = cudaStreamSynchronize(st);
+    if (err != cudaSuccess) {
+        ytk::set_error("RT-DETRv2 output copy failed: %s", cudaGetErrorString(err));
+        return YTK_ERR;
+    }
+    return YTK_OK;
+}
+
+// The reference-keyed state_dict entries as the models' loaders read them.
+static ytk::WeightSet load_weights(const ytk_tensor* tensors, int n) {
+    ytk::WeightSet ws;
+    for (int i = 0; i < n; ++i) {
+        ytk::TensorView v;
+        v.data = tensors[i].data;
+        v.ndim = tensors[i].ndim;
+        for (int d = 0; d < 4; ++d) v.shape[d] = d < v.ndim ? tensors[i].shape[d] : 1;
+        ws.map[tensors[i].name] = v;
+    }
+    return ws;
+}
+
+// host conversion of the 16-bit GEMM operand type (the read-out launches no kernel)
+static float op_bits_to_f32(uint16_t v) {
+#ifdef YTK_OPERAND_BF16
+    __nv_bfloat16_raw r;
+    r.x = v;
+    return __bfloat162float(__nv_bfloat16(r));
+#else
+    __half_raw r;
+    r.x = v;
+    return __half2float(__half(r));
+#endif
+}
+
+// The debug read-out of every handle: `p` holds the product of `shape` values on the device, 4-byte (fp32, or int32 bit
+// patterns) or the 16-bit GEMM operand type, copied to host fp32.  shape4 receives `shape`; host_out null: shape query.
+static int read_debug(const char* who, const char* name, const void* p, bool four_byte, std::array<int, 4> shape,
+                      float* host_out, long long capacity, int* shape4) {
+    for (int i = 0; i < 4; ++i) shape4[i] = shape[i];
+    if (!host_out) return YTK_OK;
+    const long long cnt = (long long)shape[0] * shape[1] * shape[2] * shape[3];
+    if (cnt > capacity) {
+        ytk::set_error("debug tensor '%s' needs %lld floats, capacity %lld", name, cnt, capacity);
+        return YTK_ERR;
+    }
+    const cudaError_t sync = cudaDeviceSynchronize();
+    if (sync != cudaSuccess) {
+        ytk::set_error("%s: device error before the copy: %s", who, cudaGetErrorString(sync));
+        return YTK_ERR;
+    }
+    cudaError_t err;
+    if (four_byte) {
+        err = cudaMemcpy(host_out, p, cnt * 4, cudaMemcpyDeviceToHost);
+    } else {
+        std::vector<uint16_t> tmp((size_t)cnt);
+        err = cudaMemcpy(tmp.data(), p, cnt * 2, cudaMemcpyDeviceToHost);
+        if (err == cudaSuccess)
+            for (long long i = 0; i < cnt; ++i) host_out[i] = op_bits_to_f32(tmp[i]);
+    }
+    if (err != cudaSuccess) {
+        ytk::set_error("%s('%s'): copy failed: %s", who, name, cudaGetErrorString(err));
+        return YTK_ERR;
+    }
+    return YTK_OK;
+}
+
+// The device `ptr` lives on, in *dev.  False after set_error("<who>: <what> is not a device pointer") when `ptr` is not
+// device memory.
+static bool device_of(const void* ptr, const char* who, const char* what, int* dev) {
+    cudaPointerAttributes attr{};
+    if (cudaPointerGetAttributes(&attr, ptr) != cudaSuccess || attr.type != cudaMemoryTypeDevice) {
+        cudaGetLastError();
+        ytk::set_error("%s: %s is not a device pointer", who, what);
+        return false;
+    }
+    *dev = attr.device;
+    return true;
+}
+
+// Allocates `bytes` on the stream and, if `host` is given, uploads it.  The copy is from pageable memory: the call
+// returns after the data is staged, so `host` may go out of scope.  The caller frees the buffer with cudaFreeAsync.
+static void* stream_buffer(const void* host, size_t bytes, cudaStream_t st, const char* who) {
+    void* d = nullptr;
+    if (cudaMallocAsync(&d, bytes, st) != cudaSuccess) {
+        cudaGetLastError();
+        ytk::set_error("%s: cudaMallocAsync(%zu) failed", who, bytes);
+        return nullptr;
+    }
+    if (host && cudaMemcpyAsync(d, host, bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) {
+        cudaGetLastError();
+        cudaFreeAsync(d, st);
+        ytk::set_error("%s: upload of %zu bytes failed", who, bytes);
+        return nullptr;
+    }
+    return d;
+}
+
+// Host records to upload: `bytes` bytes at `p`.
+struct Part {
+    const void* p;
+    size_t bytes;
+};
+
+// Concatenates `parts` into one host blob and uploads it with one copy: to `dst` when given (the caller's scratch),
+// else into a new stream_buffer the caller frees with cudaFreeAsync.  Returns where the blob went, null after set_error.
+static uint8_t* upload_parts(std::initializer_list<Part> parts, void* dst, cudaStream_t st, const char* who) {
+    std::vector<uint8_t> blob;
+    for (const Part& q : parts) blob.insert(blob.end(), (const uint8_t*)q.p, (const uint8_t*)q.p + q.bytes);
+    if (!dst) return static_cast<uint8_t*>(stream_buffer(blob.data(), blob.size(), st, who));
+    const cudaError_t err = cudaMemcpyAsync(dst, blob.data(), blob.size(), cudaMemcpyHostToDevice, st);
+    if (err != cudaSuccess) {
+        ytk::set_error("%s: record upload failed: %s", who, cudaGetErrorString(err));
+        return nullptr;
+    }
+    return static_cast<uint8_t*>(dst);
 }
 
 extern "C" {
@@ -532,17 +710,11 @@ int ytk_op_single_query_attn_f16(int mode, const void* q, const void* kv, int B,
         }
         descs[i] = ytk::CropDesc{c.pix_off, c.w, c.wp, c.tok_off, c.ntok, c.group};
     }
-    const size_t bytes = descs.size() * sizeof(ytk::CropDesc);
-    void* descs_dev = nullptr;
-    if (cudaMallocAsync(&descs_dev, bytes, st) != cudaSuccess) {
-        cudaGetLastError();
-        ytk::set_error("ytk_op_single_query_attn_f16: cudaMallocAsync(%zu) failed", bytes);
-        return YTK_ERR;
-    }
-    // pageable source: the call returns after the records are staged, so `descs` may go out of scope
-    int rc = cudaMemcpyAsync(descs_dev, descs.data(), bytes, cudaMemcpyHostToDevice, st) != cudaSuccess;
-    if (rc) ytk::set_error("ytk_op_single_query_attn_f16: record upload failed");
-    if (!rc) rc = ytk::launch_dec_cross_attn(q, kv, reinterpret_cast<const ytk::CropDesc*>(descs_dev), B, D, heads, out, st);
+    const char* who = "ytk_op_single_query_attn_f16";
+    void* descs_dev = stream_buffer(descs.data(), descs.size() * sizeof(ytk::CropDesc), st, who);
+    if (!descs_dev) return YTK_ERR;
+    const int rc =
+        ytk::launch_dec_cross_attn(q, kv, reinterpret_cast<const ytk::CropDesc*>(descs_dev), B, D, heads, out, st);
     cudaFreeAsync(descs_dev, st);
     return rc ? YTK_ERR : YTK_OK;
 }
@@ -745,24 +917,6 @@ int ytk_op_apply_rep_cut(const int* rep_cut, int B, int S, int C, int eos_id, in
                : YTK_OK;
 }
 
-// Allocates `bytes` on the stream and, if `host` is given, uploads it.  The copy is from pageable memory: the call
-// returns after the data is staged, so `host` may go out of scope.  The caller frees the buffer with cudaFreeAsync.
-static void* stream_buffer(const void* host, size_t bytes, cudaStream_t st, const char* who) {
-    void* d = nullptr;
-    if (cudaMallocAsync(&d, bytes, st) != cudaSuccess) {
-        cudaGetLastError();
-        ytk::set_error("%s: cudaMallocAsync(%zu) failed", who, bytes);
-        return nullptr;
-    }
-    if (host && cudaMemcpyAsync(d, host, bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) {
-        cudaGetLastError();
-        cudaFreeAsync(d, st);
-        ytk::set_error("%s: upload of %zu bytes failed", who, bytes);
-        return nullptr;
-    }
-    return d;
-}
-
 // A page table: n records {page_off, H, W, rectangle} of pages back to back in `pages_bytes` bytes (ytk_page).  Records
 // come from the caller: a page beyond the buffer, an empty page or a rectangle outside its page is an error, and so is
 // a rectangle other than the whole page where the entry reads whole pages.
@@ -836,11 +990,8 @@ int ytk_op_dbnet_stem_f16(const void* canvas_dev, int n, int Hn, int Wn, const f
     std::vector<uint16_t> wp;
     ytk::pack_stem_weights(w_host, nullptr, &wp);
     const size_t wbytes = wp.size() * 2;
-    std::vector<uint8_t> blob(wbytes + 64 * 4);
-    memcpy(blob.data(), wp.data(), wbytes);
-    memcpy(blob.data() + wbytes, bias_host, 64 * 4);
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-    uint8_t* d = static_cast<uint8_t*>(stream_buffer(blob.data(), blob.size(), st, "ytk_op_dbnet_stem_f16"));
+    uint8_t* d = upload_parts({{wp.data(), wbytes}, {bias_host, 64 * 4}}, nullptr, st, "ytk_op_dbnet_stem_f16");
     if (!d) return YTK_ERR;
     ytk::Epilogue e;
     e.bias = reinterpret_cast<const float*>(d + wbytes);
@@ -946,12 +1097,9 @@ int ytk_op_dbnet_head_f32(const void* x_dev, int n, int H, int W, const float* w
     std::vector<float> bias, fin;
     ytk::pack_convt_head(w1_host, b1_host, nullptr, nullptr, w2_host, &wp, &bias, &fin);
     const size_t wbytes = wp.size() * 2, bbytes = bias.size() * 4;
-    std::vector<uint8_t> blob(wbytes + bbytes + fin.size() * 4);
-    memcpy(blob.data(), wp.data(), wbytes);
-    memcpy(blob.data() + wbytes, bias.data(), bbytes);
-    memcpy(blob.data() + wbytes + bbytes, fin.data(), fin.size() * 4);
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-    uint8_t* d = static_cast<uint8_t*>(stream_buffer(blob.data(), blob.size(), st, "ytk_op_dbnet_head_f32"));
+    uint8_t* d = upload_parts({{wp.data(), wbytes}, {bias.data(), bbytes}, {fin.data(), fin.size() * 4}}, nullptr, st,
+                              "ytk_op_dbnet_head_f32");
     if (!d) return YTK_ERR;
     ytk::ConvGeom g{n, H, W, 64, 64, 1, 1, 1, 0, 1, 256};
     ytk::Epilogue e;
@@ -984,13 +1132,9 @@ int ytk_dbnet_post_front(const float* prob_dev, int n_pages, int H, int W, float
                        ytk::dbpost_scratch_bytes(n_pages, H, W));
         return YTK_ERR;
     }
-    cudaPointerAttributes attr;
-    if (cudaPointerGetAttributes(&attr, prob_dev) != cudaSuccess || attr.type != cudaMemoryTypeDevice) {
-        cudaGetLastError();
-        ytk::set_error("ytk_dbnet_post_front: prob_dev is not a device pointer");
-        return YTK_ERR;
-    }
-    DevGuard dev_guard(attr.device);
+    int dev;
+    if (!device_of(prob_dev, "ytk_dbnet_post_front", "prob_dev", &dev)) return YTK_ERR;
+    DevGuard dev_guard(dev);
     if (ytk::launch_dbpost_front(prob_dev, n_pages, H, W, thresh, reinterpret_cast<int*>(scratch_dev),
                                  reinterpret_cast<ytk::DbRun*>(runs_dev), max_runs_per_page, meta_dev,
                                  static_cast<cudaStream_t>(cuda_stream))) {
@@ -1005,20 +1149,11 @@ int ytk_dbnet_create(const ytk_tensor* tensors, int n_tensors, int shortest_size
         ytk::set_error("ytk_dbnet_create: null argument");
         return YTK_ERR;
     }
-    ytk::WeightSet ws;
-    for (int i = 0; i < n_tensors; ++i) {
-        ytk::TensorView v;
-        v.data = tensors[i].data;
-        v.ndim = tensors[i].ndim;
-        for (int d = 0; d < 4; ++d) v.shape[d] = d < v.ndim ? tensors[i].shape[d] : 1;
-        ws.map[tensors[i].name] = v;
-    }
     auto h = std::make_unique<ytk_dbnet>();
-    cudaGetDevice(&h->device);
     h->shortest = shortest_size;
     h->limit = limit_size;
-    if (const char* me = getenv("YTK_DBNET_MAX_ENGINES")) h->max_engines = std::max(1, atoi(me));
-    if (h->model.load(ws)) return YTK_ERR;
+    if (const char* me = getenv("YTK_DBNET_MAX_ENGINES")) h->engines.capacity = std::max(1, atoi(me));
+    if (h->model.load(load_weights(tensors, n_tensors))) return YTK_ERR;
     *out = h.release();
     return YTK_OK;
 }
@@ -1026,11 +1161,7 @@ int ytk_dbnet_create(const ytk_tensor* tensors, int n_tensors, int shortest_size
 void ytk_dbnet_destroy(ytk_dbnet* h) {
     if (!h) return;
     DevGuard dev_guard(h->device);
-    if (h->last_done) {
-        cudaEventSynchronize(h->last_done);
-        cudaEventDestroy(h->last_done);
-    }
-    if (h->stage) cudaFree(h->stage);
+    if (h->last_done) cudaEventSynchronize(h->last_done);
     delete h;
 }
 
@@ -1063,18 +1194,17 @@ static int dbnet_forward_table(const char* who, ytk_dbnet* h, const uint8_t* pag
             return YTK_ERR;
         }
     }
-    std::lock_guard<std::mutex> lk(h->mu);
-    DevGuard dev_guard(h->device);  // host threads start on device 0: the handle's device is the one that counts
+    HandleCall call(h);
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-    ytk::DbnetEngine* e = get_engine(h, n_pages, Hn, Wn);
+    ytk::DbnetEngine* e = h->engines.get(std::make_tuple(n_pages, Hn, Wn), h->model, n_pages, Hn, Wn);
     if (!e) return YTK_ERR;
     // the staging buffer holds [host pages (16-byte aligned) |] the page table
     const size_t page_bytes = pages_on_device ? 0 : (size_t)(pages_bytes + 15) / 16 * 16;
     const size_t table_bytes = (size_t)n_pages * sizeof(ytk_page);
-    if (ensure_stage(h, page_bytes + table_bytes)) return YTK_ERR;
-    order_after_previous(h, st);
+    if (h->reserve(h->stage, page_bytes + table_bytes, "input staging buffer")) return YTK_ERR;
+    h->order_after_previous(st);
     const uint8_t* src = pages;
-    uint8_t* stage = reinterpret_cast<uint8_t*>(h->stage);
+    uint8_t* stage = h->stage.p;
     if (!pages_on_device) {
         if (cudaMemcpyAsync(stage, pages, (size_t)pages_bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) {
             ytk::set_error("%s: H2D copy of pages failed", who);
@@ -1113,21 +1243,20 @@ int ytk_dbnet_forward_table_u8(ytk_dbnet* h, const uint8_t* pages, int pages_on_
 
 int ytk_dbnet_forward_f32(ytk_dbnet* h, const float* x, int x_on_device, int n, int H, int W, float* prob_out,
                           int out_on_device, void* cuda_stream) {
-    std::lock_guard<std::mutex> lk(h->mu);
-    DevGuard dev_guard(h->device);  // host threads start on device 0: the handle's device is the one that counts
+    HandleCall call(h);
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-    ytk::DbnetEngine* e = get_engine(h, n, H, W);
+    ytk::DbnetEngine* e = h->engines.get(std::make_tuple(n, H, W), h->model, n, H, W);
     if (!e) return YTK_ERR;
-    order_after_previous(h, st);
+    h->order_after_previous(st);
     const float* src = x;
     if (!x_on_device) {
         const size_t bytes = (size_t)n * 3 * H * W * 4;
-        if (ensure_stage(h, bytes)) return YTK_ERR;
-        if (cudaMemcpyAsync(h->stage, x, bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) {
+        if (h->reserve(h->stage, bytes, "input staging buffer")) return YTK_ERR;
+        if (cudaMemcpyAsync(h->stage.p, x, bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) {
             ytk::set_error("H2D copy of input tensor failed");
             return YTK_ERR;
         }
-        src = reinterpret_cast<const float*>(h->stage);
+        src = reinterpret_cast<const float*>(h->stage.p);
     }
     if (ytk::launch_pack_nchw_f32(src, n, H, W, e->input, st)) {
         ytk::set_error("input pack launch failed");
@@ -1137,42 +1266,32 @@ int ytk_dbnet_forward_f32(ytk_dbnet* h, const float* x, int x_on_device, int n, 
 }
 
 double ytk_dbnet_flops(ytk_dbnet* h, int n_pages, int Hn, int Wn) {
-    std::lock_guard<std::mutex> lk(h->mu);
-    DevGuard dev_guard(h->device);  // host threads start on device 0: the handle's device is the one that counts
-    ytk::DbnetEngine* e = get_engine(h, n_pages, Hn, Wn);
+    HandleCall call(h);
+    ytk::DbnetEngine* e = h->engines.get(std::make_tuple(n_pages, Hn, Wn), h->model, n_pages, Hn, Wn);
     return e ? e->flops : -1.0;
 }
 
 int ytk_dbnet_debug_tensor(ytk_dbnet* h, int n_pages, int Hn, int Wn, const char* name, float* host_out,
                            long long capacity, int* shape4) {
-    std::lock_guard<std::mutex> lk(h->mu);
-    DevGuard dev_guard(h->device);  // host threads start on device 0: the handle's device is the one that counts
-    ytk::DbnetEngine* e = get_engine(h, n_pages, Hn, Wn);
-    if (!e) return YTK_ERR;
+    if (!h || !name || !shape4) {
+        ytk::set_error("ytk_dbnet_debug_tensor: null argument");
+        return YTK_ERR;
+    }
+    HandleCall call(h);
+    // never build an engine here: a fresh one has run nothing, and an evicted one's results are gone
+    const ytk::DbnetEngine* e = h->engines.find(std::make_tuple(n_pages, Hn, Wn));
+    if (!e) {
+        ytk::set_error("DBNet debug tensor '%s': no engine for the shape n %d, %dx%d (never run, or evicted)", name,
+                       n_pages, Hn, Wn);
+        return YTK_ERR;
+    }
     auto it = e->dbg.find(name);
     if (it == e->dbg.end() || !it->second.p) {
         ytk::set_error("no debug tensor named '%s'", name);
         return YTK_ERR;
     }
     const ytk::DebugTensor& t = it->second;
-    const long long n = (long long)t.n * t.h * t.w * t.c;
-    shape4[0] = t.n; shape4[1] = t.h; shape4[2] = t.w; shape4[3] = t.c;
-    if (n > capacity) {
-        ytk::set_error("debug tensor '%s' needs %lld floats, capacity %lld", name, n, capacity);
-        return YTK_ERR;
-    }
-    cudaDeviceSynchronize();
-    if (t.f32) {
-        if (cudaMemcpy(host_out, t.p, n * 4, cudaMemcpyDeviceToHost) != cudaSuccess) return YTK_ERR;
-    } else {
-        float* tmp = nullptr;
-        if (cudaMalloc(&tmp, n * 4) != cudaSuccess) return YTK_ERR;
-        ytk::launch_op_to_f32(t.p, tmp, n, 0);
-        cudaError_t err = cudaMemcpy(host_out, tmp, n * 4, cudaMemcpyDeviceToHost);
-        cudaFree(tmp);
-        if (err != cudaSuccess) return YTK_ERR;
-    }
-    return YTK_OK;
+    return read_debug("ytk_dbnet_debug_tensor", name, t.p, t.f32, {t.n, t.h, t.w, t.c}, host_out, capacity, shape4);
 }
 
 static_assert(sizeof(ytk_crop_geom) == sizeof(ytk::CropGeom), "ytk_crop_geom and ytk::CropGeom must have one layout");
@@ -1216,22 +1335,12 @@ int ytk_extract_crops_table_u8(const uint8_t* pages_dev, long long pages_bytes, 
                        scratch_bytes, rec_off, rec_bytes, tab_bytes);
         return YTK_ERR;
     }
-    cudaPointerAttributes attr;
-    if (cudaPointerGetAttributes(&attr, pages_dev) != cudaSuccess || attr.type != cudaMemoryTypeDevice) {
-        cudaGetLastError();
-        ytk::set_error("%s: pages_dev is not a device pointer", who);
-        return YTK_ERR;
-    }
-    DevGuard dev_guard(attr.device);
+    int device;
+    if (!device_of(pages_dev, who, "pages_dev", &device)) return YTK_ERR;
+    DevGuard dev_guard(device);
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-    std::vector<uint8_t> blob((size_t)(rec_bytes + tab_bytes));
-    memcpy(blob.data(), geoms, (size_t)rec_bytes);
-    memcpy(blob.data() + rec_bytes, table, (size_t)tab_bytes);
-    cudaError_t err = cudaMemcpyAsync(scratch_dev + rec_off, blob.data(), blob.size(), cudaMemcpyHostToDevice, st);
-    if (err != cudaSuccess) {
-        ytk::set_error("%s: record upload failed: %s", who, cudaGetErrorString(err));
+    if (!upload_parts({{geoms, (size_t)rec_bytes}, {table, (size_t)tab_bytes}}, scratch_dev + rec_off, st, who))
         return YTK_ERR;
-    }
     const ytk::CropGeom* dev = reinterpret_cast<const ytk::CropGeom*>(scratch_dev + rec_off);
     const ytk::RtSrc* tab = reinterpret_cast<const ytk::RtSrc*>(scratch_dev + rec_off + rec_bytes);
     if (ytk::launch_extract_crops_table(pages_dev, tab, dev, n_crops, scratch_dev, canvases_dev, st)) {
@@ -1267,22 +1376,12 @@ int ytk_halve_pages_table_u8(const uint8_t* src_dev, long long src_bytes, const 
         ytk::set_error("%s: scratch_dev holds %lld bytes, need %lld (two page tables)", who, scratch_bytes, 2 * tab_bytes);
         return YTK_ERR;
     }
-    cudaPointerAttributes attr;
-    if (cudaPointerGetAttributes(&attr, src_dev) != cudaSuccess || attr.type != cudaMemoryTypeDevice) {
-        cudaGetLastError();
-        ytk::set_error("%s: src_dev is not a device pointer", who);
-        return YTK_ERR;
-    }
-    DevGuard dev_guard(attr.device);
+    int device;
+    if (!device_of(src_dev, who, "src_dev", &device)) return YTK_ERR;
+    DevGuard dev_guard(device);
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-    std::vector<uint8_t> blob((size_t)(2 * tab_bytes));
-    memcpy(blob.data(), src_table, (size_t)tab_bytes);
-    memcpy(blob.data() + tab_bytes, dst_table, (size_t)tab_bytes);
-    cudaError_t err = cudaMemcpyAsync(scratch_dev, blob.data(), blob.size(), cudaMemcpyHostToDevice, st);
-    if (err != cudaSuccess) {
-        ytk::set_error("%s: page table upload failed: %s", who, cudaGetErrorString(err));
+    if (!upload_parts({{src_table, (size_t)tab_bytes}, {dst_table, (size_t)tab_bytes}}, scratch_dev, st, who))
         return YTK_ERR;
-    }
     const ytk::RtSrc* tabs = reinterpret_cast<const ytk::RtSrc*>(scratch_dev);
     if (ytk::launch_halve_pages_table(src_dev, tabs, n_pages, dst_dev, tabs + n_pages, max_pixels, st)) {
         ytk::set_error("%s: kernel launch failed", who);
@@ -1304,13 +1403,8 @@ int ytk_pack_pages_u8(const ytk_page_src* srcs, int n, uint8_t* dst_dev, long lo
         return YTK_ERR;
     }
     if (check_page_table(table, n, dst_bytes, true, who)) return YTK_ERR;
-    cudaPointerAttributes attr;
-    if (cudaPointerGetAttributes(&attr, dst_dev) != cudaSuccess || attr.type != cudaMemoryTypeDevice) {
-        cudaGetLastError();
-        ytk::set_error("%s: dst_dev is not a device pointer", who);
-        return YTK_ERR;
-    }
-    const int device = attr.device;
+    int device;
+    if (!device_of(dst_dev, who, "dst_dev", &device)) return YTK_ERR;
     long long max_pixels = 0;
     for (int i = 0; i < n; ++i) {
         const ytk_page_src& s = srcs[i];
@@ -1323,10 +1417,8 @@ int ytk_pack_pages_u8(const ytk_page_src* srcs, int n, uint8_t* dst_dev, long lo
             ytk::set_error("%s: source %d is %dx%d, its page record %dx%d", who, i, s.H, s.W, table[i].H, table[i].W);
             return YTK_ERR;
         }
-        cudaPointerAttributes a;
-        if (cudaPointerGetAttributes(&a, s.data) != cudaSuccess || a.type != cudaMemoryTypeDevice ||
-            a.device != device) {
-            cudaGetLastError();
+        int src_device;
+        if (!device_of(s.data, who, "a source", &src_device) || src_device != device) {
             ytk::set_error("%s: source %d is not in device memory of device %d (the device of dst_dev)", who, i, device);
             return YTK_ERR;
         }
@@ -1341,14 +1433,7 @@ int ytk_pack_pages_u8(const ytk_page_src* srcs, int n, uint8_t* dst_dev, long lo
     }
     DevGuard dev_guard(device);
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-    std::vector<uint8_t> blob((size_t)(src_bytes + tab_bytes));
-    memcpy(blob.data(), srcs, (size_t)src_bytes);
-    memcpy(blob.data() + src_bytes, table, (size_t)tab_bytes);
-    cudaError_t err = cudaMemcpyAsync(scratch_dev, blob.data(), blob.size(), cudaMemcpyHostToDevice, st);
-    if (err != cudaSuccess) {
-        ytk::set_error("%s: record upload failed: %s", who, cudaGetErrorString(err));
-        return YTK_ERR;
-    }
+    if (!upload_parts({{srcs, (size_t)src_bytes}, {table, (size_t)tab_bytes}}, scratch_dev, st, who)) return YTK_ERR;
     const ytk::PageSrc* dev_srcs = reinterpret_cast<const ytk::PageSrc*>(scratch_dev);
     const ytk::RtSrc* dev_tab = reinterpret_cast<const ytk::RtSrc*>(scratch_dev + src_bytes);
     if (ytk::launch_pack_pages(dev_srcs, dev_tab, n, max_pixels, dst_dev, st)) {
@@ -1363,39 +1448,32 @@ int ytk_parseq_create(const ytk_tensor* tensors, int n_tensors, const ytk_parseq
         ytk::set_error("ytk_parseq_create: null argument");
         return YTK_ERR;
     }
-    ytk::WeightSet ws;
-    for (int i = 0; i < n_tensors; ++i) {
-        ytk::TensorView v;
-        v.data = tensors[i].data;
-        v.ndim = tensors[i].ndim;
-        for (int d = 0; d < 4; ++d) v.shape[d] = d < v.ndim ? tensors[i].shape[d] : 1;
-        ws.map[tensors[i].name] = v;
-    }
     ytk::ParseqCfg c{cfg->embed_dim, cfg->enc_heads, cfg->enc_depth, cfg->patch_h, cfg->patch_w, cfg->img_h,
                      cfg->img_w, cfg->num_tokens, cfg->max_label_length, cfg->dec_heads, cfg->mlp_ratio,
                      cfg->dec_mlp_ratio, cfg->refine_iters, cfg->repetition_stop, cfg->rep_period_max,
                      cfg->rep_min_run_p1, cfg->rep_min_repeats, cfg->decode_ar};
     auto h = std::make_unique<ytk_parseq>();
-    cudaGetDevice(&h->device);
-    if (h->model.load(ws, c)) return YTK_ERR;
+    if (h->model.load(load_weights(tensors, n_tensors), c)) return YTK_ERR;
     h->engine.m = &h->model;
     *out = h.release();
     return YTK_OK;
 }
 
-void ytk_parseq_destroy(ytk_parseq* h) { delete h; }
+void ytk_parseq_destroy(ytk_parseq* h) {
+    if (!h) return;
+    DevGuard dev_guard(h->device);
+    delete h;
+}
 
 void ytk_parseq_set_refine_iters(ytk_parseq* h, int refine_iters) {
-    std::lock_guard<std::mutex> lk(h->mu);
-    DevGuard dev_guard(h->device);  // host threads start on device 0: the handle's device is the one that counts
+    HandleCall call(h);
     h->model.cfg.refine_iters = refine_iters;
 }
 
 int ytk_parseq_forward_crops(ytk_parseq* h, const uint8_t* crops_ptr, int crops_on_device, long long crops_bytes,
                              const ytk_crop* crops, int n_crops, int n_groups, int32_t* ids_out, float* probs_out,
                              int32_t* group_len_out, void* cuda_stream) {
-    std::lock_guard<std::mutex> lk(h->mu);
-    DevGuard dev_guard(h->device);  // host threads start on device 0: the handle's device is the one that counts
+    HandleCall call(h);
     ytk::ParseqBatch b;
     b.crops = crops_ptr;
     b.crops_on_device = crops_on_device;
@@ -1422,8 +1500,7 @@ int ytk_parseq_forward_crops(ytk_parseq* h, const uint8_t* crops_ptr, int crops_
 int ytk_parseq_forward_f32(ytk_parseq* h, const float* images, int images_on_device, int B, int W, float* logits_out,
                            int logits_on_device, int32_t* ids_out, float* probs_out, int32_t* steps_out,
                            int32_t* rep_cut_out, float* memory_out, void* cuda_stream) {
-    std::lock_guard<std::mutex> lk(h->mu);
-    DevGuard dev_guard(h->device);  // host threads start on device 0: the handle's device is the one that counts
+    HandleCall call(h);
     const int pw = h->model.cfg.pw, gh = h->model.gh;
     if (W % pw != 0 || W > h->model.cfg.img_w || W <= 0) {
         ytk::set_error("ytk_parseq_forward_f32: width %d must be a positive multiple of %d and <= %d", W, pw,
@@ -1463,22 +1540,9 @@ int ytk_parseq_set_debug(ytk_parseq* h, int on) {
         ytk::set_error("ytk_parseq_set_debug: null handle");
         return YTK_ERR;
     }
-    std::lock_guard<std::mutex> lk(h->mu);
+    HandleCall call(h);
     h->engine.debug = on ? 1 : 0;
     return YTK_OK;
-}
-
-// host conversion of the 16-bit GEMM operand type (the read-out launches no kernel)
-static float op_bits_to_f32(uint16_t v) {
-#ifdef YTK_OPERAND_BF16
-    __nv_bfloat16_raw r;
-    r.x = v;
-    return __bfloat162float(__nv_bfloat16(r));
-#else
-    __half_raw r;
-    r.x = v;
-    return __half2float(__half(r));
-#endif
 }
 
 int ytk_parseq_debug_tensor(ytk_parseq* h, const char* name, float* host_out, long long capacity, int* shape4) {
@@ -1486,41 +1550,12 @@ int ytk_parseq_debug_tensor(ytk_parseq* h, const char* name, float* host_out, lo
         ytk::set_error("ytk_parseq_debug_tensor: null argument");
         return YTK_ERR;
     }
-    std::lock_guard<std::mutex> lk(h->mu);
-    DevGuard dev_guard(h->device);
+    HandleCall call(h);
     ytk::ParseqEngine::View v;
     if (h->engine.debug_view(name, &v)) return YTK_ERR;
-    const long long cnt = v.rows * v.cols;
-    shape4[0] = (int)v.rows;
-    shape4[1] = v.cols;
-    shape4[2] = shape4[3] = 1;
-    if (!host_out) return YTK_OK;  // shape query
-    if (cnt > capacity) {
-        ytk::set_error("debug tensor '%s' needs %lld floats, capacity %lld", name, cnt, capacity);
-        return YTK_ERR;
-    }
-    const cudaError_t sync = cudaDeviceSynchronize();
-    if (sync != cudaSuccess) {
-        ytk::set_error("ytk_parseq_debug_tensor: device error before the copy: %s", cudaGetErrorString(sync));
-        return YTK_ERR;
-    }
-    cudaError_t err;
-    if (v.kind != 0) {  // fp32 values / int32 bit patterns
-        err = cudaMemcpy(host_out, v.p, cnt * 4, cudaMemcpyDeviceToHost);
-        if (err != cudaSuccess) {
-            ytk::set_error("ytk_parseq_debug_tensor('%s'): copy failed: %s", name, cudaGetErrorString(err));
-            return YTK_ERR;
-        }
-        return YTK_OK;
-    }
-    std::vector<uint16_t> tmp((size_t)cnt);
-    err = cudaMemcpy(tmp.data(), v.p, cnt * 2, cudaMemcpyDeviceToHost);
-    if (err != cudaSuccess) {
-        ytk::set_error("ytk_parseq_debug_tensor('%s'): copy failed: %s", name, cudaGetErrorString(err));
-        return YTK_ERR;
-    }
-    for (long long i = 0; i < cnt; ++i) host_out[i] = op_bits_to_f32(tmp[i]);
-    return YTK_OK;
+    // kind != 0: fp32 values or int32 bit patterns
+    return read_debug("ytk_parseq_debug_tensor", name, v.p, v.kind != 0, {(int)v.rows, v.cols, 1, 1}, host_out,
+                      capacity, shape4);
 }
 
 int ytk_op_assign_best_overlap_f64(const double* word_boxes_dev, int n_words, const double* elem_boxes_dev,
@@ -1566,19 +1601,12 @@ int ytk_op_assign_best_overlap_f64(const double* word_boxes_dev, int n_words, co
         ytk::set_error("%s: word_boxes_dev and elem_boxes_dev must be 16-byte aligned", who);
         return YTK_ERR;
     }
-    cudaPointerAttributes attr{};
-    if (cudaPointerGetAttributes(&attr, word_boxes_dev) != cudaSuccess || attr.type != cudaMemoryTypeDevice) {
-        cudaGetLastError();
-        ytk::set_error("%s: word_boxes_dev is not a device pointer", who);
-        return YTK_ERR;
-    }
-    DevGuard dev_guard(attr.device);
+    int device;
+    if (!device_of(word_boxes_dev, who, "word_boxes_dev", &device)) return YTK_ERR;
+    DevGuard dev_guard(device);
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
     const size_t gbytes = dg.size() * sizeof(ytk::OverlapGroup), ibytes = items.size() * sizeof(ytk::OverlapItem);
-    std::vector<uint8_t> blob(gbytes + ibytes);
-    std::memcpy(blob.data(), dg.data(), gbytes);
-    std::memcpy(blob.data() + gbytes, items.data(), ibytes);
-    uint8_t* d = static_cast<uint8_t*>(stream_buffer(blob.data(), blob.size(), st, who));
+    uint8_t* d = upload_parts({{dg.data(), gbytes}, {items.data(), ibytes}}, nullptr, st, who);
     if (!d) return YTK_ERR;
     const int rc = ytk::launch_assign_best_overlap(word_boxes_dev, elem_boxes_dev, elem_skip_dev,
                                                    reinterpret_cast<const ytk::OverlapGroup*>(d),
@@ -1589,88 +1617,14 @@ int ytk_op_assign_best_overlap_f64(const double* word_boxes_dev, int n_words, co
     return rc ? YTK_ERR : YTK_OK;
 }
 
-}  // extern "C"
-
-
 // ------------------------------------------------------------------------------------------------ RT-DETRv2
-struct ytk_rtdetr {
-    ytk::RtdetrModel model;
-    std::map<int, std::unique_ptr<ytk::RtdetrEngine>> engines;   // per batch size
-    std::mutex mu;
-    int device = 0;
-    cudaEvent_t last_done = nullptr;   // buffers of an engine are shared by all calls: order them (see ytk_dbnet)
-    int debug = 0;                     // ytk_rtdetr_set_debug: forwards also capture the stages overwritten in place
-    // ytk_rtdetr_forward_u8: device copy of host pages, and the resize scratch (records, coefficients, intermediates)
-    uint8_t* pages = nullptr;
-    size_t pages_cap = 0;
-    uint8_t* scratch = nullptr;
-    size_t scratch_cap = 0;
-};
-
-// Grows a handle-owned buffer; the previous call may still be reading the old one.
-static int rt_reserve(ytk_rtdetr* h, uint8_t** buf, size_t* cap, size_t bytes, const char* what) {
-    if (*cap >= bytes) return 0;
-    if (h->last_done) cudaEventSynchronize(h->last_done);
-    if (*buf) cudaFree(*buf);
-    *buf = nullptr;
-    *cap = 0;
-    if (cudaMalloc(buf, bytes) != cudaSuccess) {
-        *buf = nullptr;
-        ytk::set_error("cudaMalloc(%zu) for the %s failed", bytes, what);
-        return 1;
-    }
-    *cap = bytes;
-    return 0;
-}
-
-// Runs the engine on its packed input and copies the outputs (the common tail of both forward entries).
-static int rt_finish(ytk_rtdetr* h, ytk::RtdetrEngine* e, int n, float* pred_logits, float* pred_boxes, int out_on_device,
-                     cudaStream_t st) {
-    if (e->run(st, h->debug != 0)) return YTK_ERR;
-    const int K = h->model.cfg.num_queries, C = h->model.cfg.num_classes;
-    const cudaMemcpyKind kind = out_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-    cudaError_t err = cudaMemcpyAsync(pred_logits, e->out_logits, (size_t)n * K * C * 4, kind, st);
-    if (err == cudaSuccess) err = cudaMemcpyAsync(pred_boxes, e->boxes, (size_t)n * K * 16, kind, st);
-    if (!h->last_done) cudaEventCreateWithFlags(&h->last_done, cudaEventDisableTiming);
-    if (h->last_done) cudaEventRecord(h->last_done, st);
-    if (err == cudaSuccess && !out_on_device) err = cudaStreamSynchronize(st);
-    if (err != cudaSuccess) {
-        ytk::set_error("RT-DETRv2 output copy failed: %s", cudaGetErrorString(err));
-        return YTK_ERR;
-    }
-    return YTK_OK;
-}
-
-static ytk::RtdetrEngine* rt_engine(ytk_rtdetr* h, int n) {
-    auto it = h->engines.find(n);
-    if (it != h->engines.end()) return it->second.get();
-    if (h->engines.size() >= 4) {
-        cudaDeviceSynchronize();
-        h->engines.erase(h->engines.begin());
-    }
-    auto e = std::make_unique<ytk::RtdetrEngine>();
-    if (e->build(h->model, n)) return nullptr;
-    ytk::RtdetrEngine* p = e.get();
-    h->engines[n] = std::move(e);
-    return p;
-}
-
 int ytk_rtdetr_create(const ytk_tensor* tensors, int n_tensors, int num_classes, int num_queries, int img_size,
                       ytk_rtdetr** out) {
     if (!tensors || !out) {
         ytk::set_error("ytk_rtdetr_create: null argument");
         return YTK_ERR;
     }
-    ytk::WeightSet ws;
-    for (int i = 0; i < n_tensors; ++i) {
-        ytk::TensorView v;
-        v.data = tensors[i].data;
-        v.ndim = tensors[i].ndim;
-        for (int d = 0; d < 4; ++d) v.shape[d] = d < v.ndim ? tensors[i].shape[d] : 1;
-        ws.map[tensors[i].name] = v;
-    }
     auto h = std::make_unique<ytk_rtdetr>();
-    cudaGetDevice(&h->device);
     ytk::RtCfg cfg;
     cfg.num_classes = num_classes;
     cfg.num_queries = num_queries;
@@ -1679,7 +1633,7 @@ int ytk_rtdetr_create(const ytk_tensor* tensors, int n_tensors, int num_classes,
         ytk::set_error("ytk_rtdetr_create: num_classes %d (1..8) / num_queries %d unsupported", num_classes, num_queries);
         return YTK_ERR;
     }
-    if (h->model.load(ws, cfg)) return YTK_ERR;
+    if (h->model.load(load_weights(tensors, n_tensors), cfg)) return YTK_ERR;
     *out = h.release();
     return YTK_OK;
 }
@@ -1687,13 +1641,8 @@ int ytk_rtdetr_create(const ytk_tensor* tensors, int n_tensors, int num_classes,
 void ytk_rtdetr_destroy(ytk_rtdetr* h) {
     if (!h) return;
     DevGuard dev_guard(h->device);
-    if (h->last_done) {
-        cudaEventSynchronize(h->last_done);
-        cudaEventDestroy(h->last_done);
-    }
+    if (h->last_done) cudaEventSynchronize(h->last_done);
     cudaDeviceSynchronize();
-    if (h->pages) cudaFree(h->pages);
-    if (h->scratch) cudaFree(h->scratch);
     delete h;
 }
 
@@ -1705,12 +1654,11 @@ int ytk_rtdetr_forward_f32(ytk_rtdetr* h, const float* x, int x_on_device, int n
         ytk::set_error("ytk_rtdetr_forward_f32: null or empty argument");
         return YTK_ERR;
     }
-    std::lock_guard<std::mutex> lk(h->mu);
-    DevGuard dev_guard(h->device);
+    HandleCall call(h);
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
-    ytk::RtdetrEngine* e = rt_engine(h, n);
+    ytk::RtdetrEngine* e = h->engines.get(n, h->model, n);
     if (!e) return YTK_ERR;
-    if (h->last_done) cudaStreamWaitEvent(st, h->last_done, 0);
+    h->order_after_previous(st);
     const int S = h->model.cfg.img;
     const float* src = x;
     if (!x_on_device) {
@@ -1733,29 +1681,27 @@ int ytk_rtdetr_forward_u8(ytk_rtdetr* h, const uint8_t* pages, int pages_on_devi
         ytk::set_error("ytk_rtdetr_forward_u8: null or empty argument");
         return YTK_ERR;
     }
-    std::lock_guard<std::mutex> lk(h->mu);
-    DevGuard dev_guard(h->device);
+    HandleCall call(h);
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
     ytk::ResampleJob job;
     if (ytk::resample_prepare(reinterpret_cast<const ytk::RtSrc*>(srcs), n, h->model.cfg.img, pages_bytes,
                               "ytk_rtdetr_forward_u8", &job))
         return YTK_ERR;
-    ytk::RtdetrEngine* e = rt_engine(h, n);
+    ytk::RtdetrEngine* e = h->engines.get(n, h->model, n);
     if (!e) return YTK_ERR;
-    if (!pages_on_device && rt_reserve(h, &h->pages, &h->pages_cap, (size_t)pages_bytes, "page staging buffer"))
-        return YTK_ERR;
-    if (rt_reserve(h, &h->scratch, &h->scratch_cap, (size_t)job.bytes, "resize scratch")) return YTK_ERR;
-    if (h->last_done) cudaStreamWaitEvent(st, h->last_done, 0);
+    if (!pages_on_device && h->reserve(h->pages, (size_t)pages_bytes, "page staging buffer")) return YTK_ERR;
+    if (h->reserve(h->scratch, (size_t)job.bytes, "resize scratch")) return YTK_ERR;
+    h->order_after_previous(st);
     const uint8_t* src = pages;
     if (!pages_on_device) {
-        cudaError_t err = cudaMemcpyAsync(h->pages, pages, (size_t)pages_bytes, cudaMemcpyHostToDevice, st);
+        cudaError_t err = cudaMemcpyAsync(h->pages.p, pages, (size_t)pages_bytes, cudaMemcpyHostToDevice, st);
         if (err != cudaSuccess) {
             ytk::set_error("H2D copy of the pages failed: %s", cudaGetErrorString(err));
             return YTK_ERR;
         }
-        src = h->pages;
+        src = h->pages.p;
     }
-    if (ytk::launch_resample(src, job, h->scratch, e->input, 1, st)) return YTK_ERR;
+    if (ytk::launch_resample(src, job, h->scratch.p, e->input, 1, st)) return YTK_ERR;
     return rt_finish(h, e, n, pred_logits, pred_boxes, out_on_device, st);
 }
 
@@ -1782,22 +1728,17 @@ int ytk_op_resize_bilinear_u8(const uint8_t* pages_dev, long long pages_bytes, c
         ytk::set_error("ytk_op_resize_bilinear_u8: scratch_dev holds %lld bytes, need %lld", scratch_bytes, job.bytes);
         return YTK_ERR;
     }
-    cudaPointerAttributes attr;
-    if (cudaPointerGetAttributes(&attr, pages_dev) != cudaSuccess || attr.type != cudaMemoryTypeDevice) {
-        cudaGetLastError();
-        ytk::set_error("ytk_op_resize_bilinear_u8: pages_dev is not a device pointer");
-        return YTK_ERR;
-    }
-    DevGuard dev_guard(attr.device);
+    int device;
+    if (!device_of(pages_dev, "ytk_op_resize_bilinear_u8", "pages_dev", &device)) return YTK_ERR;
+    DevGuard dev_guard(device);
     return ytk::launch_resample(pages_dev, job, scratch_dev, out_rgb_dev, 0, static_cast<cudaStream_t>(cuda_stream))
                ? YTK_ERR
                : YTK_OK;
 }
 
 double ytk_rtdetr_flops(ytk_rtdetr* h, int n) {
-    std::lock_guard<std::mutex> lk(h->mu);
-    DevGuard dev_guard(h->device);
-    ytk::RtdetrEngine* e = rt_engine(h, n);
+    HandleCall call(h);
+    ytk::RtdetrEngine* e = h->engines.get(n, h->model, n);
     return e ? e->flops : -1.0;
 }
 
@@ -1806,7 +1747,7 @@ int ytk_rtdetr_set_debug(ytk_rtdetr* h, int on) {
         ytk::set_error("ytk_rtdetr_set_debug: null handle");
         return YTK_ERR;
     }
-    std::lock_guard<std::mutex> lk(h->mu);
+    HandleCall call(h);
     h->debug = on ? 1 : 0;
     return YTK_OK;
 }
@@ -1816,43 +1757,16 @@ int ytk_rtdetr_debug_tensor(ytk_rtdetr* h, int n, const char* name, float* host_
         ytk::set_error("ytk_rtdetr_debug_tensor: null argument");
         return YTK_ERR;
     }
-    std::lock_guard<std::mutex> lk(h->mu);
-    DevGuard dev_guard(h->device);
+    HandleCall call(h);
     // never build an engine here: a fresh one has run nothing, and an evicted one's results are gone
-    auto eit = h->engines.find(n);
-    if (eit == h->engines.end()) {
+    const ytk::RtdetrEngine* e = h->engines.find(n);
+    if (!e) {
         ytk::set_error("RT-DETRv2 debug tensor '%s': no engine for batch size %d (never run, or evicted)", name, n);
         return YTK_ERR;
     }
     ytk::DebugTensor t;
-    if (eit->second->debug_view(name, &t)) return YTK_ERR;
-    const long long cnt = (long long)t.n * t.h * t.w * t.c;
-    shape4[0] = t.n;
-    shape4[1] = t.h;
-    shape4[2] = t.w;
-    shape4[3] = t.c;
-    if (!host_out) return YTK_OK;  // shape query
-    if (cnt > capacity) {
-        ytk::set_error("debug tensor '%s' needs %lld floats, capacity %lld", name, cnt, capacity);
-        return YTK_ERR;
-    }
-    const cudaError_t sync = cudaDeviceSynchronize();
-    if (sync != cudaSuccess) {
-        ytk::set_error("ytk_rtdetr_debug_tensor: device error before the copy: %s", cudaGetErrorString(sync));
-        return YTK_ERR;
-    }
-    cudaError_t err;
-    if (t.f32) {
-        err = cudaMemcpy(host_out, t.p, cnt * 4, cudaMemcpyDeviceToHost);
-    } else {
-        std::vector<uint16_t> tmp((size_t)cnt);
-        err = cudaMemcpy(tmp.data(), t.p, cnt * 2, cudaMemcpyDeviceToHost);
-        if (err == cudaSuccess)
-            for (long long i = 0; i < cnt; ++i) host_out[i] = op_bits_to_f32(tmp[i]);
-    }
-    if (err != cudaSuccess) {
-        ytk::set_error("ytk_rtdetr_debug_tensor('%s'): copy failed: %s", name, cudaGetErrorString(err));
-        return YTK_ERR;
-    }
-    return YTK_OK;
+    if (e->debug_view(name, &t)) return YTK_ERR;
+    return read_debug("ytk_rtdetr_debug_tensor", name, t.p, t.f32, {t.n, t.h, t.w, t.c}, host_out, capacity, shape4);
 }
+
+}  // extern "C"

@@ -442,14 +442,4 @@ int launch_asf(const void* a, void* fuse, int n_img, int H, int W, const float* 
     return cudaGetLastError() != cudaSuccess;
 }
 
-// fp32 -> bf16 conversion helper for weight upload / debug
-__global__ void op_to_f32_kernel(const op_t* __restrict__ in, float* __restrict__ out, long long n) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = op2f(in[i]);
-}
-int launch_op_to_f32(const void* in, float* out, long long n, cudaStream_t st) {
-    op_to_f32_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(reinterpret_cast<const op_t*>(in), out, n);
-    return cudaGetLastError() != cudaSuccess;
-}
-
 }  // namespace ytk

@@ -21,6 +21,5 @@ int launch_upsample(const void* src, int n_img, int Hs, int Ws, int C, void* dst
 int launch_asf(const void* a, void* fuse, int n_img, int H, int W, const float* w1_dev, const float* w2_dev,
                const float* host_sp3, float host_sp1, const float* host_att, float* gsum, float* gvec, float* gmean,
                float* m, cudaStream_t st);
-int launch_op_to_f32(const void* in, float* out, long long n, cudaStream_t st);
 
 }  // namespace ytk

@@ -76,8 +76,37 @@ class _DeviceModel:
     def parameters(self):
         return (v for v in self._sd.values() if torch.is_floating_point(v))
 
+    # -- handle management: a subclass gives its create call (_create) and the name of its destroy function (_DESTROY)
+    def _ensure(self):
+        self._require_cuda()
+        if self._handle is None:
+            tab, keep = _lib.tensor_table(self._sd)
+            h = ctypes.c_void_p()
+            with torch.cuda.device(self.cuda_device()):     # the handle binds to the device current at create()
+                _lib.check(self._create(tab, ctypes.byref(h)))
+            self._handle = h
+        return self._handle
+
     def _release(self):
-        raise NotImplementedError
+        if self._handle is not None:
+            getattr(_lib.lib(), self._DESTROY)(self._handle)
+            self._handle = None
+
+    def __del__(self):
+        try:
+            self._release()
+        except Exception:
+            pass
+
+    def _read_debug(self, fn, *args):
+        """Test hook behind debug_tensor: fn(handle, *args, host_out, capacity, shape4) asked for the shape, then read
+        into a float32 numpy array of that shape."""
+        h = self._ensure()
+        shape = (ctypes.c_int * 4)()
+        _lib.check(fn(h, *args, None, 0, shape))
+        buf = np.empty([int(v) for v in shape], dtype=np.float32)
+        _lib.check(fn(h, *args, buf.ctypes.data, buf.size, shape))
+        return buf
 
     def _require_cuda(self):
         if not torch.cuda.is_available():
@@ -387,28 +416,10 @@ class DBNet(_DeviceModel):
         self._shortest = int(cfg.data.shortest_size) if cfg is not None else 1280
         self._limit = int(cfg.data.limit_size) if cfg is not None else 1600
 
-    # -- handle management
-    def _ensure(self):
-        self._require_cuda()
-        if self._handle is None:
-            L = _lib.lib()
-            tab, keep = _lib.tensor_table(self._sd)
-            h = ctypes.c_void_p()
-            with torch.cuda.device(self.cuda_device()):     # the handle binds to the device current at create()
-                _lib.check(L.ytk_dbnet_create(tab, len(tab), self._shortest, self._limit, ctypes.byref(h)))
-            self._handle = h
-        return self._handle
+    _DESTROY = "ytk_dbnet_destroy"
 
-    def _release(self):
-        if self._handle is not None:
-            _lib.lib().ytk_dbnet_destroy(self._handle)
-            self._handle = None
-
-    def __del__(self):
-        try:
-            self._release()
-        except Exception:
-            pass
+    def _create(self, tab, out):
+        return _lib.lib().ytk_dbnet_create(tab, len(tab), self._shortest, self._limit, out)
 
     def input_size(self, h, w):
         """(Hn, Wn) the network sees for an h x w page = reference resize_shortest_edge (functions.py:212-224)."""
@@ -463,6 +474,11 @@ class DBNet(_DeviceModel):
 
     def flops(self, n, Hn, Wn):
         return _lib.lib().ytk_dbnet_flops(self._ensure(), n, Hn, Wn)
+
+    def debug_tensor(self, n, Hn, Wn, name):
+        """Test hook: an intermediate activation (names in include/yomitoku_b200.h, ytk_dbnet_debug_tensor) of the last
+        run at the input shape (n, Hn, Wn) as a CPU float32 tensor (n, h, w, c)."""
+        return torch.from_numpy(self._read_debug(_lib.lib().ytk_dbnet_debug_tensor, n, Hn, Wn, name.encode()))
 
 
 # ======================================================================================================== PARSeq
@@ -578,33 +594,16 @@ class PARSeq(_DeviceModel):
     def num_classes(self):
         return self.cfg.num_tokens - 2
 
-    def _ensure(self):
-        self._require_cuda()
-        if self._handle is None:
-            c = self.cfg
-            L = _lib.lib()
-            tab, keep = _lib.tensor_table(self._sd)
-            cc = _lib.YtkParseqCfg(c.encoder.embed_dim, c.encoder.num_heads, c.encoder.depth, c.encoder.patch_size[0],
-                                   c.encoder.patch_size[1], c.data.img_size[0], c.data.img_size[1], c.num_tokens,
-                                   c.max_label_length, c.decoder.num_heads, c.encoder.mlp_ratio, c.decoder.mlp_ratio,
-                                   self._refine_iters, 1 if self.repetition_stop else 0, self.rep_period_max,
-                                   self.rep_min_run_p1, self.rep_min_repeats, 1 if self.decode_ar else 0)
-            h = ctypes.c_void_p()
-            with torch.cuda.device(self.cuda_device()):     # the handle binds to the device current at create()
-                _lib.check(L.ytk_parseq_create(tab, len(tab), ctypes.byref(cc), ctypes.byref(h)))
-            self._handle = h
-        return self._handle
+    _DESTROY = "ytk_parseq_destroy"
 
-    def _release(self):
-        if self._handle is not None:
-            _lib.lib().ytk_parseq_destroy(self._handle)
-            self._handle = None
-
-    def __del__(self):
-        try:
-            self._release()
-        except Exception:
-            pass
+    def _create(self, tab, out):
+        c = self.cfg
+        cc = _lib.YtkParseqCfg(c.encoder.embed_dim, c.encoder.num_heads, c.encoder.depth, c.encoder.patch_size[0],
+                               c.encoder.patch_size[1], c.data.img_size[0], c.data.img_size[1], c.num_tokens,
+                               c.max_label_length, c.decoder.num_heads, c.encoder.mlp_ratio, c.decoder.mlp_ratio,
+                               self._refine_iters, 1 if self.repetition_stop else 0, self.rep_period_max,
+                               self.rep_min_run_p1, self.rep_min_repeats, 1 if self.decode_ar else 0)
+        return _lib.lib().ytk_parseq_create(tab, len(tab), ctypes.byref(cc), out)
 
     def __call__(self, images, max_length=None, memory_out=None):
         return self.forward(images, max_length, memory_out)
@@ -696,11 +695,8 @@ class PARSeq(_DeviceModel):
     def debug_tensor(self, name):
         """Test hook: a stage of the last forward (names in include/yomitoku_b200.h, ytk_parseq_debug_tensor) as a CPU
         tensor [rows, cols] at the engine's padded width: float32, or int32 for the integer buffers."""
-        h = self._ensure()
-        shape = (ctypes.c_int * 4)()
-        _lib.check(_lib.lib().ytk_parseq_debug_tensor(h, name.encode(), None, 0, shape))
-        buf = torch.empty((shape[0], shape[1]), dtype=torch.float32)
-        _lib.check(_lib.lib().ytk_parseq_debug_tensor(h, name.encode(), buf.data_ptr(), buf.numel(), shape))
+        a = self._read_debug(_lib.lib().ytk_parseq_debug_tensor, name.encode())     # shape (rows, cols, 1, 1)
+        buf = torch.from_numpy(a.reshape(a.shape[:2]))
         if name in ("ar.tgt", "ar.raw", "ar.group_len", "ar.rep_cut", "dec.klen", "dec.kpad", "dec.ctx"):
             return buf.view(torch.int32)
         return buf
@@ -841,27 +837,10 @@ class RTDETRv2(_DeviceModel):
                              % (list(cfg.data.img_size), list(d.eval_spatial_size)))
         self._sd = _rtdetr_random_state_dict(self.num_classes, seed, self.img_size)
 
-    def _ensure(self):
-        self._require_cuda()
-        if self._handle is None:
-            tab, keep = _lib.tensor_table(self._sd)
-            h = ctypes.c_void_p()
-            with torch.cuda.device(self.cuda_device()):
-                _lib.check(_lib.lib().ytk_rtdetr_create(tab, len(tab), self.num_classes, self.num_queries, self.img_size,
-                                                        ctypes.byref(h)))
-            self._handle = h
-        return self._handle
+    _DESTROY = "ytk_rtdetr_destroy"
 
-    def _release(self):
-        if self._handle is not None:
-            _lib.lib().ytk_rtdetr_destroy(self._handle)
-            self._handle = None
-
-    def __del__(self):
-        try:
-            self._release()
-        except Exception:
-            pass
+    def _create(self, tab, out):
+        return _lib.lib().ytk_rtdetr_create(tab, len(tab), self.num_classes, self.num_queries, self.img_size, out)
 
     def __call__(self, tensor, targets=None):
         return self.forward(tensor)
@@ -914,10 +893,4 @@ class RTDETRv2(_DeviceModel):
 
     def debug_tensor(self, n, name):
         """Intermediate activation of the last forward of batch size n (test hook) as a numpy array."""
-        h = self._ensure()
-        shape = (ctypes.c_int * 4)()
-        _lib.check(_lib.lib().ytk_rtdetr_debug_tensor(h, n, name.encode(), None, 0, shape))
-        dims = [int(v) for v in shape]
-        buf = np.empty(dims, dtype=np.float32)
-        _lib.check(_lib.lib().ytk_rtdetr_debug_tensor(h, n, name.encode(), buf.ctypes.data, buf.size, shape))
-        return buf
+        return self._read_debug(_lib.lib().ytk_rtdetr_debug_tensor, n, name.encode())
