@@ -506,6 +506,28 @@ int ytk_op_resize_bilinear_u8(const uint8_t* pages_dev, long long pages_bytes, c
 long long ytk_op_resize_bilinear_scratch_bytes(const ytk_rtdetr_src* srcs, int n, int size);
 double ytk_rtdetr_flops(ytk_rtdetr* h, int n);
 
+/* ---- Whole pages resized to per-page sizes (the searchable PDF's page images): per record, the BGR page as RGB,
+ * Image.fromarray(rgb).resize((out_w, out_h), filter) bit for bit (Pillow 12's fixed-point separable resample; an axis
+ * whose size does not change has no pass, so an unchanged page is a BGR -> RGB copy), written planar. ---- */
+#define YTK_RESAMPLE_LANCZOS 1   /* Pillow's Image.LANCZOS */
+#define YTK_RESAMPLE_BILINEAR 2  /* Pillow's Image.BILINEAR */
+typedef struct {
+    long long page_off;   /* byte offset of the page in pages_dev: H*W*3 bytes, BGR */
+    int H, W;             /* page size (>= 1) */
+    int out_w, out_h;     /* output size (>= 1) */
+    long long out_off;    /* byte offset in out_dev of the output, [3][out_h][out_w] u8 R, G, B planes */
+} ytk_resize_page;        /* 32 bytes */
+/* recs: n host records (1..65535).  Invalid records (a page beyond pages_bytes, an output size below 1, an output
+ * outside out_bytes, two outputs that overlap, an unknown filter) are an error, not a launch.  scratch_dev holds at
+ * least ytk_resize_pages_scratch_bytes(recs, n, filter) bytes: the call allocates nothing.  Asynchronous on the stream:
+ * one H2D copy + one or two kernel launches (one when no page needs two passes). */
+int ytk_resize_pages_u8(const uint8_t* pages_dev, long long pages_bytes, const ytk_resize_page* recs, int n, int filter,
+                        uint8_t* scratch_dev, long long scratch_bytes, uint8_t* out_dev, long long out_bytes,
+                        void* cuda_stream);
+/* scratch bytes ytk_resize_pages_u8 needs (page extents are not checked here), -1 if a record or the filter is
+ * invalid */
+long long ytk_resize_pages_scratch_bytes(const ytk_resize_page* recs, int n, int filter);
+
 /* ---- Table semantic parser: the word-to-element assignment of reference TableSemanticParser.aggregate
  * (src/yomitoku/table_semantic_parser.py:683-701), every table and the paragraphs of every page in one launch. ---- */
 typedef struct {

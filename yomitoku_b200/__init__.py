@@ -16,6 +16,7 @@ Files in, documents out:
     from yomitoku_b200.export import export_markdown, export_html, export_csv, export_json
     result.to_markdown(path, img=page)                    # also to_html / to_csv (DocumentAnalyzerSchema)
     python -m yomitoku_b200 <file-or-dir> -f md -o out    # the command line (cli.py): batched analyze_pages
+    create_searchable_pdf(pages, results, "out.pdf")      # page images + invisible text layer (searchable_pdf.py)
 
 Fields out of forms (extractor.py): `extract(parser(page)[0], schema)` or `TableSemanticParser.extract_pages(pages,
 schema)` with a YAML `ExtractionSchema`, and `python -m yomitoku_b200.extract <dir> -s schema.yaml -o out` (extract.py).
@@ -27,6 +28,7 @@ from .extractor import ExtractionSchema, extract
 from .layout_analyzer import LayoutAnalyzer
 from .layout_parser import LayoutParser
 from .ocr import OCR
+from .searchable_pdf import create_searchable_pdf
 from .table_cell_detector import CellDetector
 from .table_semantic_parser import TableSemanticParser
 from .table_structure_recognizer import TableStructureRecognizer
@@ -35,4 +37,4 @@ from .text_recognizer import TextRecognizer
 
 __all__ = ["OCR", "TextDetector", "TextRecognizer", "DocumentAnalyzer", "LayoutAnalyzer", "LayoutParser",
            "TableStructureRecognizer", "CellDetector", "TableSemanticParser", "DevicePages", "device_pages",
-           "load_image", "ExtractionSchema", "extract"]
+           "load_image", "ExtractionSchema", "extract", "create_searchable_pdf"]

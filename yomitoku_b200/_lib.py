@@ -224,6 +224,11 @@ def _declare_rtdetr(lib):
                                               c_void_p]
     lib.ytk_op_resize_bilinear_scratch_bytes.restype = c_ll
     lib.ytk_op_resize_bilinear_scratch_bytes.argtypes = [c_void_p, c_int, c_int]
+    lib.ytk_resize_pages_u8.restype = c_int
+    lib.ytk_resize_pages_u8.argtypes = [c_void_p, c_ll, c_void_p, c_int, c_int, c_void_p, c_ll, c_void_p, c_ll,
+                                        c_void_p]
+    lib.ytk_resize_pages_scratch_bytes.restype = c_ll
+    lib.ytk_resize_pages_scratch_bytes.argtypes = [c_void_p, c_int, c_int]
     lib.ytk_rtdetr_create.restype = c_int
     lib.ytk_rtdetr_create.argtypes = [P(YtkTensor), c_int, c_int, c_int, c_int, P(c_void_p)]
     lib.ytk_rtdetr_destroy.restype = None

@@ -13,7 +13,8 @@ is done.  Each page's files are what the exporter writes for `analyzer(page)` on
 as a page image is logged and skipped.
 
 Not available here: the visualisations (-v), searchable-PDF output (-f pdf, --font_path, --pdf_quality) and PDF input
-(--dpi): there is no visualiser for the batched path, and no PDF writer or renderer among the dependencies.
+(--dpi): there is no visualiser for the batched path and no PDF renderer among the dependencies.  Searchable PDFs are
+written from Python with `create_searchable_pdf(pages, results, path, image_quality=...)` (searchable_pdf.py).
 """
 import argparse
 import os
@@ -77,8 +78,9 @@ def output_format(args):
     """The validated output format ("markdown" -> "md"); also checks --encoding and --batch."""
     fmt = args.format.lower()
     if fmt == "pdf":
-        raise ValueError("Searchable PDF output (-f pdf) is not available in this package: it has no PDF writer. "
-                         "Supported formats are %s" % SUPPORT_OUTPUT_FORMAT)
+        raise ValueError("Searchable PDF output (-f pdf) is not available on this command line: write it from Python "
+                         "with yomitoku_b200.create_searchable_pdf(pages, results, path). Supported formats are %s"
+                         % SUPPORT_OUTPUT_FORMAT)
     if fmt not in SUPPORT_OUTPUT_FORMAT:
         raise ValueError(f"Invalid output format: {args.format}. Supported formats are {SUPPORT_OUTPUT_FORMAT}")
     if args.encoding not in SUPPORT_ENCODING:

@@ -1683,9 +1683,11 @@ int ytk_rtdetr_forward_u8(ytk_rtdetr* h, const uint8_t* pages, int pages_on_devi
     }
     HandleCall call(h);
     cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
+    const int S = h->model.cfg.img;
+    // the engine input: [n][S][S][64] 16-bit operands, 128 bytes a pixel
+    const std::vector<ytk::ResampleSrc> rs = ytk::square_sources(reinterpret_cast<const ytk::RtSrc*>(srcs), n, S, 128);
     ytk::ResampleJob job;
-    if (ytk::resample_prepare(reinterpret_cast<const ytk::RtSrc*>(srcs), n, h->model.cfg.img, pages_bytes,
-                              "ytk_rtdetr_forward_u8", &job))
+    if (ytk::resample_prepare(rs.data(), n, ytk::kFilterBilinear, pages_bytes, "ytk_rtdetr_forward_u8", &job))
         return YTK_ERR;
     ytk::RtdetrEngine* e = h->engines.get(n, h->model, n);
     if (!e) return YTK_ERR;
@@ -1701,14 +1703,15 @@ int ytk_rtdetr_forward_u8(ytk_rtdetr* h, const uint8_t* pages, int pages_on_devi
         }
         src = h->pages.p;
     }
-    if (ytk::launch_resample(src, job, h->scratch.p, e->input, 1, st)) return YTK_ERR;
+    if (ytk::launch_resample(src, job, h->scratch.p, e->input, ytk::kOutEngine, st)) return YTK_ERR;
     return rt_finish(h, e, n, pred_logits, pred_boxes, out_on_device, st);
 }
 
 long long ytk_op_resize_bilinear_scratch_bytes(const ytk_rtdetr_src* srcs, int n, int size) {
+    const std::vector<ytk::ResampleSrc> rs = ytk::square_sources(reinterpret_cast<const ytk::RtSrc*>(srcs), n, size, 3);
     ytk::ResampleJob job;
-    if (ytk::resample_prepare(reinterpret_cast<const ytk::RtSrc*>(srcs), n, size, LLONG_MAX,
-                              "ytk_op_resize_bilinear_scratch_bytes", &job))
+    if (ytk::resample_prepare(rs.data(), n, ytk::kFilterBilinear, LLONG_MAX, "ytk_op_resize_bilinear_scratch_bytes",
+                              &job))
         return -1;
     return job.bytes;
 }
@@ -1720,9 +1723,9 @@ int ytk_op_resize_bilinear_u8(const uint8_t* pages_dev, long long pages_bytes, c
         ytk::set_error("ytk_op_resize_bilinear_u8: null argument");
         return YTK_ERR;
     }
+    const std::vector<ytk::ResampleSrc> rs = ytk::square_sources(reinterpret_cast<const ytk::RtSrc*>(srcs), n, size, 3);
     ytk::ResampleJob job;
-    if (ytk::resample_prepare(reinterpret_cast<const ytk::RtSrc*>(srcs), n, size, pages_bytes,
-                              "ytk_op_resize_bilinear_u8", &job))
+    if (ytk::resample_prepare(rs.data(), n, ytk::kFilterBilinear, pages_bytes, "ytk_op_resize_bilinear_u8", &job))
         return YTK_ERR;
     if (scratch_bytes < job.bytes) {
         ytk::set_error("ytk_op_resize_bilinear_u8: scratch_dev holds %lld bytes, need %lld", scratch_bytes, job.bytes);
@@ -1731,7 +1734,80 @@ int ytk_op_resize_bilinear_u8(const uint8_t* pages_dev, long long pages_bytes, c
     int device;
     if (!device_of(pages_dev, "ytk_op_resize_bilinear_u8", "pages_dev", &device)) return YTK_ERR;
     DevGuard dev_guard(device);
-    return ytk::launch_resample(pages_dev, job, scratch_dev, out_rgb_dev, 0, static_cast<cudaStream_t>(cuda_stream))
+    return ytk::launch_resample(pages_dev, job, scratch_dev, out_rgb_dev, ytk::kOutRGB,
+                                static_cast<cudaStream_t>(cuda_stream))
+               ? YTK_ERR
+               : YTK_OK;
+}
+
+static_assert(sizeof(ytk_resize_page) == 32, "ytk_resize_page is a 32-byte record");
+
+// The records of ytk_resize_pages_u8 as resample sources (the whole page each), with their output checks: an output of
+// 3 * out_w * out_h bytes inside out_bytes, no two outputs overlapping.
+static int resize_page_sources(const ytk_resize_page* recs, int n, long long out_bytes, const char* who,
+                               std::vector<ytk::ResampleSrc>* rs) {
+    if (!recs || n < 1 || n > 65535) {
+        ytk::set_error("%s: %d pages (1..65535)", who, n);
+        return 1;
+    }
+    rs->resize(n);
+    std::vector<std::pair<long long, long long>> spans(n);  // (out_off, bytes)
+    for (int i = 0; i < n; ++i) {
+        const ytk_resize_page& r = recs[i];
+        (*rs)[i] = ytk::ResampleSrc{ytk::RtSrc{r.page_off, r.H, r.W, 0, 0, r.W, r.H}, r.out_w, r.out_h, r.out_off};
+        if (r.out_w < 1 || r.out_h < 1) continue;  // resample_prepare names it
+        const long long bytes = 3LL * r.out_w * r.out_h;
+        if (r.out_off < 0 || r.out_off > out_bytes || bytes > out_bytes - r.out_off) {
+            ytk::set_error("%s: page %d: output of %lld bytes at %lld lies outside the %lld output bytes", who, i, bytes,
+                           r.out_off, out_bytes);
+            return 1;
+        }
+        spans[i] = {r.out_off, bytes};
+    }
+    std::vector<int> order(n);
+    for (int i = 0; i < n; ++i) order[i] = i;
+    std::sort(order.begin(), order.end(), [&](int a, int b) { return spans[a].first < spans[b].first; });
+    for (int k = 1; k < n; ++k) {
+        const int a = order[k - 1], b = order[k];
+        if (spans[a].second > 0 && spans[b].second > 0 && spans[a].first + spans[a].second > spans[b].first) {
+            ytk::set_error("%s: the outputs of pages %d and %d overlap", who, a, b);
+            return 1;
+        }
+    }
+    return 0;
+}
+
+long long ytk_resize_pages_scratch_bytes(const ytk_resize_page* recs, int n, int filter) {
+    std::vector<ytk::ResampleSrc> rs;
+    ytk::ResampleJob job;
+    if (resize_page_sources(recs, n, LLONG_MAX, "ytk_resize_pages_scratch_bytes", &rs) ||
+        ytk::resample_prepare(rs.data(), n, filter, LLONG_MAX, "ytk_resize_pages_scratch_bytes", &job))
+        return -1;
+    return job.bytes;
+}
+
+int ytk_resize_pages_u8(const uint8_t* pages_dev, long long pages_bytes, const ytk_resize_page* recs, int n, int filter,
+                        uint8_t* scratch_dev, long long scratch_bytes, uint8_t* out_dev, long long out_bytes,
+                        void* cuda_stream) {
+    static const char* who = "ytk_resize_pages_u8";
+    if (!pages_dev || !recs || !scratch_dev || !out_dev) {
+        ytk::set_error("%s: null argument", who);
+        return YTK_ERR;
+    }
+    std::vector<ytk::ResampleSrc> rs;
+    ytk::ResampleJob job;
+    if (resize_page_sources(recs, n, out_bytes, who, &rs) ||
+        ytk::resample_prepare(rs.data(), n, filter, pages_bytes, who, &job))
+        return YTK_ERR;
+    if (scratch_bytes < job.bytes) {
+        ytk::set_error("%s: scratch_dev holds %lld bytes, need %lld", who, scratch_bytes, job.bytes);
+        return YTK_ERR;
+    }
+    int device;
+    if (!device_of(pages_dev, who, "pages_dev", &device)) return YTK_ERR;
+    DevGuard dev_guard(device);
+    return ytk::launch_resample(pages_dev, job, scratch_dev, out_dev, ytk::kOutPlanar,
+                                static_cast<cudaStream_t>(cuda_stream))
                ? YTK_ERR
                : YTK_OK;
 }
